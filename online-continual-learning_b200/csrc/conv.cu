@@ -215,16 +215,7 @@ __device__ __forceinline__ void conv_epilogue(const ConvArgs& a, float (&acc)[PT
       S += s_fin[(g * BN + tid) * 2 + 0];
       Q += s_fin[(g * BN + tid) * 2 + 1];
     }
-    const double cnt = (double)a.M;
-    const double mean = S / cnt;
-    double var = Q / cnt - mean * mean;
-    if (var < 0.0) var = 0.0;
-    const int c = n0 + tid;
-    a.save_mean[c] = (float)mean;
-    a.save_invstd[c] = (float)(1.0 / sqrt(var + (double)a.eps));
-    const double unbiased = (a.M > 1) ? var * cnt / (cnt - 1.0) : var;
-    a.run_mean[c] = (1.f - a.momentum) * a.run_mean[c] + a.momentum * (float)mean;
-    a.run_var[c] = (1.f - a.momentum) * a.run_var[c] + a.momentum * (float)unbiased;
+    bn_finalize(a, n0 + tid, S, Q);
   }
 }
 
@@ -754,7 +745,7 @@ int launch_conv(const ConvArgs& a, cudaStream_t stream) {
   // 3x3 stride-1 convolutions on 8/16/32-wide maps: tensor cores fed from a halo patch (conv_tcp.cu);
   // other 3x3 stride-1 shapes with enough 128-pixel tiles: tensor cores with an im2col tile (conv_tc.cu).
   if (a.force_path == 3) {
-    if (!conv_tcp_eligible(a)) { set_error("launch_conv: shape not covered by the halo-patch tensor-core kernel"); return B200OCL_EUNSUPPORTED; }
+    if (!conv_tcp_eligible(a)) { set_error("launch_conv: launch not covered by the halo-patch tensor-core kernel (3x3 stride 1, no train mode)"); return B200OCL_EUNSUPPORTED; }
     return launch_conv_tcp(a, stream);
   }
   if (a.force_path == 2) {
@@ -762,7 +753,7 @@ int launch_conv(const ConvArgs& a, cudaStream_t stream) {
     return launch_conv_tc(a, stream);
   }
   if (a.force_path == 0) {
-    if (conv_tcp_eligible(a) && conv_tcp_mode_allowed(a)) return launch_conv_tcp(a, stream);   // precision policy: conv_tcp.cu
+    if (conv_tcp_eligible(a)) return launch_conv_tcp(a, stream);
     if (conv_tc_eligible(a)) return launch_conv_tc(a, stream);
   }
   // Forward convolutions and stride-1 data gradients with enough pixels go to the patch kernel:

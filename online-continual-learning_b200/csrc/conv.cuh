@@ -24,7 +24,7 @@ struct ConvArgs {
   int tc_kb, tc_bn;  // its K blocks and real channels per tile
   const float* w_tp; // halo-patch tensor-core image (conv_tcp.cu), nullable
   int tp_bn, tp_slices;
-  int tp_ps, tp_bs;  // set by the launcher: patch stages, weight ring depth
+  int tp_ps, tp_bs, tp_tiles;  // set by the launcher: patch stages, weight ring depth, 128-position tiles
   int force_path;    // 0 automatic; 1 CUDA-core kernels only; 2 conv_tc; 3 conv_tcp (selftest: fails if not eligible)
   int parity_order;  // stride-2 data gradient only: pixels enumerated [parity class][n][h/2][w/2] so that a CTA
                      //    sees one class and skips the taps that cannot reach it (9 of 36 tap-pixel pairs are live)
@@ -50,6 +50,26 @@ struct ConvArgs {
   float momentum;
 };
 
+// running = (1 - m) * running + m * s with one fixed rounding sequence (m * s rounded, then one fused multiply-add),
+// so that the train-mode epilogues and the deferred apply (net_fwd.cu) move a running statistic to the same bits.
+__device__ __forceinline__ float bn_running_update(float run, float s, float m) {
+  return __fmaf_rn(1.f - m, run, __fmul_rn(m, s));
+}
+
+// BatchNorm finalize of channel c from its fp64 batch sums S = sum x and Q = sum x^2 over a.M pixels: batch mean,
+// 1/sqrt(biased variance + eps), and the running mean / unbiased variance moved by a.momentum.
+__device__ __forceinline__ void bn_finalize(const ConvArgs& a, int c, double S, double Q) {
+  const double cnt = (double)a.M;
+  const double mean = S / cnt;
+  double var = Q / cnt - mean * mean;
+  if (var < 0.0) var = 0.0;
+  a.save_mean[c] = (float)mean;
+  a.save_invstd[c] = (float)(1.0 / sqrt(var + (double)a.eps));
+  const double unbiased = (a.M > 1) ? var * cnt / (cnt - 1.0) : var;
+  a.run_mean[c] = bn_running_update(a.run_mean[c], (float)mean, a.momentum);
+  a.run_var[c] = bn_running_update(a.run_var[c], (float)unbiased, a.momentum);
+}
+
 // Upper bound of gridDim.x over every tiling launch_conv may choose (sizes stat_part).
 int conv_max_grid_m(int M);
 int launch_conv(const ConvArgs& a, cudaStream_t stream);   // CK, CN multiples of 20
@@ -58,6 +78,5 @@ int launch_conv_tc(const ConvArgs& a, cudaStream_t stream);  // conv_tc.cu: wgmm
 bool conv_tc_eligible(const ConvArgs& a);
 int launch_conv_tcp(const ConvArgs& a, cudaStream_t stream);  // conv_tcp.cu: wgmma fed from a halo patch
 bool conv_tcp_eligible(const ConvArgs& a);
-bool conv_tcp_mode_allowed(const ConvArgs& a);   // launch kinds (eval / train / data gradient) the policy sends to conv_tcp
 
 }  // namespace b200ocl

@@ -17,8 +17,6 @@
 //      holds pixel row t for the epilogue.
 // Epilogues as in conv.cu: folded eval BN (+ReLU, +residual), raw store + deterministic fp64 batch
 // statistics for training, raw / accumulate for the flipped stride-1 data gradient.
-#include <stdlib.h>
-
 #include "conv.cuh"
 #include "umma.cuh"
 
@@ -259,16 +257,7 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(ConvArgs a) {
             S += s_fin[(g * bn + tid) * 2 + 0];
             Q += s_fin[(g * bn + tid) * 2 + 1];
           }
-          const double cnt = (double)a.M;
-          const double mean = S / cnt;
-          double var = Q / cnt - mean * mean;
-          if (var < 0.0) var = 0.0;
-          const int c = n0 + tid;
-          a.save_mean[c] = (float)mean;
-          a.save_invstd[c] = (float)(1.0 / sqrt(var + (double)a.eps));
-          const double unbiased = (a.M > 1) ? var * cnt / (cnt - 1.0) : var;
-          a.run_mean[c] = (1.f - a.momentum) * a.run_mean[c] + a.momentum * (float)mean;
-          a.run_var[c] = (1.f - a.momentum) * a.run_var[c] + a.momentum * (float)unbiased;
+          bn_finalize(a, n0 + tid, S, Q);
         }
       }
     }
@@ -295,12 +284,7 @@ int launch_tc(const ConvArgs& a, cudaStream_t stream) {
 }  // namespace
 
 bool conv_tc_eligible(const ConvArgs& a) {
-  static int enabled = -1;
-  if (enabled < 0) {
-    const char* e = getenv("B200OCL_TC");
-    enabled = (e && e[0] == '0') ? 0 : 1;
-  }
-  if (!enabled || !a.w_tc || a.ks != 3 || a.stride != 1 || a.transposed || a.CK % 20 != 0) return false;
+  if (!a.w_tc || a.ks != 3 || a.stride != 1 || a.transposed || a.CK % 20 != 0) return false;
   if (a.Hin != a.Hout || a.Win != a.Wout) return false;
   // enough 128-pixel tiles to occupy a good part of the machine; small problems stay on the fp32 kernels
   const long ctas = (long)((a.M + 127) / 128) * (a.CN / a.tc_bn);

@@ -25,14 +25,13 @@
 // sum in tap order (a long tensor-core accumulation truncates, see conv_tc.cu).  Roles:
 //   warps 0-7  two consumer warpgroups: warpgroup g issues the MMAs of tile rows 64g .. 64g+63 and promotes
 //              them; the fragments of a finished tile go through shared memory to warps 0-3, which run the
-//              epilogue with one pixel row per thread: folded eval BN / raw + batch statistics / accumulate
+//              epilogue with one pixel row per thread: folded eval BN (+ residual, ReLU) / raw / accumulate
 //   warp  8    weight loader (one elected lane): cp.async.bulk of pre-split, pre-swizzled [NT x 32] tiles,
 //              resident for the whole kernel when all 9 taps fit (cin <= 32), a ring otherwise
 //   warps 9-12 patch loaders: coalesced LDG.128 of NHWC pixels, cvt.rna.tf32 split, swizzled stores
-// CTAs are persistent over pixel tiles (one CTA per SM); batch statistics are accumulated per CTA in
-// fp64 in a fixed order and finalised by the last CTA (deterministic, as everywhere else).
-#include <stdlib.h>
-
+// CTAs are persistent over pixel tiles (one CTA per SM).  The kernel serves eval-mode forwards and
+// stride-1 data gradients; train-mode forwards, which need batch statistics, run on conv.cu or conv_tc.cu
+// (conv_tcp_eligible says why).
 #include "conv.cuh"
 #include "umma.cuh"
 
@@ -90,7 +89,6 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* patch0 = smem_raw;                                          // [PS][hi | lo][PROWS][128 B]
   __shared__ __align__(8) uint64_t pfull[TP_PS_MAX], pempty[TP_PS_MAX], bfull[9], bempty[TP_BS_MAX];
-  __shared__ bool is_last;
   __shared__ int s_fail;
   __shared__ float s_coef[3 * 80];   // eval BN: mean, scale, shift per channel of the tile
 
@@ -100,13 +98,12 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
   const int slices = a.tp_slices;
   const TileGeom G = tile_geom(a.N, a.Hin, a.Win);
   const int PS = a.tp_ps, BS = a.tp_bs;            // patch stages, weight ring depth (launcher fits them to smem)
-  const int taps_n = a.ks * a.ks;                  // 9, or 1 (1x1 convolution = the centre tap of the padded geometry)
-  const bool one_tap = taps_n == 1;
+  // the tile loops run to a.tp_tiles (= G.tiles_m): a kernel parameter is not a register live across them, which
+  // keeps conv_tcp_kernel<48> within 128 registers without spills
   float* sB = reinterpret_cast<float*>(smem_raw + (size_t)PS * 2 * G.pbytes);   // weight blocks
   const bool resident = (slices == 1 && NT == 32);   // all 9 weight blocks stay in shared memory
   const int b_slots = resident ? 9 : BS;
-  float* s_t = sB + (size_t)b_slots * B_BLOCK;  // [128][bn + 1] transpose scratch for the batch statistics
-  float* s_acc = s_t + 128 * (bn + 1);          // [128][NT + 1] finished tile, one pixel row per epilogue thread
+  float* s_acc = sB + (size_t)b_slots * B_BLOCK;   // [128][NT + 1] finished tile, one pixel row per epilogue thread
 
   if (tid == 0) {
     for (int i = 0; i < TP_PS_MAX; ++i) {
@@ -119,13 +116,13 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
     s_fail = 0;
   }
   __syncthreads();
-  const float* wimg = a.w_tp + (size_t)blockIdx.y * slices * taps_n * B_BLOCK;
+  const float* wimg = a.w_tp + (size_t)blockIdx.y * slices * 9 * B_BLOCK;
 
   if (warp >= TP_LOADER_WARP) {
     // =========================================================== patch loaders (128 threads)
     const int lt = tid - 32 * TP_LOADER_WARP;
     int pc = 0;
-    for (int tile = blockIdx.x; tile < G.tiles_m; tile += gridDim.x) {
+    for (int tile = blockIdx.x; tile < a.tp_tiles; tile += gridDim.x) {
       for (int sl = 0; sl < slices; ++sl, ++pc) {
         const int ch_valid = min(32, a.CK - sl * 32);       // real channels in this slice (multiple of 4)
         const int nch = 2 * ((ch_valid + 7) / 8);            // 16-byte chunks the MMAs will read per row
@@ -189,21 +186,21 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
     const uint32_t bytes = (uint32_t)(B_BLOCK * sizeof(float));
     if (resident) {
       if (umma::elect_one_sync()) {
-        for (int b = 0; b < taps_n; ++b) {
+        for (int b = 0; b < 9; ++b) {
           mbar_expect_tx(&bfull[b], bytes);
           bulk_g2s(sB + (size_t)b * B_BLOCK, wimg + (size_t)b * B_BLOCK, bytes, &bfull[b]);
         }
       }
     } else {
       int q = 0;
-      for (int tile = blockIdx.x; tile < G.tiles_m; tile += gridDim.x)
+      for (int tile = blockIdx.x; tile < a.tp_tiles; tile += gridDim.x)
         for (int sl = 0; sl < slices; ++sl)
-          for (int tap = 0; tap < taps_n; ++tap, ++q) {
+          for (int tap = 0; tap < 9; ++tap, ++q) {
             const int bs = q % BS;
             if (!umma::mbar_wait(&bempty[bs], (uint32_t)(((q / BS) & 1) ^ 1))) s_fail = 1;
             if (umma::elect_one_sync()) {
               mbar_expect_tx(&bfull[bs], bytes);
-              bulk_g2s(sB + (size_t)bs * B_BLOCK, wimg + (size_t)(sl * taps_n + tap) * B_BLOCK, bytes, &bfull[bs]);
+              bulk_g2s(sB + (size_t)bs * B_BLOCK, wimg + (size_t)(sl * 9 + tap) * B_BLOCK, bytes, &bfull[bs]);
             }
             __syncwarp();
           }
@@ -232,10 +229,9 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
       }
       esync();
     }
-    double statS = 0.0, statQ = 0.0;           // thread c < bn: running sums of channel c over this CTA's tiles
-    int pc = 0, q = 0;                         // (tile, slice) pairs; position in the weight stream
+    int pc = 0, q = 0;                       // (tile, slice) pairs; position in the weight stream
     bool b_ready = false;
-    for (int tile = blockIdx.x; tile < G.tiles_m; tile += gridDim.x) {
+    for (int tile = blockIdx.x; tile < a.tp_tiles; tile += gridDim.x) {
       float accf[R];
 #pragma unroll
       for (int i = 0; i < R; ++i) accf[i] = 0.f;
@@ -245,8 +241,8 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
         if (!umma::mbar_wait(&pfull[ps], (uint32_t)((pc / PS) & 1))) s_fail = 1;
         const uint64_t dAs = dA0 + (uint64_t)(ps * A_STAGE);
 #pragma unroll 1
-        for (int tap = 0; tap < taps_n; ++tap, ++q) {
-          const int kh = one_tap ? 1 : tap / 3, kw = one_tap ? 1 : tap - 3 * (tap / 3);
+        for (int tap = 0; tap < 9; ++tap, ++q) {
+          const int kh = tap / 3, kw = tap - 3 * kh;
           const int b = resident ? tap : q % BS;
           if (!(resident && b_ready))
             if (!umma::mbar_wait(&bfull[b], resident ? 0u : (uint32_t)((q / BS) & 1))) s_fail = 1;
@@ -277,9 +273,8 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
       const int sp = tile * 128 + et;                    // strip position of this MMA row
       const int img = sp / G.pp, rem = sp - img * G.pp;
       const int y = rem / G.wp, x = rem - y * G.wp;
-      // halo positions and (stride 2) odd positions are by-products
-      const bool valid = img < a.N && y < a.Hin && x < a.Win && (a.stride == 1 || ((y | x) & 1) == 0);
-      const size_t m = ((size_t)img * a.Hout + (a.stride == 1 ? y : y >> 1)) * a.Wout + (a.stride == 1 ? x : x >> 1);
+      const bool valid = img < a.N && y < a.Hin && x < a.Win;   // halo positions are by-products
+      const size_t m = ((size_t)img * a.Hin + y) * a.Win + x;   // stride 1: output pixel = input pixel
       // pre[] = the residual (eval) or the gradient being accumulated into (data gradient), 0 otherwise; the
       // loads are issued before the tile's row is read back from s_acc.
       float acc[NT], pre[NT];
@@ -319,107 +314,14 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
             *reinterpret_cast<float4*>(o + c0) = make_float4(rr[0], rr[1], rr[2], rr[3]);
           }
         }
-      } else {
-        if (valid) {
-          float* o = a.out + m * a.CN + n0;
+      } else if (valid) {
+        float* o = a.out + m * a.CN + n0;
 #pragma unroll
-          for (int c0 = 0; c0 < NT; c0 += 4) {
-            if (c0 >= bn) break;
-            // raw / train: pre == 0; accumulate: pre = previous contents
-            *reinterpret_cast<float4*>(o + c0) = make_float4(acc[c0] + pre[c0], acc[c0 + 1] + pre[c0 + 1],
-                                                             acc[c0 + 2] + pre[c0 + 2], acc[c0 + 3] + pre[c0 + 3]);
-          }
-        }
-        if (a.mode == CONV_TRAIN) {
-          // transpose through shared memory; the 128 rows of a channel are summed in fp64 by 128 / bn threads
-          // (contiguous row ranges, combined in range order: the association is fixed)
-#pragma unroll
-          for (int c = 0; c < NT; ++c)
-            if (c < bn) s_t[et * (bn + 1) + c] = valid ? acc[c] : 0.f;   // by-product rows do not count
-          esync();
-          const int parts = 128 / bn;                      // 6 (bn = 20) or 3 (bn = 40)
-          const int rows_pp = (128 + parts - 1) / parts;
-          const int ch = et % bn, part = et / bn;
-          double S = 0.0, Q = 0.0;
-          if (part < parts) {
-            const int r1 = min(128, (part + 1) * rows_pp);
-            for (int rr = part * rows_pp; rr < r1; ++rr) {
-              const double xv = (double)s_t[rr * (bn + 1) + ch];
-              S += xv;
-              Q += xv * xv;
-            }
-          }
-          esync();                                         // s_t fully read
-          double* s_p = reinterpret_cast<double*>(s_t);    // [parts][bn][2] (<= 1920 B)
-          if (part < parts) {
-            s_p[(part * bn + ch) * 2 + 0] = S;
-            s_p[(part * bn + ch) * 2 + 1] = Q;
-          }
-          esync();
-          if (et < bn) {
-            double Ss = 0.0, Qs = 0.0;
-            for (int pp = 0; pp < parts; ++pp) {
-              Ss += s_p[(pp * bn + et) * 2 + 0];
-              Qs += s_p[(pp * bn + et) * 2 + 1];
-            }
-            statS += Ss;
-            statQ += Qs;
-          }
-          esync();
-        }
-      }
-    }
-    if (epi && a.mode == CONV_TRAIN) {
-      if (et < bn) {
-        double* dst = a.stat_part + ((size_t)blockIdx.x * a.CN + n0 + et) * 2;
-        dst[0] = statS;
-        dst[1] = statQ;
-      }
-      __threadfence();
-      esync();
-      if (et == 0) is_last = (atomicAdd(a.counter + blockIdx.y, 1u) == gridDim.x - 1);
-      esync();
-      if (is_last) {
-        __threadfence();
-        const int groups = 128 / bn;
-        const int ch = et % bn, grp = et / bn;
-        double* s_fin = reinterpret_cast<double*>(s_t);   // [groups][bn][2]
-        if (grp < groups) {
-          double S = 0.0, Q = 0.0;
-          unsigned int b = grp;
-          for (; b + 3 * groups < gridDim.x; b += 4 * groups) {
-            double2 pv[4];
-#pragma unroll
-            for (int u = 0; u < 4; ++u)
-              pv[u] = __ldcg(reinterpret_cast<const double2*>(a.stat_part + ((size_t)(b + u * groups) * a.CN + n0 + ch) * 2));
-            S += (pv[0].x + pv[1].x) + (pv[2].x + pv[3].x);
-            Q += (pv[0].y + pv[1].y) + (pv[2].y + pv[3].y);
-          }
-          for (; b < gridDim.x; b += groups) {
-            const double2 pv = __ldcg(reinterpret_cast<const double2*>(a.stat_part + ((size_t)b * a.CN + n0 + ch) * 2));
-            S += pv.x;
-            Q += pv.y;
-          }
-          s_fin[(grp * bn + ch) * 2 + 0] = S;
-          s_fin[(grp * bn + ch) * 2 + 1] = Q;
-        }
-        esync();
-        if (et < bn) {
-          double Sm = 0.0, Q = 0.0;
-          for (int gq = 0; gq < groups; ++gq) {
-            Sm += s_fin[(gq * bn + et) * 2 + 0];
-            Q += s_fin[(gq * bn + et) * 2 + 1];
-          }
-          const double cnt = (double)a.M;
-          const double mean = Sm / cnt;
-          double var = Q / cnt - mean * mean;
-          if (var < 0.0) var = 0.0;
-          const int c = n0 + et;
-          a.save_mean[c] = (float)mean;
-          a.save_invstd[c] = (float)(1.0 / sqrt(var + (double)a.eps));
-          const double unbiased = (a.M > 1) ? var * cnt / (cnt - 1.0) : var;
-          a.run_mean[c] = (1.f - a.momentum) * a.run_mean[c] + a.momentum * (float)mean;
-          a.run_var[c] = (1.f - a.momentum) * a.run_var[c] + a.momentum * (float)unbiased;
+        for (int c0 = 0; c0 < NT; c0 += 4) {
+          if (c0 >= bn) break;
+          // raw: pre == 0; accumulate: pre = previous contents
+          *reinterpret_cast<float4*>(o + c0) = make_float4(acc[c0] + pre[c0], acc[c0 + 1] + pre[c0 + 1],
+                                                           acc[c0 + 2] + pre[c0 + 2], acc[c0 + 3] + pre[c0 + 3]);
         }
       }
     }
@@ -430,28 +332,32 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
 }
 
 template <int NT>
-size_t tcp_smem_bytes(const TileGeom& G, int bn, int slices, int ps, int bs) {
+size_t tcp_smem_bytes(const TileGeom& G, int slices, int ps, int bs) {
   const int b_slots = (slices == 1 && NT == 32) ? 9 : bs;
   return (size_t)ps * 2 * G.pbytes + (size_t)b_slots * 2 * NT * 32 * sizeof(float) +
-         (size_t)128 * (bn + 1) * sizeof(float) + (size_t)128 * (NT + 1) * sizeof(float) + 1024;
+         (size_t)128 * (NT + 1) * sizeof(float) + 1024;
 }
 
 template <int NT>
 int launch_tcp(ConvArgs a, cudaStream_t stream) {
-  const TileGeom G0 = tile_geom(a.N, a.Hin, a.Win);
-  // deepest pipeline that fits: 3 patch stages + 6 weight slots, 3 + 4, else 2 + 6
-  const size_t limit = 227 * 1024 - 4096;     // static shared memory (barriers, coefficients) comes on top
+  const TileGeom G = tile_geom(a.N, a.Hin, a.Win);
+  // Deepest pipeline that fits: 3 patch stages + 6 weight slots, 3 + 4, else 2 + 6.  The fit still sets aside the
+  // [128][bn + 1] float scratch of the batch-statistics epilogue this kernel used to have (the smem it allocates does
+  // not include it), so every shape keeps the depth it was measured with; handing that room to deeper pipelines is a
+  // performance change of its own.
+  const size_t limit = 227 * 1024 - 4096      // static shared memory (barriers, coefficients) comes on top
+                       - (size_t)128 * (a.tp_bn + 1) * sizeof(float);
   a.tp_ps = 3; a.tp_bs = 6;
-  if (tcp_smem_bytes<NT>(G0, a.tp_bn, a.tp_slices, a.tp_ps, a.tp_bs) > limit) a.tp_bs = 4;
-  if (tcp_smem_bytes<NT>(G0, a.tp_bn, a.tp_slices, a.tp_ps, a.tp_bs) > limit) { a.tp_ps = 2; a.tp_bs = 6; }
-  const size_t smem = tcp_smem_bytes<NT>(G0, a.tp_bn, a.tp_slices, a.tp_ps, a.tp_bs);
+  if (tcp_smem_bytes<NT>(G, a.tp_slices, a.tp_ps, a.tp_bs) > limit) a.tp_bs = 4;
+  if (tcp_smem_bytes<NT>(G, a.tp_slices, a.tp_ps, a.tp_bs) > limit) { a.tp_ps = 2; a.tp_bs = 6; }
+  const size_t smem = tcp_smem_bytes<NT>(G, a.tp_slices, a.tp_ps, a.tp_bs);
   static size_t configured_dev[B200OCL_MAX_DEVICES] = {};
   size_t& configured = configured_dev[b200ocl::device_slot()];
   if (smem > configured) {
     B200OCL_CUDA(cudaFuncSetAttribute(conv_tcp_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = smem;
   }
-  const TileGeom G = tile_geom(a.N, a.Hin, a.Win);
+  a.tp_tiles = G.tiles_m;
   const int n_tiles = a.CN / a.tp_bn;
   int gx = sm_count() / n_tiles;
   if (gx < 1) gx = 1;
@@ -459,7 +365,7 @@ int launch_tcp(ConvArgs a, cudaStream_t stream) {
   // even out the tiles per CTA (e.g. 880 tiles on 132 CTAs = 7 rounds -> 126 CTAs of 7, one of 2)
   const int rounds = (G.tiles_m + gx - 1) / gx;
   gx = (G.tiles_m + rounds - 1) / rounds;
-  // one kernel, three epilogues (eval / train / data gradient): profiled as one class
+  // one kernel, two epilogues (eval / data gradient): profiled as one class
   B200OCL_PROF("conv_tcp",
                2.0 * a.M * (double)a.CN * a.CK * 9.0, stream);
   conv_tcp_kernel<NT><<<dim3(gx, n_tiles), TP_THREADS, smem, stream>>>(a);
@@ -469,34 +375,15 @@ int launch_tcp(ConvArgs a, cudaStream_t stream) {
 
 }  // namespace
 
-bool conv_tcp_mode_allowed(const ConvArgs& a) {
-  // Which launch kinds take the tensor-core path: bit 0 eval features, bit 1 train-mode forward, bit 2 data gradient
-  // (B200OCL_TCP_MODES).  Default 5 = eval + data gradient: the train-mode forward stays on the fp32 kernels, because
-  // the truncating tensor-core accumulate leaves a small sign-dependent bias that a train-mode forward differentiates
-  // through BatchNorm, while eval features and data gradients keep to the fp32 bar of the drop-in comparison
-  // (tests/test_gpu_dropin.py runs this default policy).
-  static int modes = -1;
-  if (modes < 0) {
-    const char* m = getenv("B200OCL_TCP_MODES");
-    modes = (m && m[0] >= '0' && m[0] <= '7') ? (m[0] - '0') : 5;
-  }
-  const int bit = a.mode == CONV_EVAL ? 1 : (a.mode == CONV_TRAIN ? 2 : 4);
-  return (modes & bit) != 0;
-}
-
 bool conv_tcp_eligible(const ConvArgs& a) {
-  // read per call (a getenv is negligible next to a launch) so that tools can switch paths in-process
-  const char* e = getenv("B200OCL_TCP");
-  const char* e2 = getenv("B200OCL_TC");
-  const bool enabled = !((e && e[0] == '0') || (e2 && e2[0] == '0'));
-  if (!enabled || !a.w_tp || a.transposed || a.CK % 4 != 0) return false;
-  if (!((a.ks == 3 && a.pad == 1) || (a.ks == 1 && a.pad == 0))) return false;
-  if (a.stride != 1 && (a.stride != 2 || a.flip)) return false;          // stride 2: forward only
-  if (a.Hout != (a.Hin + 2 * a.pad - a.ks) / a.stride + 1 || a.Wout != (a.Win + 2 * a.pad - a.ks) / a.stride + 1) return false;
+  // Precision policy: no train-mode forwards.  The truncating tensor-core accumulate leaves a small sign-dependent
+  // bias that a train-mode forward differentiates through BatchNorm, while eval features and data gradients keep to
+  // the fp32 bar of the drop-in comparison (tests/test_gpu_dropin.py).
+  if (a.mode == CONV_TRAIN || !a.w_tp || a.transposed || a.CK % 4 != 0) return false;
+  if (a.ks != 3 || a.pad != 1 || a.stride != 1 || a.Hout != a.Hin || a.Wout != a.Win) return false;
   if (128 + 2 * (a.Win + 2) + 2 > 16 * TP_LD_MAX) return false;   // strip rows one stage holds (W <= 37)
   if ((long)a.N * (a.Hin + 2) * (a.Win + 2) > 2000000000L) return false;
   if (a.tp_bn <= 0 || a.tp_bn > 40 || a.CN % a.tp_bn != 0) return false;
-  // stat_part holds one row per persistent CTA; sized for conv_max_grid_m(M) >= tiles
   return true;
 }
 

@@ -12,6 +12,7 @@
 // in fixed order by one finalize kernel for all layers (deterministic; no float atomics).
 #include <float.h>
 #include <math.h>
+#include <stdlib.h>
 
 #include "net_ws.cuh"
 
@@ -328,11 +329,6 @@ __global__ void __launch_bounds__(256, 1) bn_bwd_fused_kernel(BnBwdArgs a) {
 int launch_bn_bwd(BnBwdArgs a, cudaStream_t stream) {
   {
     // fused path: rows split evenly over at most one CTA per SM, all of a CTA's rows resident in shared memory
-    static int use_fused = -1;
-    if (use_fused < 0) {
-      const char* e = getenv("B200OCL_BN_FUSED");
-      use_fused = (e && e[0] == '0') ? 0 : 1;
-    }
     const int cols = a.C / 4;
     const int R = 256 / cols;
     const int sms = sm_count();
@@ -343,7 +339,7 @@ int launch_bn_bwd(BnBwdArgs a, cudaStream_t stream) {
     const int groups = 256 / a.C > 0 ? 256 / a.C : 1;
     const int srows = R > groups ? R : groups;
     const size_t smem = (size_t)srows * a.C * 2 * sizeof(double) + (size_t)rows * a.C * 2 * sizeof(float);
-    if (use_fused && a.ready && grid <= sms && smem <= 200 * 1024 &&
+    if (a.ready && grid <= sms && smem <= 200 * 1024 &&
         (size_t)grid * a.C * 2 * sizeof(double) <= (size_t)bn_bwd_part_capacity(a.M, a.C, sms)) {
       static bool configured_dev[B200OCL_MAX_DEVICES] = {};
       bool& configured = configured_dev[device_slot()];
@@ -895,7 +891,7 @@ extern "C" int b200ocl_net_backward(const b200ocl_net_desc* desc, const b200ocl_
     {
       // 3x3 stride-1 layers on 4..32-wide maps: wgmma with the activation read in place from a strip (wgrad_tc.cu)
       const WgradTcCfg tg = wgrad_tc_cfg(N, c.hin, c.win, c.ks, c.stride, c.pad, c.cin, c.cout, sms);
-      if (tg.eligible && wgrad_tc_enabled()) {
+      if (tg.eligible) {
         WgradTcArgs ta{};
         ta.x = x; ta.dz = dz;
         ta.part = w.wg_part + w.wg_off[ci];
@@ -1042,7 +1038,7 @@ extern "C" int b200ocl_net_backward(const b200ocl_net_desc* desc, const b200ocl_
       e.cout = p.conv[i].cout;
       e.taps = p.conv[i].ks * p.conv[i].ks;
       e.splits = (i == 0) ? grid : wgrad_cfg(p.conv[i], N, sms).splits;
-      if (i > 0 && wgrad_tc_enabled()) {
+      if (i > 0) {
         const ConvL& ci_ = p.conv[i];
         const WgradTcCfg tg = wgrad_tc_cfg(N, ci_.hin, ci_.win, ci_.ks, ci_.stride, ci_.pad, ci_.cin, ci_.cout, sms);
         if (tg.eligible) e.splits = tg.chains;

@@ -92,7 +92,7 @@ struct TpPackTable {
   int n;
   struct {
     unsigned int w_off, img_off;
-    int cin, cout, bn, nt, slices, dgrad, taps;
+    int cin, cout, bn, nt, slices, dgrad;
   } e[2 * NET_MAX_CONV];
 };
 
@@ -102,31 +102,31 @@ __global__ void __launch_bounds__(256) tp_pack_kernel(TpPackTable t, const float
   const int n_ch = L.dgrad ? L.cin : L.cout;
   const int k_ch = L.dgrad ? L.cout : L.cin;
   const int n_tiles = n_ch / L.bn;
-  const int total = n_tiles * L.slices * L.taps * L.nt * 8;   // (tile, slice, tap, row, 16-byte chunk)
+  const int total = n_tiles * L.slices * 9 * L.nt * 8;   // (tile, slice, tap, row, 16-byte chunk)
   for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < total; e += gridDim.x * blockDim.x) {
     const int c = e & 7;
     int r = e >> 3;
     const int row = r % L.nt;
     r /= L.nt;
-    const int tap = r % L.taps;
-    r /= L.taps;
+    const int tap = r % 9;
+    r /= 9;
     const int sl = r % L.slices, tile = r / L.slices;
     float v[4] = {0.f, 0.f, 0.f, 0.f};
     const int k0 = sl * 32 + c * 4;
     if (row < L.bn && k0 < k_ch) {
       const int nch = tile * L.bn + row;
-      const int wt = L.dgrad ? L.taps - 1 - tap : tap;
+      const int wt = L.dgrad ? 8 - tap : tap;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         const int co = L.dgrad ? k0 + j : nch;
         const int ci = L.dgrad ? nch : k0 + j;
-        v[j] = params[L.w_off + ((size_t)co * L.cin + ci) * L.taps + wt];
+        v[j] = params[L.w_off + ((size_t)co * L.cin + ci) * 9 + wt];
       }
     }
     float4 h, l;
     umma::split_tf32(v[0], h.x, l.x); umma::split_tf32(v[1], h.y, l.y);
     umma::split_tf32(v[2], h.z, l.z); umma::split_tf32(v[3], h.w, l.w);
-    float* base = packed + L.img_off + ((size_t)((tile * L.slices + sl) * L.taps + tap) * 2) * L.nt * 32;
+    float* base = packed + L.img_off + ((size_t)((tile * L.slices + sl) * 9 + tap) * 2) * L.nt * 32;
     const int off = umma::sw128_offset_f32(row, c);
     *reinterpret_cast<float4*>(base + off) = h;
     *reinterpret_cast<float4*>(base + L.nt * 32 + off) = l;
@@ -180,7 +180,6 @@ int launch_pack(const NetPlan& p, const float* params, float* packed, cudaStream
       e.nt = tc_nt(e.bn);
       e.slices = d ? c.tp_sl_d : c.tp_sl_f;
       e.dgrad = d;
-      e.taps = c.ks * c.ks;
     }
   }
   if (tp.n) {
@@ -434,39 +433,6 @@ int conv_eval(const NetPlan& p, const b200ocl_net_state& st, int ci, int N, cons
 }
 
 
-// Diagnostic (B200OCL_RESTAT=1): recompute a layer's batch mean / invstd from the STORED raw output, two passes in
-// fp64, one CTA per channel -- isolates "the statistics of the producing kernel" from "the values it stored".
-__global__ void __launch_bounds__(256) bn_restat_kernel(const float* __restrict__ z, int M, int C, float eps,
-                                                        float* __restrict__ mean_out, float* __restrict__ invstd_out) {
-  __shared__ double s_a[256];
-  const int c = blockIdx.x, tid = threadIdx.x;
-  double s = 0.0;
-  for (int m = tid; m < M; m += 256) s += (double)z[(size_t)m * C + c];
-  s_a[tid] = s;
-  __syncthreads();
-  for (int o = 128; o > 0; o >>= 1) {
-    if (tid < o) s_a[tid] += s_a[tid + o];
-    __syncthreads();
-  }
-  const double mean = s_a[0] / (double)M;
-  __syncthreads();
-  double q = 0.0;
-  for (int m = tid; m < M; m += 256) {
-    const double dlt = (double)z[(size_t)m * C + c] - mean;
-    q += dlt * dlt;
-  }
-  s_a[tid] = q;
-  __syncthreads();
-  for (int o = 128; o > 0; o >>= 1) {
-    if (tid < o) s_a[tid] += s_a[tid + o];
-    __syncthreads();
-  }
-  if (tid == 0) {
-    mean_out[c] = (float)mean;
-    invstd_out[c] = (float)(1.0 / sqrt(s_a[0] / (double)M + (double)eps));
-  }
-}
-
 // Eval-statistics forward (GSS-greedy differentiates the network in eval mode, gss_greedy_update.py:16): the
 // "saved" statistics that bn_apply and the backward use are the RUNNING ones; the batch statistics the train-mode
 // convolution computes go to a throw-away buffer and the running statistics are left alone.
@@ -511,15 +477,6 @@ int conv_train(const NetPlan& p, const b200ocl_net_state& st, const TrainWs& w, 
   if (rc == 0 && eval_stats) {
     bn_save_running_kernel<<<(b.c + 127) / 128, 128, 0, stream>>>(st.bn_stats + b.stat_off, st.bn_stats + b.stat_off + b.c, a.eps,
                                                                    b.c, a.save_mean, a.save_invstd);
-    B200OCL_LAUNCHED();
-  }
-  static int restat = -1;
-  if (restat < 0) {
-    const char* e = getenv("B200OCL_RESTAT");
-    restat = (e && e[0] == '1') ? 1 : 0;
-  }
-  if (rc == 0 && restat) {
-    bn_restat_kernel<<<c.cout, 256, 0, stream>>>(a.out, N * c.hout * c.wout, c.cout, a.eps, a.save_mean, a.save_invstd);
     B200OCL_LAUNCHED();
   }
   return rc;
@@ -577,12 +534,12 @@ int head_forward(const NetPlan& p, const b200ocl_net_state& st, const float* fea
   return B200OCL_OK;
 }
 
-// running = (1 - momentum) * running + momentum * s for every BN statistic (the expression the convolution epilogues
-// use), plus num_batches_tracked += 1: one deferred train-mode pass applied to the running statistics
+// running = (1 - momentum) * running + momentum * s for every BN statistic (bn_running_update, as in the convolution
+// epilogues), plus num_batches_tracked += 1: one deferred train-mode pass applied to the running statistics
 __global__ void bn_running_apply_kernel(float* __restrict__ run, const float* __restrict__ s, int n, float momentum,
                                         long long* __restrict__ tracked, int n_bn) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) run[i] = (1.f - momentum) * run[i] + momentum * s[i];
+  if (i < n) run[i] = bn_running_update(run[i], s[i], momentum);
   if (tracked && i < n_bn) tracked[i] += 1;
 }
 
@@ -667,7 +624,7 @@ static void selftest_layer(b200ocl::ConvL& c, int cin, int cout, int H, int W, i
   c.wout = b200ocl::conv_out(W, ks, stride, c.pad);
   c.w_off = 0;
   pk = 0;
-  b200ocl::conv_pack_layout(c, pk, true);
+  b200ocl::conv_pack_layout(c, pk);
 }
 
 size_t b200ocl_conv_selftest_workspace_bytes(int N, int cin, int cout, int H, int W, int ks, int stride) {

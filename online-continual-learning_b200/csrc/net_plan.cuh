@@ -77,7 +77,7 @@ struct NetPlan {
 inline int conv_out(int x, int ks, int stride, int pad) { return (x + 2 * pad - ks) / stride + 1; }
 
 // Packed-arena layout of one convolution (kernel-side weight copies); c.cin/cout/ks/stride/hin/win set.
-inline void conv_pack_layout(ConvL& c, size_t& pk, bool tp_all = false) {
+inline void conv_pack_layout(ConvL& c, size_t& pk) {
   const int cin = c.cin, cout = c.cout, ks = c.ks, stride = c.stride, hin = c.hin, win = c.win;
   c.pkf_off = pk; pk += (size_t)cout * cin * ks * ks;
   c.pkd_off = pk; pk += (size_t)cout * cin * ks * ks;
@@ -90,20 +90,14 @@ inline void conv_pack_layout(ConvL& c, size_t& pk, bool tp_all = false) {
     c.tc_f_off = pk; pk += (size_t)(cout / c.tc_bn_f) * c.tc_kb_f * 2 * tc_nt(c.tc_bn_f) * 32;
     c.tc_d_off = pk; pk += (size_t)(cin / c.tc_bn_d) * c.tc_kb_d * 2 * tc_nt(c.tc_bn_d) * 32;
   }
-  // conv_tcp.cu: images for the 3x3 stride-1 convolutions on maps with W <= 37 (forward + data gradient).  The
-  // kernel also runs 3x3 stride-2 and 1x1 convolutions (it computes them at input resolution and keeps every
-  // other row / column), but it wastes three of four computed positions there, so the network plan only asks for those images in the kernel selftest (tp_all).
-  if (cin % 20 == 0 && win <= 37 && ((ks == 3 && c.pad == 1) || (ks == 1 && c.pad == 0)) &&
-      (tp_all || (ks == 3 && stride == 1))) {
-    const int taps = ks * ks;
+  // conv_tcp.cu: images for the 3x3 stride-1 convolutions on maps with W <= 37 (forward + data gradient)
+  if (ks == 3 && stride == 1 && c.pad == 1 && cin % 20 == 0 && win <= 37) {
     c.tp_bn_f = cout < 40 ? cout : 40;
     c.tp_sl_f = (cin + 31) / 32;
-    c.tp_f_off = pk; pk += (size_t)(cout / c.tp_bn_f) * c.tp_sl_f * taps * 2 * tc_nt(c.tp_bn_f) * 32;
-    if (ks == 3 && stride == 1) {
-      c.tp_bn_d = cin < 40 ? cin : 40;
-      c.tp_sl_d = (cout + 31) / 32;
-      c.tp_d_off = pk; pk += (size_t)(cin / c.tp_bn_d) * c.tp_sl_d * 9 * 2 * tc_nt(c.tp_bn_d) * 32;
-    }
+    c.tp_f_off = pk; pk += (size_t)(cout / c.tp_bn_f) * c.tp_sl_f * 9 * 2 * tc_nt(c.tp_bn_f) * 32;
+    c.tp_bn_d = cin < 40 ? cin : 40;
+    c.tp_sl_d = (cout + 31) / 32;
+    c.tp_d_off = pk; pk += (size_t)(cin / c.tp_bn_d) * c.tp_sl_d * 9 * 2 * tc_nt(c.tp_bn_d) * 32;
   }
 }
 

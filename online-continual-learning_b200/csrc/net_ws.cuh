@@ -1,7 +1,6 @@
 // net_ws.cuh -- carving of the caller-provided workspaces of the ResNet engine.
 #pragma once
 #include "wgrad_tc.cuh"
-#include <stdlib.h>
 #include "conv.cuh"
 #include "net_plan.cuh"
 
@@ -49,11 +48,7 @@ inline WgradCfg wgrad_cfg(const ConvL& c, int N, int sms) {
   // >= 16 resident warps per SM overall, at least 64 pixels of reduction per CTA (fewer, larger splits
   // measured slower: the kernel needs the parallelism more than the finalize pass needs fewer partials)
   const int warps_per_cta = g.kw * g.nw;
-  static int target = 0;   // resident warps per SM the split count aims for (B200OCL_WG_WARPS, default 8)
-  if (!target) {
-    const char* e = getenv("B200OCL_WG_WARPS");
-    target = (e && atoi(e) > 0) ? atoi(e) : 8;
-  }
+  constexpr int target = 8;   // resident warps per SM the split count aims for
   int splits = (target * sms + warps_per_cta * g.grid_k * g.grid_n - 1) / (warps_per_cta * g.grid_k * g.grid_n);
   const int max_by_pixels = (M + 63) / 64;
   if (splits > max_by_pixels) splits = max_by_pixels;
@@ -66,11 +61,7 @@ inline WgradCfg wgrad_cfg(const ConvL& c, int N, int sms) {
 // Grid of the BN-backward reduction over M pixels x C channels (shared by sizing and launch).
 inline int bn_bwd_rows_per_cta(int M, int C, int sms) {
   const int R = 256 / (C / 4);
-  static int per_sm = 0;   // CTAs per SM the row split aims for (B200OCL_BN_CTAS, default 2)
-  if (!per_sm) {
-    const char* e = getenv("B200OCL_BN_CTAS");
-    per_sm = (e && atoi(e) > 0) ? atoi(e) : 2;
-  }
+  constexpr int per_sm = 2;   // CTAs per SM the row split aims for
   int rows = (M + per_sm * sms - 1) / (per_sm * sms);
   if (rows < 4 * R) rows = 4 * R;
   return (rows + R - 1) / R * R;

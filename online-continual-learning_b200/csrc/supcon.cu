@@ -23,7 +23,6 @@
 //                 using l_ji = l_ij (anchor set == contrast set in 'all' mode, loss.py:60-62).
 // Anchors are in view-major order a = v*B + b (loss.py:56); features/grad are [B,V,d].
 #include <float.h>
-#include <stdlib.h>
 #include <math.h>
 
 #include "common.cuh"
@@ -279,8 +278,8 @@ __device__ __forceinline__ void logit_tile(const float* __restrict__ sA, const f
 // RES: the whole contrast set (all n_tiles x TN rows) is resident in shared memory, staged once with one
 // mbarrier -- the shape of the replay path itself (A = 220 anchors, d = 128: 113 KB).  Otherwise rows stream
 // through a two-slot ring, tile t+1 in flight while tile t is consumed.
-template <int RM, int RN, int NC, bool RES, int MINB>
-__global__ void __launch_bounds__(SC_THREADS, MINB) supcon_fused_kernel(SupconParams p) {
+template <int RM, int RN, int NC, bool RES>
+__global__ void __launch_bounds__(SC_THREADS, 1) supcon_fused_kernel(SupconParams p) {
   constexpr int TM = 16 * RM, TN = 16 * RN, WP = TM + 4;
   extern __shared__ __align__(128) unsigned char raw[];
   const int P = p.d + 4;
@@ -508,11 +507,6 @@ __global__ void __launch_bounds__(SC_THREADS, MINB) supcon_fused_kernel(SupconPa
   }
 }
 
-inline bool env_flag(const char* name) {
-  const char* e = getenv(name);
-  return e && e[0] == '1';
-}
-
 template <int RM, int RN, int NC, bool RES>
 size_t fused_smem_bytes(int A, int d) {
   constexpr int TM = 16 * RM, TN = 16 * RN, WP = TM + 4;
@@ -521,40 +515,39 @@ size_t fused_smem_bytes(int A, int d) {
   return 128 + (size_t)(TM + b_rows) * P * 4 + (size_t)TN * WP * 4 + (size_t)b_rows * 16 + (size_t)TM * 4;
 }
 
-template <int RM, int RN, int NC, bool RES, int MINB>
+template <int RM, int RN, int NC, bool RES>
 int launch_fused(SupconParams p, cudaStream_t stream) {
   constexpr int TM = 16 * RM;
   const size_t smem = fused_smem_bytes<RM, RN, NC, RES>(p.A, p.d);
   static bool configured_dev[B200OCL_MAX_DEVICES] = {};
   bool& configured = configured_dev[device_slot()];
   if (!configured) {
-    B200OCL_CUDA(cudaFuncSetAttribute(supcon_fused_kernel<RM, RN, NC, RES, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    B200OCL_CUDA(cudaFuncSetAttribute(supcon_fused_kernel<RM, RN, NC, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     configured = true;
   }
   p.n_units = (p.A + TM - 1) / TM;
-  // the grid-wide wait needs every CTA resident: MINB CTAs per SM when this launch's shared memory allows it
+  // the grid-wide wait needs every CTA resident: one CTA per SM
   int per_sm = 0;
-  B200OCL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, supcon_fused_kernel<RM, RN, NC, RES, MINB>, SC_THREADS, smem));
+  B200OCL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, supcon_fused_kernel<RM, RN, NC, RES>, SC_THREADS, smem));
   if (per_sm < 1) {
     set_error("b200ocl_supcon: fused kernel does not fit on an SM (%zu bytes of shared memory)", smem);
     return B200OCL_EUNSUPPORTED;
   }
-  if (per_sm > MINB) per_sm = MINB;
-  const int coresident = per_sm * sm_count();
+  const int coresident = sm_count();
   const int grid = p.n_units < coresident ? p.n_units : coresident;
   B200OCL_PROF("supcon", 2.0 * 4.0 * p.A * p.d + 8.0 * p.B, stream);
-  supcon_fused_kernel<RM, RN, NC, RES, MINB><<<grid, SC_THREADS, smem, stream>>>(p);
+  supcon_fused_kernel<RM, RN, NC, RES><<<grid, SC_THREADS, smem, stream>>>(p);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }
 
-template <int RM, int RN, bool RES, int MINB>
+template <int RM, int RN, bool RES>
 int launch_fused_nc(const SupconParams& p, cudaStream_t stream) {
   switch ((p.d + 63) / 64) {
-    case 1: return launch_fused<RM, RN, 1, RES, MINB>(p, stream);
-    case 2: return launch_fused<RM, RN, 2, RES, MINB>(p, stream);
-    case 3: return launch_fused<RM, RN, 3, RES, MINB>(p, stream);
-    default: return launch_fused<RM, RN, 4, RES, MINB>(p, stream);
+    case 1: return launch_fused<RM, RN, 1, RES>(p, stream);
+    case 2: return launch_fused<RM, RN, 2, RES>(p, stream);
+    case 3: return launch_fused<RM, RN, 3, RES>(p, stream);
+    default: return launch_fused<RM, RN, 4, RES>(p, stream);
   }
 }
 
@@ -608,13 +601,11 @@ int b200ocl_supcon(const float* feats, const int64_t* labels, int B, int V, int 
   if (d % 4 == 0 && d <= SCF_MAX_D && (reinterpret_cast<uintptr_t>(feats) & 15) == 0 &&
       (!dfeats || (reinterpret_cast<uintptr_t>(dfeats) & 15) == 0)) {
     const int sms = sm_count();
-    if (p.A <= 16 * sms && fused_smem_bytes<1, 4, 4, true>(p.A, d) <= 200 * 1024) return launch_fused_nc<1, 4, true, 1>(p, stream);
-    if (p.A <= 16 * sms) return launch_fused_nc<1, 2, false, 1>(p, stream);
-    // large anchor sets: 64-anchor blocks, one CTA per SM.  A 32-anchor / two-CTAs-per-SM variant (16 warps per SM,
-    // B200OCL_SUPCON_2CTA=1) keeps the same shared-memory-bound inner loop: occupancy is not what bounds the kernel;
-    // the 4 x 4 register tile's lower shared-memory traffic per FMA is kept as the default.
-    if (d <= 128 && env_flag("B200OCL_SUPCON_2CTA")) return launch_fused_nc<2, 4, false, 2>(p, stream);
-    return launch_fused_nc<4, 4, false, 1>(p, stream);
+    if (p.A <= 16 * sms && fused_smem_bytes<1, 4, 4, true>(p.A, d) <= 200 * 1024) return launch_fused_nc<1, 4, true>(p, stream);
+    if (p.A <= 16 * sms) return launch_fused_nc<1, 2, false>(p, stream);
+    // large anchor sets: 64-anchor blocks, one CTA per SM.  Shared memory, not occupancy, bounds the inner loop, so
+    // the 4 x 4 register tile with the least shared-memory traffic per FMA is used.
+    return launch_fused_nc<4, 4, false>(p, stream);
   }
   static bool configured_dev[B200OCL_MAX_DEVICES] = {};
   bool& configured = configured_dev[b200ocl::device_slot()];

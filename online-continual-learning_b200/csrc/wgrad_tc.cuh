@@ -2,7 +2,6 @@
 // workspace sizing (net_ws.cuh), the launcher and the backward driver (net_bwd.cu).
 #pragma once
 #include <cuda_runtime.h>
-#include <stdlib.h>
 
 namespace b200ocl {
 
@@ -23,16 +22,6 @@ inline int wgrad_tc_tiles(int N, int H, int W) {
   return (int)(last / 128) + 1;
 }
 
-// Which weight gradients take the tensor-core kernel: B200OCL_WGRAD_TC = 0 none, 1 every covered layer (default).
-inline int wgrad_tc_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("B200OCL_WGRAD_TC");
-    on = (e && e[0] == '0') ? 0 : 1;
-  }
-  return on;
-}
-
 inline WgradTcCfg wgrad_tc_cfg(int N, int H, int W, int ks, int stride, int pad, int cin, int cout, int sms) {
   WgradTcCfg g{};
   g.eligible = (ks == 3 && stride == 1 && pad == 1 && cin % 4 == 0 && cout % 4 == 0 && cin >= 4 && cout >= 4 &&
@@ -41,12 +30,7 @@ inline WgradTcCfg wgrad_tc_cfg(int N, int H, int W, int ks, int stride, int pad,
   g.slices = (cin + 31) / 32;
   g.cout_blocks = (cout + 31) / 32;
   g.tiles = wgrad_tc_tiles(N, H, W);
-  static int tpc = 0;      // B200OCL_WGRAD_TPC: tiles per tensor-core accumulation chain (default 2 = 256 positions, ~2e-6 relative)
-  if (!tpc) {
-    const char* e = getenv("B200OCL_WGRAD_TPC");
-    tpc = (e && atoi(e) > 0 && atoi(e) <= 16) ? atoi(e) : 2;
-  }
-  g.tpc = tpc;
+  g.tpc = 2;   // 256 positions per tensor-core accumulation chain: ~2e-6 relative
   g.chains = (g.tiles + g.tpc - 1) / g.tpc;
   int want = sms / (g.slices * g.cout_blocks);
   if (want < 1) want = 1;

@@ -236,7 +236,7 @@ def test_backward_supcon_two_views(eng_mod, golden_dir):
     p64, bn64 = oresnet.seeded_state(spec, 13, dtype=torch.float64)
     leaves = {k: v.clone().requires_grad_(True) for k, v in p64.items()}
     # A ReLU whose exact pre-activation lies within fp32 rounding of zero may take either branch in ANY fp32
-    # implementation (measured with tools/scr_grad_debug.py: one such unit flips channel 60 of layer3.1.bn2 and
+    # implementation (measured: one such unit flips channel 60 of layer3.1.bn2 and
     # moves that channel's gradients by 2-3e-2, all other channels agree with fp64 to 3e-6).  Record the margins.
     margins = []
     relu = oresnet.F.relu

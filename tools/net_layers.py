@@ -1,7 +1,6 @@
 """Per-launch timings of one eval feature pass / train forward+backward at the batch sizes of the
 replay step (GPU box).  Uses the library's own CUDA-event profiler; every launch carries ~4 us of event
-overhead, so compare rows, not absolute values.   usage: python tools/net_layers.py [out.csv]
-Select the convolution path with B200OCL_TC=0|1 in the environment."""
+overhead, so compare rows, not absolute values.   usage: python tools/net_layers.py [out.csv]"""
 import os
 import sys
 
@@ -34,7 +33,7 @@ def main():
         for _ in range(3):
             eng.features_eval(x)
         torch.cuda.synchronize()
-        mark('features_eval N=%d TC=%s' % (n, os.environ.get('B200OCL_TC', 'default')))
+        mark('features_eval N=%d' % n)
         lib.b200ocl_profile_begin()
         eng.features_eval(x)
         lib.b200ocl_profile_end()
@@ -44,7 +43,7 @@ def main():
             o, ws = eng.forward_train(x)
             eng.backward(x, torch.ones_like(o) / n, ws)
         torch.cuda.synchronize()
-        mark('train fwd+bwd N=%d TC=%s' % (n, os.environ.get('B200OCL_TC', 'default')))
+        mark('train fwd+bwd N=%d' % n)
         lib.b200ocl_profile_begin()
         o, ws = eng.forward_train(x)
         eng.backward(x, torch.ones_like(o) / n, ws)
