@@ -118,6 +118,8 @@ def make_params(kind, **over):
         base.update(agent='ER', retrieve='random', update='GSS', eps_mem_batch=10, gss_mem_strength=10, gss_batch_size=10)
     elif kind == 'scr_aser':
         base.update(agent='SCR', retrieve='ASER', update='ASER', eps_mem_batch=100)
+    elif kind == 'lwf':
+        base.update(agent='LWF', retrieve='random', update='random', eps_mem_batch=10)
     else:
         raise ValueError(kind)
     base.update(over)

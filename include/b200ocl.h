@@ -233,6 +233,29 @@ int b200ocl_net_sgd_step(const b200ocl_net_desc* desc, const b200ocl_net_state* 
 int b200ocl_ce_loss(const float* logits, const int64_t* labels, int N, int C, float* loss, float* per_sample,
                     float* dlogits, int64_t* n_correct, void* stream);
 
+/* The training-trick criteria of agents/base.py:93-107 with the distillation term of utils/kd_manager.py:6-28 mixed in
+ * (exp_replay.py:41-47, agem.py:40-46, lwf.py:38-40), over logits [N,C], labels [N], in one launch:
+ *   loss[1] = w_ce * criterion + w_kd * kd, dlogits [N,C] = its gradient, n_correct[1] = #(argmax over all C == label)
+ *   (ties lowest index).  Outputs nullable.
+ * criterion by mode:
+ *   B200OCL_CLS_CE         mean CE over all C columns;
+ *   B200OCL_CLS_LABELS     labels trick: CE over the columns of the classes present in this batch (found on the device),
+ *                          C <= B200OCL_CLS_MAX_C;
+ *   B200OCL_CLS_SEPARATED  separated softmax: cols[n_cols] = old_labels ++ new_labels (duplicates allowed), log-softmax
+ *                          over cols[0,n_old) and over cols[n_old,n_cols) separately, NLL at position pos_table[label]
+ *                          (table_len entries, -1 = unmapped); only the target's segment gets a gradient, and a column
+ *                          held at several positions sums their terms in position order.
+ * kd = 4 * mean_i sum_c -softmax(teacher_ic/2) * log_softmax(logits_ic/2) (temperature 2) when teacher != NULL,
+ * else kd = 0.  A label outside [0,C), or unmapped in the table, sets *err_flag = 1 (nullable, never cleared) and adds
+ * nothing to the loss or gradient.  One CTA, fixed-order sums, no atomics: repeated launches are bit-identical. */
+#define B200OCL_CLS_CE 0
+#define B200OCL_CLS_LABELS 1
+#define B200OCL_CLS_SEPARATED 2
+#define B200OCL_CLS_MAX_C 12288
+int b200ocl_cls_loss(const float* logits, const int64_t* labels, int N, int C, int mode, const int64_t* cols,
+                     int n_cols, int n_old, const int64_t* pos_table, int table_len, const float* teacher, float w_ce,
+                     float w_kd, float* loss, float* dlogits, int64_t* n_correct, int* err_flag, void* stream);
+
 /* ---------------------------------------------------------------- SCR augmentation
  * The second view of agents/scr.py:18-24,54 (kornia RandomResizedCrop -> RandomHorizontalFlip ->
  * ColorJitter -> RandomGrayscale) in one kernel over NCHW fp32 images in [0,1].

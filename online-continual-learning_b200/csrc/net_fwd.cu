@@ -343,6 +343,34 @@ __global__ void __launch_bounds__(256) l2norm_fwd_kernel(const float* __restrict
 }
 
 // ----------------------------------------------------------------------------- cross-entropy
+// Warp-wide maximum (ties to the lowest index) and log-sum-exp of the K values get(0..K-1) of one row.  Lanes take
+// strided elements and reduce through shuffles, so the summation order is the same on every call.
+struct RowLse {
+  float mx;
+  int arg;
+  float lse;
+};
+
+template <class Get>
+__device__ __forceinline__ RowLse row_lse(Get get, int K, int lane) {
+  float mx = -FLT_MAX;
+  int arg = 0;
+  for (int c = lane; c < K; c += 32) {
+    const float v = get(c);
+    if (v > mx) { mx = v; arg = c; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float om = __shfl_xor_sync(FULL_MASK, mx, o);
+    const int oa = __shfl_xor_sync(FULL_MASK, arg, o);
+    if (om > mx || (om == mx && oa < arg)) { mx = om; arg = oa; }
+  }
+  float z = 0.f;
+  for (int c = lane; c < K; c += 32) z += expf(get(c) - mx);
+  z = warp_sum(z);
+  return RowLse{mx, arg, mx + logf(z)};
+}
+
 __global__ void __launch_bounds__(256) ce_kernel(const float* __restrict__ logits, const long long* __restrict__ labels,
                                                  int N, int C, float* __restrict__ loss, float* __restrict__ per_sample,
                                                  float* __restrict__ dlogits, long long* __restrict__ n_correct) {
@@ -353,23 +381,10 @@ __global__ void __launch_bounds__(256) ce_kernel(const float* __restrict__ logit
   int corr = 0;
   for (int n = warp; n < N; n += 8) {   // fixed assignment of rows to warps: deterministic sum
     const float* lr = logits + (size_t)n * C;
-    float mx = -FLT_MAX;
-    int arg = 0;
-    for (int c = lane; c < C; c += 32) {
-      const float v = lr[c];
-      if (v > mx) { mx = v; arg = c; }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float om = __shfl_xor_sync(FULL_MASK, mx, o);
-      const int oa = __shfl_xor_sync(FULL_MASK, arg, o);
-      if (om > mx || (om == mx && oa < arg)) { mx = om; arg = oa; }
-    }
-    float z = 0.f;
-    for (int c = lane; c < C; c += 32) z += expf(lr[c] - mx);
-    z = warp_sum(z);
+    const RowLse r = row_lse([=](int c) { return __ldg(lr + c); }, C, lane);
+    const float lse = r.lse;
+    const int arg = r.arg;
     const long long y = labels[n];
-    const float lse = mx + logf(z);
     const float l = lse - lr[y];
     if (per_sample && lane == 0) per_sample[n] = l;
     if (dlogits) {
@@ -388,6 +403,118 @@ __global__ void __launch_bounds__(256) ce_kernel(const float* __restrict__ logit
     for (int w = 0; w < 8; ++w) { t += s_loss[w]; k += s_corr[w]; }
     if (loss) *loss = t / (float)N;
     if (n_correct) *n_correct = k;
+  }
+}
+
+// ----------------------------------------------------------------------------- classification-loss variants
+// The criteria of agents/base.py:93-113 besides plain CE and SupCon, with the distillation term of
+// utils/kd_manager.py:6-11 mixed in (exp_replay.py:41-47, agem.py:40-46, lwf.py:38-40).  Like ce_kernel: one CTA,
+// a fixed assignment of rows to warps and fixed-order sums, so repeated launches give identical bits.
+struct ClsLossArgs {
+  const float* logits;
+  const long long* labels;
+  int N, C, mode;
+  const long long* cols;     // separated softmax: old_labels ++ new_labels (duplicates allowed)
+  int n_cols, n_old;         // ... and the segment boundary
+  const long long* pos;      // label -> position in cols (lbl_inv_map), -1 where unmapped
+  int n_pos;
+  const float* teacher;      // nullable: teacher logits [N,C]
+  float w_ce, w_kd;
+  float* loss;
+  float* dlogits;
+  long long* n_correct;
+  int* err;
+};
+
+constexpr float KD_T = 2.f;  // loss_fn_kd's temperature (kd_manager.py:6)
+
+__global__ void __launch_bounds__(256) cls_loss_kernel(ClsLossArgs a) {
+  extern __shared__ int s_on[];          // labels trick: class c occurs in the batch
+  __shared__ float s_ce[8], s_kd[8];
+  __shared__ int s_corr[8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int C = a.C;
+  if (a.mode == B200OCL_CLS_LABELS) {
+    // the batch's class set labels.unique(): a presence map over the C columns.  CE over the present columns with
+    // each label remapped to its rank among them is CE over those columns at the label's own column.
+    for (int c = threadIdx.x; c < C; c += blockDim.x) s_on[c] = 0;
+    __syncthreads();
+    for (int n = threadIdx.x; n < a.N; n += blockDim.x) {
+      const long long y = a.labels[n];
+      if (y >= 0 && y < C) s_on[y] = 1;
+    }
+    __syncthreads();
+  }
+  const float invN = 1.f / (float)a.N;
+  float ce_sum = 0.f, kd_sum = 0.f;
+  int corr = 0;
+  for (int n = warp; n < a.N; n += 8) {
+    const float* lr = a.logits + (size_t)n * C;
+    const float* tr = a.teacher ? a.teacher + (size_t)n * C : nullptr;
+    const long long y = a.labels[n];
+    bool bad = y < 0 || y >= C;
+    int p = 0, s0 = 0, s1 = 0;           // separated softmax: the target's position and its segment [s0, s1)
+    if (a.mode == B200OCL_CLS_SEPARATED) {
+      const long long q = (!bad && y < a.n_pos) ? a.pos[y] : -1;
+      bad = bad || q < 0 || q >= a.n_cols;
+      p = bad ? 0 : (int)q;
+      s0 = p < a.n_old ? 0 : a.n_old;
+      s1 = p < a.n_old ? a.n_old : a.n_cols;
+    }
+    if (bad) {                           // the host raises KeyError; the row adds nothing
+      if (lane == 0 && a.err) *a.err = 1;
+      if (a.dlogits)
+        for (int c = lane; c < C; c += 32) a.dlogits[(size_t)n * C + c] = 0.f;
+      continue;
+    }
+    const RowLse all = row_lse([=](int c) { return __ldg(lr + c); }, C, lane);     // arg-max over every column (meters)
+    const int arg = all.arg;
+    float lse = all.lse, tgt = lr[y];
+    if (a.mode == B200OCL_CLS_LABELS) {
+      lse = row_lse([=](int c) { return s_on[c] ? __ldg(lr + c) : -INFINITY; }, C, lane).lse;
+    } else if (a.mode == B200OCL_CLS_SEPARATED) {
+      const long long* cs = a.cols + s0;
+      lse = row_lse([=](int k) { return __ldg(lr + __ldg(cs + k)); }, s1 - s0, lane).lse;
+      tgt = lr[a.cols[p]];
+    }
+    ce_sum += lse - tgt;
+    corr += (arg == (int)y) ? 1 : 0;
+    float lse_s = 0.f, lse_t = 0.f;
+    if (tr) {                            // T^2 * sum_c -softmax(t/T)_c * log_softmax(s/T)_c
+      lse_s = row_lse([=](int c) { return __ldg(lr + c) / KD_T; }, C, lane).lse;
+      lse_t = row_lse([=](int c) { return __ldg(tr + c) / KD_T; }, C, lane).lse;
+      float k = 0.f;
+      for (int c = lane; c < C; c += 32) k -= expf(tr[c] / KD_T - lse_t) * (lr[c] / KD_T - lse_s);
+      kd_sum += warp_sum(k) * (KD_T * KD_T);
+    }
+    if (a.dlogits) {
+      const float sce = a.w_ce * invN, skd = a.w_kd * KD_T * invN;
+      for (int c = lane; c < C; c += 32) {
+        float g = 0.f;
+        if (a.mode == B200OCL_CLS_SEPARATED) {
+          // every position of the target's segment that holds column c, in position order
+          const float e = expf(lr[c] - lse);
+          for (int k = s0; k < s1; ++k)
+            if (a.cols[k] == c) g += e - (k == p ? 1.f : 0.f);
+        } else if (a.mode == B200OCL_CLS_CE || s_on[c]) {
+          g = expf(lr[c] - lse) - (c == (int)y ? 1.f : 0.f);
+        }
+        float d = g * sce;
+        if (tr) d = fmaf(skd, expf(lr[c] / KD_T - lse_s) - expf(tr[c] / KD_T - lse_t), d);
+        a.dlogits[(size_t)n * C + c] = d;
+      }
+    }
+  }
+  if (lane == 0) { s_ce[warp] = ce_sum; s_kd[warp] = kd_sum; s_corr[warp] = corr; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float ce = 0.f, kd = 0.f;
+    int k = 0;
+    for (int w = 0; w < 8; ++w) { ce += s_ce[w]; kd += s_kd[w]; k += s_corr[w]; }
+    float l = a.w_ce * (ce / (float)a.N);
+    if (a.teacher) l += a.w_kd * (kd / (float)a.N);
+    if (a.loss) *a.loss = l;
+    if (a.n_correct) *a.n_correct = k;
   }
 }
 
@@ -870,6 +997,31 @@ int b200ocl_ce_loss(const float* logits, const int64_t* labels, int N, int C, fl
   B200OCL_PROF("ce_loss", 8.0 * N * C, stream);
   ce_kernel<<<1, 256, 0, stream>>>(logits, reinterpret_cast<const long long*>(labels), N, C, loss, per_sample, dlogits,
                                    reinterpret_cast<long long*>(n_correct));
+  B200OCL_LAUNCHED();
+  return B200OCL_OK;
+}
+
+int b200ocl_cls_loss(const float* logits, const int64_t* labels, int N, int C, int mode, const int64_t* cols,
+                     int n_cols, int n_old, const int64_t* pos_table, int table_len, const float* teacher, float w_ce,
+                     float w_kd, float* loss, float* dlogits, int64_t* n_correct, int* err_flag, void* stream_) {
+  using namespace b200ocl;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200OCL_CHECK_ARG(logits && labels && N >= 1 && C >= 1, "need logits, labels, N >= 1, C >= 1");
+  B200OCL_CHECK_ARG(mode == B200OCL_CLS_CE || mode == B200OCL_CLS_LABELS || mode == B200OCL_CLS_SEPARATED, "unknown mode");
+  B200OCL_CHECK_ARG(mode != B200OCL_CLS_SEPARATED ||
+                    (cols && pos_table && n_cols >= 1 && n_old >= 0 && n_old <= n_cols && table_len >= 0),
+                    "separated softmax needs cols [n_cols >= 1], 0 <= n_old <= n_cols and a position table");
+  if (mode == B200OCL_CLS_LABELS && C > B200OCL_CLS_MAX_C) {
+    set_error("b200ocl_cls_loss: labels trick over C = %d > %d classes", C, B200OCL_CLS_MAX_C);
+    return B200OCL_EUNSUPPORTED;
+  }
+  ClsLossArgs a{logits, reinterpret_cast<const long long*>(labels), N, C, mode,
+                reinterpret_cast<const long long*>(cols), n_cols, n_old,
+                reinterpret_cast<const long long*>(pos_table), table_len, teacher, w_ce, w_kd, loss, dlogits,
+                reinterpret_cast<long long*>(n_correct), err_flag};
+  const size_t smem = mode == B200OCL_CLS_LABELS ? (size_t)C * sizeof(int) : 0;
+  B200OCL_PROF("cls_loss", (teacher ? 12.0 : 8.0) * N * C, stream);
+  cls_loss_kernel<<<1, 256, smem, stream>>>(a);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }

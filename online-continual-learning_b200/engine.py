@@ -123,6 +123,7 @@ class Engine:
         self.dim_in, self.out_dim = self.info.dim_in, self.info.out_dim
         self.state = ArenaState(self.info, self.device)
         self._virtual = None
+        self._teacher = None
         self._eval_ws = {}
         self._train_ws = {}
         self._graphs = {}
@@ -178,6 +179,34 @@ class Engine:
             self._virtual = ArenaState(self.info, self.device, with_grads=False)
         return self._virtual
 
+    # ------------------------------------------------------------------ distillation teacher
+    TEACHER_SLOT = 6
+
+    def update_teacher(self):
+        """copy.deepcopy(model) of KdManager.update_teacher (utils/kd_manager.py:18-19): parameters, BN running
+        statistics and num_batches_tracked copied into one persistent arena set.  Every call writes the same buffers, so
+        the pointers a captured teacher forward holds stay valid."""
+        t = self._teacher
+        if t is None:
+            t = self._teacher = ArenaState(self.info, self.device, with_grads=False)
+        t.params.copy_(self.state.params)
+        t.bn_stats.copy_(self.state.bn_stats)
+        t.bn_tracked.copy_(self.state.bn_tracked)
+        self.pack(t)
+
+    @property
+    def teacher(self):
+        """The teacher's arenas, None until update_teacher() has run."""
+        return self._teacher
+
+    def teacher_forward(self, x, slot=TEACHER_SLOT):
+        """teacher_model.forward(x) under no_grad (kd_manager.py:24-25).  The copy was taken from a model in train
+        mode and never switched, so this is a train-mode forward: batch statistics, and the teacher's own running
+        statistics move (they never feed anything).  Graphed like the live forward, under its own key."""
+        if self._teacher is None:
+            raise RuntimeError('no teacher: call update_teacher() first')
+        return self.forward_train(x, state=self._teacher, slot=slot, _tag='teacher')[0]
+
     # ------------------------------------------------------------------ passes
     def _x(self, x):
         _need_cuda(x)
@@ -230,15 +259,17 @@ class Engine:
                 self._train_ws[key] = ws
         return ws
 
-    def forward_train(self, x, ws=None, state=None, slot=0, eval_stats=False, defer_stats=False):
+    def forward_train(self, x, ws=None, state=None, slot=0, eval_stats=False, defer_stats=False, _tag='fwd'):
         """model.train(); model.forward(x).  Returns (out [N,out_dim], workspace kept for backward).
         eval_stats=True: model.eval() forward that can be differentiated (running statistics, nothing updated).
         defer_stats=True: the BN running statistics are left alone; apply_running_stats(ws, N) moves them later (so that
         the train-mode passes of one step can run concurrently on different streams and still update the statistics in
-        the reference's order)."""
+        the reference's order).  _tag: the graph key of a forward over another persistent state (the teacher's); other
+        forwards over a state= run eagerly."""
         x = self._x(x)
         n = x.shape[0]
-        graphed = _GRAPHS and ws is None and state is None and (n, slot) in self._train_ws and not eval_stats
+        graphed = (_GRAPHS and ws is None and (state is None) == (_tag == 'fwd') and (n, slot) in self._train_ws
+                   and not eval_stats)
         if ws is None:
             ws = self.train_workspace(n, slot)
         st = state or self.state
@@ -251,10 +282,10 @@ class Engine:
             _native.check(rc, name)
 
         if graphed:
-            key = ('fwd', n, slot, bool(defer_stats))
+            key = (_tag, n, slot, bool(defer_stats))
             e = self._graphs.get(key)
             if e is None:
-                other = self._graphs.get(('fwd', n, slot, not defer_stats))     # one static input per (n, slot)
+                other = self._graphs.get((_tag, n, slot, not defer_stats))      # one static input per (n, slot)
                 e = self._graphs[key] = _Graphed([other.inputs[0] if other is not None else torch.empty_like(x)],
                                                  [torch.empty((n, self.out_dim), dtype=torch.float32, device=x.device)])
             e.inputs[0].copy_(x)
@@ -340,4 +371,37 @@ def ce_loss(logits, labels, want_grad=True, want_per_sample=False, want_correct=
     rc = _lib().b200ocl_ce_loss(logits.data_ptr(), labels.data_ptr(), n, c, out['loss'].data_ptr(),
                                 ptr(out['per_sample']), ptr(out['dlogits']), ptr(out['n_correct']), _stream())
     _native.check(rc, 'b200ocl_ce_loss')
+    return out
+
+
+CLS_MODES = {'ce': 0, 'labels_trick': 1, 'separated_softmax': 2}
+
+
+def cls_loss(logits, labels, mode='ce', cols=None, n_old=0, pos_table=None, teacher=None, w_ce=1.0, w_kd=0.0,
+             err=None, want_grad=True, want_correct=False):
+    """w_ce * criterion + w_kd * distillation (b200ocl_cls_loss); returns dict(loss[1], dlogits, n_correct[1]).
+    mode 'labels_trick' | 'separated_softmax' | 'ce'; separated softmax takes cols = old_labels ++ new_labels (int64
+    device tensor), the boundary n_old and pos_table (label -> position, -1 unmapped).  teacher: teacher logits or None
+    (no distillation term).  err: int32 device flag [1] set to 1 by an unmapped label."""
+    _need_cuda(logits, labels, cols, pos_table, teacher, err)
+    logits = logits.detach().to(torch.float32).contiguous()
+    labels = labels.detach().to(torch.int64).contiguous()
+    n, c = logits.shape
+    if teacher is not None:
+        teacher = teacher.detach().to(torch.float32).contiguous()
+        if teacher.shape != logits.shape:
+            raise ValueError('teacher logits must match the logits in shape')
+    m = CLS_MODES[mode]
+    if m == 2:
+        cols, pos_table = cols.to(torch.int64).contiguous(), pos_table.to(torch.int64).contiguous()
+    dev = logits.device
+    out = {'loss': torch.empty(1, dtype=torch.float32, device=dev)}
+    out['dlogits'] = torch.empty_like(logits) if want_grad else None
+    out['n_correct'] = torch.empty(1, dtype=torch.int64, device=dev) if want_correct else None
+    ptr = lambda t: 0 if t is None else t.data_ptr()
+    rc = _lib().b200ocl_cls_loss(logits.data_ptr(), labels.data_ptr(), n, c, m, ptr(cols) if m == 2 else 0,
+                                 cols.numel() if m == 2 else 0, int(n_old), ptr(pos_table) if m == 2 else 0,
+                                 pos_table.numel() if m == 2 else 0, ptr(teacher), float(w_ce), float(w_kd),
+                                 out['loss'].data_ptr(), ptr(out['dlogits']), ptr(out['n_correct']), ptr(err), _stream())
+    _native.check(rc, 'b200ocl_cls_loss')
     return out

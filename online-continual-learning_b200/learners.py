@@ -1,7 +1,8 @@
 """Agents of the replay path with the reference surface `cls(model, opt, params)`,
 `.train_learner(x_train, y_train)`, `.evaluate(test_loaders)`:
-ExperienceReplay (agents/exp_replay.py:10-104: ER / MIR / ASER) and SupContrastReplay
-(agents/scr.py:11-69), over ContinualLearner (agents/base.py:14-113).
+ExperienceReplay (agents/exp_replay.py:10-104: ER / MIR / ASER), SupContrastReplay (agents/scr.py:11-69), AGEM
+(agents/agem.py) and Lwf (agents/lwf.py), over ContinualLearner (agents/base.py:14-113) with its training tricks
+(labels trick, separated softmax, kd_trick / kd_trick_star, review trick).
 
 The loop structure, the order of train-mode forwards (they move BN running statistics) and the
 order of buffer operations follow the reference step exactly; what changes is who does the
@@ -14,7 +15,7 @@ import torch
 
 from . import memory, ops
 from .augment import SCRTransform
-from .engine import ce_loss
+from .engine import ce_loss, cls_loss
 from .memory import Buffer, input_size_match
 from .nets import adopt, engine_of, EngineModel
 
@@ -91,6 +92,33 @@ class StreamFeeder(object):
             yield self.x[i * b:(i + 1) * b], self.y[i * b:(i + 1) * b], self.y_host[i * b:(i + 1) * b]
 
 
+def separated_softmax_table(old_labels, new_labels, lbl_inv_map):
+    """Host side of the separated-softmax criterion (agents/base.py:100-106): the column list old_labels ++ new_labels
+    (a label recurs in it when it recurs across tasks), the segment boundary, and the label -> position table of
+    lbl_inv_map as an int64 array (-1 where a label has no entry: the reference raises KeyError there)."""
+    cols = np.asarray(list(old_labels) + list(new_labels), dtype=np.int64)
+    keys = [int(k) for k in lbl_inv_map if int(k) >= 0]
+    pos = np.full(max(keys) + 1 if keys else 1, -1, dtype=np.int64)
+    for k, v in lbl_inv_map.items():
+        if int(k) >= 0:
+            pos[int(k)] = int(v)
+    return cols, len(old_labels), pos
+
+
+def kd_mix(task_seen, kd_trick=False, kd_trick_star=False, lwf=False):
+    """(w_ce, w_kd): the loss is w_ce * criterion + w_kd * distillation.  kd_trick: a = 1/(task_seen+1),
+    a * loss + (1-a) * kd; kd_trick_star: the same with 1/sqrt(task_seen+1), applied after kd_trick when both are set
+    (exp_replay.py:41-47, agem.py:40-46); LwF: the kd_trick mixing whatever the flags (lwf.py:38-40)."""
+    w_ce, w_kd = 1.0, 0.0
+    if kd_trick or lwf:
+        a = 1.0 / (task_seen + 1)
+        w_ce, w_kd = a, 1.0 - a
+    if kd_trick_star and not lwf:
+        b = 1.0 / ((task_seen + 1) ** 0.5)
+        w_ce, w_kd = b * w_ce, b * w_kd + (1.0 - b)
+    return w_ce, w_kd
+
+
 class ContinualLearner(torch.nn.Module):
     """Label bookkeeping and loss dispatch of agents/base.py:14-113 for the replay path."""
 
@@ -110,9 +138,20 @@ class ContinualLearner(torch.nn.Module):
         self.lbl_inv_map = {}
         self.class_task_map = {}
         trick = getattr(params, 'trick', None) or {}
-        unsupported = [k for k in ('labels_trick', 'kd_trick', 'separated_softmax', 'kd_trick_star') if trick.get(k)]
-        if unsupported:
-            raise NotImplementedError('tricks %s are outside the replay-path scope (SURVEY section 8f)' % unsupported)
+        self._trick = {k: bool(trick.get(k)) for k in ('labels_trick', 'separated_softmax', 'kd_trick', 'kd_trick_star')}
+        contrastive = params.agent in ('SCR', 'SCP')
+        if contrastive and (self._trick['labels_trick'] or self._trick['separated_softmax']):
+            # base.py:95-107 would feed [B,2,128] projections to a CE branch
+            raise NotImplementedError('labels_trick / separated_softmax do not apply to the SupCon loss of %s' % params.agent)
+        # base.py:96-107: exactly one criterion, labels trick first
+        self._mode = ('labels_trick' if self._trick['labels_trick'] else
+                      'separated_softmax' if self._trick['separated_softmax'] else 'ce')
+        self._lwf = params.agent == 'LWF'
+        # base.py:90-91 takes the teacher for kd_trick or LwF; SCR never reads it, so it is not taken there
+        self._takes_teacher = (self._trick['kd_trick'] or self._lwf) and not contrastive
+        self._teacher_live = False
+        self._sep = None           # separated softmax: (cols, n_old, position table) on the device, one upload per task
+        self._err = None           # device flag: a label the criterion cannot map (KeyError in the reference)
         if isinstance(model, EngineModel):
             self.engine = model.engine
         else:
@@ -172,14 +211,60 @@ class ContinualLearner(torch.nn.Module):
             self.lbl_inv_map[lbl] = len(self.old_labels) + i
         for i in new_labels:
             self.class_task_map[i] = self.task_seen
+        self._task_tables()
 
     def after_train(self):
         self.old_labels += self.new_labels
         self.new_labels_zombie = list(self.new_labels)
         self.new_labels.clear()
         self.task_seen += 1
+        self._task_tables()
         if (getattr(self.params, 'trick', None) or {}).get('review_trick') and hasattr(self, 'buffer'):
             self._review()
+        if self._takes_teacher:                                                     # base.py:90-91, after the review
+            self.engine.update_teacher()
+            self._teacher_live = True
+
+    # ------------------------------------------------------------------ criterion (agents/base.py:93-113)
+    def _task_tables(self):
+        """Upload the separated-softmax column list and position table (they change only between tasks)."""
+        if self._mode != 'separated_softmax':
+            return
+        cols, n_old, pos = separated_softmax_table(self.old_labels, self.new_labels, self.lbl_inv_map)
+        if cols.size == 0:
+            cols = np.zeros(1, dtype=np.int64)       # no label is mapped yet: every position lookup fails first
+        self._sep = (torch.from_numpy(cols).to(self.device), n_old, torch.from_numpy(pos).to(self.device))
+
+    def _err_flag(self):
+        if self._err is None:
+            self._err = torch.zeros(1, dtype=torch.int32, device=self.device)
+        return self._err
+
+    def _raise_label_errors(self):
+        """One read per task.  The reference raises KeyError at the step that meets an unmapped label
+        (base.py:105); here the steps of the task run to the end and the error surfaces when train_learner returns."""
+        if self._err is not None and int(self._err.item()):
+            self._err.zero_()
+            raise KeyError('a label outside the logits or without a separated-softmax position was trained on '
+                           '(the reference raises at agents/base.py:105)')
+
+    def criterion(self, logits, labels, teacher_logits=None, w_ce=1.0, w_kd=0.0, want_grad=True, want_correct=False):
+        """self.criterion(logits, labels) on the device, times w_ce, plus w_kd times the distillation loss against
+        teacher_logits when given: dict(loss[1], dlogits, n_correct[1]).  Plain CE goes through b200ocl_ce_loss as
+        before; the tricks and the distillation mixing through b200ocl_cls_loss."""
+        if self._mode == 'ce' and teacher_logits is None and w_ce == 1.0:
+            return ce_loss(logits, labels, want_grad=want_grad, want_correct=want_correct)
+        cols, n_old, pos = self._sep if self._mode == 'separated_softmax' else (None, 0, None)
+        return cls_loss(logits, labels, self._mode, cols=cols, n_old=n_old, pos_table=pos, teacher=teacher_logits,
+                        w_ce=w_ce, w_kd=w_kd, err=self._err_flag(), want_grad=want_grad, want_correct=want_correct)
+
+    def _kd_loss(self, logits, labels, x, want_grad=True, want_correct=False):
+        """criterion mixed with the distillation term for the flags in force (exp_replay.py:41-47; lwf.py:37-39):
+        the teacher forward runs only once a teacher exists and its term has a non-zero weight."""
+        w_ce, w_kd = kd_mix(self.task_seen, self._trick['kd_trick'], self._trick['kd_trick_star'], self._lwf)
+        t = self.engine.teacher_forward(x) if (self._teacher_live and w_kd != 0.0) else None
+        return self.criterion(logits, labels, t, w_ce, w_kd if t is not None else 0.0, want_grad=want_grad,
+                              want_correct=want_correct)
 
     def _review(self):
         """Review trick (agents/base.py:62-88, the published SCR setting config_CVPR/agent/scr/scr_5k.yml:10): one
@@ -213,7 +298,7 @@ class ContinualLearner(torch.nn.Module):
                 eng.backward(bx, dfeat[:, 0].contiguous(), ws1)
                 eng.backward(aug, dfeat[:, 1].contiguous(), ws2, accumulate=True)
             else:
-                ce = ce_loss(out, by, want_grad=True)
+                ce = self.criterion(out, by)                                         # base.py:80 (tricks apply, no KD)
                 eng.backward(bx, ce['dlogits'], ws)
             self._optimizer_step(lr / 10.0, wd * 10.0)                               # base.py:83-87
             self._throttle()
@@ -290,9 +375,14 @@ class ExperienceReplay(ContinualLearner):
         eng = self.engine
         lr, wd = self._lr_wd()
         aser = self._aser_branch
+        # in the ASER branch the stream and memory losses reach only the meters (and MIR's virtual step): their
+        # distillation terms, and so the teacher forwards, are skipped when nothing reads them
+        kd = not aser or meters is not None
         for _ in range(self.mem_iters):
             logits, ws = eng.forward_train(batch_x, slot=0)                         # :40  (BN stats move)
-            ce = ce_loss(logits, batch_y, want_grad=self._needs_batch_grad, want_correct=meters is not None)
+            ce = self._kd_loss(logits, batch_y, batch_x, want_grad=self._needs_batch_grad, want_correct=meters is not None) \
+                if (kd or self._needs_batch_grad) else \
+                self.criterion(logits, batch_y, want_grad=self._needs_batch_grad, want_correct=meters is not None)   # :41-47
             if meters is not None:
                 meters['acc_batch'].update(ce['n_correct'] / batch_y.size(0), batch_y.size(0))
                 meters['losses_batch'].update(ce['loss'], batch_y.size(0))
@@ -307,10 +397,11 @@ class ExperienceReplay(ContinualLearner):
                 with torch.cuda.stream(side):
                     mem_logits, ws_m = eng.forward_train(mem_x, slot=1, defer_stats=True)
                     if meters is not None:
-                        ce_m = ce_loss(mem_logits, mem_y, want_grad=False, want_correct=True)
+                        ce_m = self._kd_loss(mem_logits, mem_y, mem_x, want_grad=False, want_correct=True)
             elif mem_x.size(0) > 0:
                 mem_logits, ws_m = eng.forward_train(mem_x, slot=1)                 # :62  (BN stats move)
-                ce_m = ce_loss(mem_logits, mem_y, want_grad=not aser, want_correct=meters is not None)
+                ce_m = (self._kd_loss(mem_logits, mem_y, mem_x, want_grad=not aser, want_correct=meters is not None) if kd
+                        else self.criterion(mem_logits, mem_y, want_grad=False))    # :63-70
             if mem_x.size(0) > 0 and not both:
                 if meters is not None:
                     meters['losses_mem'].update(ce_m['loss'], mem_y.size(0))
@@ -328,7 +419,7 @@ class ExperienceReplay(ContinualLearner):
                     if meters is not None:
                         meters['losses_mem'].update(ce_m['loss'], mem_y.size(0))
                         meters['acc_mem'].update(ce_m['n_correct'] / mem_y.size(0), mem_y.size(0))
-                ce_c = ce_loss(logits_c, labels, want_grad=True)
+                ce_c = self.criterion(logits_c, labels)                             # :85 (no distillation term)
                 eng.backward(combined, ce_c['dlogits'], ws_c)                       # :86
                 self.last_loss = ce_c['loss']
             else:
@@ -354,6 +445,7 @@ class ExperienceReplay(ContinualLearner):
                           .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
                     print('==>>> it: {}, mem avg. loss: {:.6f}, running mem acc: {:.3f}'
                           .format(i, meters['losses_mem'].avg(), meters['acc_mem'].avg()))
+        self._raise_label_errors()
         self.after_train()
 
 
@@ -442,7 +534,7 @@ class AGEM(ContinualLearner):
         lr, wd = self._lr_wd()
         for _ in range(self.mem_iters):
             logits, ws = eng.forward_train(batch_x, slot=0)                          # :39
-            ce = ce_loss(logits, batch_y, want_grad=True, want_correct=meters is not None)
+            ce = self._kd_loss(logits, batch_y, batch_x, want_grad=True, want_correct=meters is not None)   # :40-46
             if meters is not None:
                 meters['acc_batch'].update(ce['n_correct'] / batch_y.size(0), batch_y.size(0))
                 meters['losses_batch'].update(ce['loss'], batch_y.size(0))
@@ -453,7 +545,7 @@ class AGEM(ContinualLearner):
                 if mem_x.size(0) > 0:
                     self._g_cur.copy_(eng.state.grads)                               # :62 grad of the current batch
                     mem_logits, ws_m = eng.forward_train(mem_x, slot=1)              # :65
-                    ce_m = ce_loss(mem_logits, mem_y, want_grad=True)
+                    ce_m = self.criterion(mem_logits, mem_y)                         # :66 (no distillation term)
                     eng.backward(mem_x, ce_m['dlogits'], ws_m)                       # :67-68 -> grad_ref in the arena
                     ops.agem_project(self._g_cur, eng.state.grads, out=eng.state.grads)   # :73-80
             self._optimizer_step(lr, wd)                                             # :81
@@ -472,4 +564,40 @@ class AGEM(ContinualLearner):
                 if i % 100 == 1 and self.verbose:
                     print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
                           .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
+        self._raise_label_errors()
+        self.after_train()
+
+
+class Lwf(ContinualLearner):
+    """Learning without Forgetting (agents/lwf.py:10-56) on the engine: no memory; per batch one train-mode forward,
+    loss = a * criterion + (1 - a) * distillation against the teacher taken after the previous task, a = 1/(task_seen+1),
+    one backward pass and one SGD step.  Evaluation is the classifier's arg-max."""
+
+    def replay_step(self, batch_x, batch_y, batch_y_host, meters=None):
+        """One iteration of lwf.py:30-46."""
+        eng = self.engine
+        lr, wd = self._lr_wd()
+        logits, ws = eng.forward_train(batch_x, slot=0)                              # :35
+        out = self._kd_loss(logits, batch_y, batch_x, want_grad=True, want_correct=meters is not None)   # :36-38
+        if meters is not None:
+            meters['acc_batch'].update(out['n_correct'] / batch_y.size(0), batch_y.size(0))
+            meters['losses_batch'].update(out['loss'], batch_y.size(0))
+        eng.backward(batch_x, out['dlogits'], ws)                                    # :45-46
+        self._optimizer_step(lr, wd)                                                 # :47
+        self.last_loss = out['loss']
+        self._throttle()
+
+    def train_learner(self, x_train, y_train):
+        self.before_train(x_train, y_train)
+        self.engine.pack()
+        self.model = self.model.train()
+        meters = {k: AverageMeter() for k in ('losses_batch', 'acc_batch')}
+        for ep in range(self.epoch):
+            stream = StreamFeeder(x_train, y_train, self.batch, self.device)
+            for i, (batch_x, batch_y, y_host) in enumerate(stream):
+                self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
+                if i % 100 == 1 and self.verbose:
+                    print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
+                          .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
+        self._raise_label_errors()
         self.after_train()
