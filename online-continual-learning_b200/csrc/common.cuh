@@ -17,13 +17,32 @@ void prof_begin(const char* kernel_class, double work, cudaStream_t stream);
 void prof_end();
 extern std::atomic<uint64_t> g_launches;
 int sm_count();
-// Function attributes (cudaFuncSetAttribute) are per device: every launcher keeps one flag per device.
 #define B200OCL_MAX_DEVICES 64
 inline int device_slot() {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= B200OCL_MAX_DEVICES) dev = 0;
   return dev;
 }
+
+// Raises the dynamic shared-memory limit of the kernels Ks to `bytes` on the current device.  Function attributes are
+// per device, so each instantiation keeps the limit it set per device and only calls cudaFuncSetAttribute when a
+// launch asks for more; a smaller request changes nothing.
+template <auto... Ks>
+cudaError_t raise_smem_limit(size_t bytes) {
+  static size_t set_dev[B200OCL_MAX_DEVICES] = {};
+  size_t& set = set_dev[device_slot()];
+  if (bytes <= set) return cudaSuccess;
+  for (const void* k : {reinterpret_cast<const void*>(Ks)...}) {
+    const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) return e;
+  }
+  set = bytes;
+  return cudaSuccess;
+}
+
+// B200OCL_OK when the caller's workspace is non-null, 256-byte aligned and at least `need` bytes; otherwise records
+// which entry point refused it and returns B200OCL_EWORKSPACE.
+int check_workspace(const char* entry, const void* ws, size_t ws_bytes, size_t need);
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
@@ -64,6 +83,22 @@ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
   } while (0)
 
 constexpr unsigned FULL_MASK = 0xffffffffu;
+
+// 16-byte global -> shared copies (cp.async.cg).  With src_bytes < 16 the rest of the 16 bytes is zero-filled.
+__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src, int src_bytes) {
+  const unsigned int s = static_cast<unsigned int>(__cvta_generic_to_shared(smem_dst));
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem_src), "r"(src_bytes));
+}
+__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
+  const unsigned int s = static_cast<unsigned int>(__cvta_generic_to_shared(smem_dst));
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem_src));
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
+// wait until at most N committed groups are still in flight
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
+}
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -25,16 +25,6 @@ namespace {
 
 constexpr int CONV_THREADS = 128;
 
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src, int src_bytes) {
-  const unsigned int s = static_cast<unsigned int>(__cvta_generic_to_shared(smem_dst));
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem_src), "r"(src_bytes));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
-}
-
 __device__ __forceinline__ double warp_sum_d(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL_MASK, v, o);
@@ -559,12 +549,7 @@ int launch_conv_ksplit(const ConvArgs& a, cudaStream_t stream) {
   constexpr int BM = 32 * PT;
   constexpr int NST = (PT == 1 && KS == 4) ? 4 : 3;
   constexpr size_t smem = (size_t)(NST * KS * (BM * 20 + 400)) * sizeof(float) + 4 * BM * sizeof(int);
-  static bool configured_dev[B200OCL_MAX_DEVICES] = {};
-  bool& configured = configured_dev[b200ocl::device_slot()];
-  if (!configured) {
-    B200OCL_CUDA(cudaFuncSetAttribute(conv_ksplit_kernel<PT, KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = true;
-  }
+  B200OCL_CUDA((raise_smem_limit<conv_ksplit_kernel<PT, KS>>(smem)));
   dim3 grid((a.M + BM - 1) / BM, a.CN / 20);
   B200OCL_PROF(a.transposed ? "conv_dgrad" : (a.mode == CONV_EVAL ? "conv_eval" : "conv_train"),
                2.0 * a.M * (double)a.CN * a.CK * a.ks * a.ks, stream);
@@ -702,12 +687,7 @@ inline PatchTile patch_tile(const ConvArgs& a, int bn, int pt) {
 template <int BN, int PT>
 int launch_conv_patch(ConvArgs a, const PatchTile& t, cudaStream_t stream) {
   a.th = t.th; a.tw = t.tw; a.ti = t.ti;
-  static size_t configured_dev[B200OCL_MAX_DEVICES] = {};
-  size_t& configured = configured_dev[b200ocl::device_slot()];
-  if (t.smem > configured) {
-    B200OCL_CUDA(cudaFuncSetAttribute(conv_patch_kernel<BN, PT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)t.smem));
-    configured = t.smem;
-  }
+  B200OCL_CUDA((raise_smem_limit<conv_patch_kernel<BN, PT>>(t.smem)));
   dim3 grid((unsigned)(t.ctas / (a.CN / BN)), a.CN / BN);
   B200OCL_PROF(a.flip ? "conv_dgrad" : (a.mode == CONV_EVAL ? "conv_eval" : "conv_train"),
                2.0 * a.M * (double)a.CN * a.CK * a.ks * a.ks, stream);
@@ -720,12 +700,7 @@ template <int BN, int PT>
 int launch_conv_cfg(const ConvArgs& a, cudaStream_t stream) {
   constexpr int WN = BN / 20, WM = 4 / WN, BM = WM * 32 * PT;
   constexpr size_t smem = (size_t)(3 * BM * 20 + 3 * 20 * BN) * sizeof(float) + 4 * BM * sizeof(int);
-  static bool configured_dev[B200OCL_MAX_DEVICES] = {};
-  bool& configured = configured_dev[b200ocl::device_slot()];
-  if (!configured) {
-    B200OCL_CUDA(cudaFuncSetAttribute(conv_kernel<BN, PT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = true;
-  }
+  B200OCL_CUDA((raise_smem_limit<conv_kernel<BN, PT>>(smem)));
   dim3 grid((a.M + BM - 1) / BM, a.CN / BN);
   B200OCL_PROF(a.transposed ? "conv_dgrad" : (a.mode == CONV_EVAL ? "conv_eval" : "conv_train"), 2.0 * a.M * (double)a.CN * a.CK * a.ks * a.ks, stream);
   conv_kernel<BN, PT><<<grid, CONV_THREADS, smem, stream>>>(a);

@@ -70,6 +70,11 @@ __device__ __forceinline__ void bn_finalize(const ConvArgs& a, int c, double S, 
   a.run_var[c] = bn_running_update(a.run_var[c], (float)unbiased, a.momentum);
 }
 
+// conv_tcp.cu stages 128 + 2 * (W + 2) + 2 strip rows per tile, TP_LD_MAX per patch-loader thread (16 rows per pass):
+// maps up to W = 37 wide.  The network plan builds halo-strip weight images exactly for the maps that fit.
+constexpr int TP_LD_MAX = 13;
+inline bool tcp_strip_fits(int W) { return 128 + 2 * (W + 2) + 2 <= 16 * TP_LD_MAX; }
+
 // Upper bound of gridDim.x over every tiling launch_conv may choose (sizes stat_part).
 int conv_max_grid_m(int M);
 int launch_conv(const ConvArgs& a, cudaStream_t stream);   // CK, CN multiples of 20

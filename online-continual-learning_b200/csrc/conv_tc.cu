@@ -26,11 +26,6 @@ namespace {
 constexpr int TC_THREADS = 128;
 constexpr int A_TILE = 128 * 32;  // floats
 
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
-  const unsigned int s = static_cast<unsigned int>(__cvta_generic_to_shared(smem_dst));
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem_src));
-}
-
 // acc += tmp for one 64-row half of the tile (fragment layout of umma.cuh)
 template <int R>
 __device__ __forceinline__ void promote(float (&acc)[R], const float (&tmp)[R]) {
@@ -104,7 +99,7 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(ConvArgs a) {
 #pragma unroll
     for (int i = 0; i < (2 * B_TILE / 4) / TC_THREADS; ++i)
       cp_async16(sB + (tid + i * TC_THREADS) * 4, bsrc + (tid + i * TC_THREADS) * 4);
-    asm volatile("cp.async.commit_group;\n" ::);
+    cp_async_commit();
     // ---- A: gather this pixel's 8 chunks (all loads first, then split + store)
     float4 v[8];
 #pragma unroll
@@ -127,7 +122,7 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(ConvArgs a) {
       *reinterpret_cast<float4*>(sAh + off) = h;
       *reinterpret_cast<float4*>(sAl + off) = l;
     }
-    asm volatile("cp.async.wait_group 0;\n" ::);
+    cp_async_wait<0>();
     umma::fence_proxy_async_smem();
     __syncthreads();
     // ---- promote the previous K block (its MMAs ran while this block was staged), then issue this one
@@ -267,12 +262,7 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(ConvArgs a) {
 template <int NT>
 int launch_tc(const ConvArgs& a, cudaStream_t stream) {
   constexpr size_t smem = (size_t)2 * (2 * A_TILE + 2 * NT * 32) * sizeof(float) + 1024;
-  static bool configured_dev[B200OCL_MAX_DEVICES] = {};
-  bool& configured = configured_dev[b200ocl::device_slot()];
-  if (!configured) {
-    B200OCL_CUDA(cudaFuncSetAttribute(conv_tc_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = true;
-  }
+  B200OCL_CUDA(raise_smem_limit<conv_tc_kernel<NT>>(smem));
   dim3 grid((a.M + 127) / 128, a.CN / a.tc_bn);
   B200OCL_PROF(a.flip ? "conv_tc_dgrad" : (a.mode == CONV_EVAL ? "conv_tc_eval" : "conv_tc_train"),
                2.0 * a.M * (double)a.CN * a.CK * 9.0, stream);

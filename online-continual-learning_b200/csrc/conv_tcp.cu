@@ -42,7 +42,6 @@ constexpr int TP_THREADS = 32 * 13;
 constexpr int TP_LOADER_WARP = 9;                   // first patch-loader warp; warp 8 loads the weights
 constexpr int TP_PS_MAX = 3;                        // patch stages: 3 when shared memory allows, else 2
 constexpr int TP_BS_MAX = 6;                        // weight ring depth (streaming mode): 6 or 4
-constexpr int TP_LD_MAX = 13;                       // patch rows a loader thread stages per tile (16 rows per pass)
 constexpr int TP_CONSUMER_WARPS = 8;                // arrivals that release a patch stage or a weight slot
 
 using umma::mbar_expect_tx;
@@ -351,12 +350,7 @@ int launch_tcp(ConvArgs a, cudaStream_t stream) {
   if (tcp_smem_bytes<NT>(G, a.tp_slices, a.tp_ps, a.tp_bs) > limit) a.tp_bs = 4;
   if (tcp_smem_bytes<NT>(G, a.tp_slices, a.tp_ps, a.tp_bs) > limit) { a.tp_ps = 2; a.tp_bs = 6; }
   const size_t smem = tcp_smem_bytes<NT>(G, a.tp_slices, a.tp_ps, a.tp_bs);
-  static size_t configured_dev[B200OCL_MAX_DEVICES] = {};
-  size_t& configured = configured_dev[b200ocl::device_slot()];
-  if (smem > configured) {
-    B200OCL_CUDA(cudaFuncSetAttribute(conv_tcp_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = smem;
-  }
+  B200OCL_CUDA(raise_smem_limit<conv_tcp_kernel<NT>>(smem));
   a.tp_tiles = G.tiles_m;
   const int n_tiles = a.CN / a.tp_bn;
   int gx = sm_count() / n_tiles;
@@ -381,7 +375,7 @@ bool conv_tcp_eligible(const ConvArgs& a) {
   // the fp32 bar of the drop-in comparison (tests/test_gpu_dropin.py).
   if (a.mode == CONV_TRAIN || !a.w_tp || a.transposed || a.CK % 4 != 0) return false;
   if (a.ks != 3 || a.pad != 1 || a.stride != 1 || a.Hout != a.Hin || a.Wout != a.Win) return false;
-  if (128 + 2 * (a.Win + 2) + 2 > 16 * TP_LD_MAX) return false;   // strip rows one stage holds (W <= 37)
+  if (!tcp_strip_fits(a.Win)) return false;
   if ((long)a.N * (a.Hin + 2) * (a.Win + 2) > 2000000000L) return false;
   if (a.tp_bn <= 0 || a.tp_bn > 40 || a.CN % a.tp_bn != 0) return false;
   return true;

@@ -386,12 +386,7 @@ int launch_knn(const KnnSvParams& p0, cudaStream_t stream) {
   p.n_tiles = (p.E + TE - 1) / TE;
   int grid = p.n_tiles < knn_grid_cap() ? p.n_tiles : knn_grid_cap();
   if (grid < 1) grid = 1;
-  static bool configured_dev[B200OCL_MAX_DEVICES] = {};
-  bool& configured = configured_dev[b200ocl::device_slot()];
-  if (!configured) {
-    B200OCL_CUDA(cudaFuncSetAttribute(knn_sv_kernel<KPL, TE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = true;
-  }
+  B200OCL_CUDA((raise_smem_limit<knn_sv_kernel<KPL, TE>>(smem)));
   B200OCL_PROF("knn_sv", 4.0 * p.d * ((double)p.E + p.C) + 8.0 * ((double)p.E + p.C) + 4.0 * p.C * 3 + (p.sv ? 4.0 * p.E * p.C : 0.0), stream);
   knn_sv_kernel<KPL, TE><<<grid, KNN_THREADS, smem, stream>>>(p);
   B200OCL_LAUNCHED();
@@ -462,12 +457,8 @@ int b200ocl_knn_sv(const float* eval_f, const int64_t* eval_y, const float* cand
   p.E = E; p.C = C; p.d = d; p.k = k;
   p.sv = sv; p.col_sum = col_sum; p.col_max = col_max; p.col_min = col_min;
   if (want_red) {
-    if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) ||
-        workspace_bytes < b200ocl_knn_sv_workspace_bytes(E, C, d)) {
-      set_error("b200ocl_knn_sv: workspace missing, misaligned or smaller than %zu bytes",
-                b200ocl_knn_sv_workspace_bytes(E, C, d));
-      return B200OCL_EWORKSPACE;
-    }
+    const int rc = check_workspace("b200ocl_knn_sv", workspace, workspace_bytes, b200ocl_knn_sv_workspace_bytes(E, C, d));
+    if (rc) return rc;
     p.counter = static_cast<unsigned int*>(workspace);
     p.part = reinterpret_cast<float*>(static_cast<unsigned char*>(workspace) + 256);
     B200OCL_CUDA(cudaMemsetAsync(p.counter, 0, sizeof(unsigned int), stream));

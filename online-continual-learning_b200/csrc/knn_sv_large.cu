@@ -235,10 +235,8 @@ int launch_knn_large(const float* eval_f, const long long* eval_y, const float* 
     set_error("b200ocl_knn_sv: d=%d exceeds %d on the large-candidate path", d, KL_MAX_D);
     return B200OCL_EUNSUPPORTED;
   }
-  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) || workspace_bytes < knn_large_workspace_bytes(C)) {
-    set_error("b200ocl_knn_sv: workspace missing, misaligned or smaller than %zu bytes", knn_large_workspace_bytes(C));
-    return B200OCL_EWORKSPACE;
-  }
+  const int rc = check_workspace("b200ocl_knn_sv", workspace, workspace_bytes, knn_large_workspace_bytes(C));
+  if (rc) return rc;
   KnnLargeParams p{};
   p.eval_f = eval_f; p.eval_y = eval_y; p.cand_f = cand_f; p.cand_y = cand_y;
   p.E = E; p.C = C; p.Cpad = knn_large_cpad(C); p.d = d; p.k = k;
@@ -251,12 +249,7 @@ int launch_knn_large(const float* eval_f, const long long* eval_y, const float* 
   B200OCL_CUDA(cudaMemsetAsync(p.counter, 0, sizeof(unsigned int), stream));
   const int S = p.Cpad < KL_S ? p.Cpad : KL_S;
   const size_t smem = (size_t)S * sizeof(unsigned long long) + (size_t)(d + KL_THREADS) * sizeof(float);
-  static bool configured_dev[B200OCL_MAX_DEVICES] = {};
-  bool& configured = configured_dev[device_slot()];
-  if (!configured) {
-    B200OCL_CUDA(cudaFuncSetAttribute(knn_sv_large_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    configured = true;
-  }
+  B200OCL_CUDA(raise_smem_limit<knn_sv_large_kernel>(200 * 1024));
   const int grid = E < grid_cap ? E : grid_cap;
   B200OCL_PROF("knn_sv", 4.0 * d * ((double)E + C) + 8.0 * ((double)E + C) + 4.0 * C * 3 + (sv ? 4.0 * E * C : 0.0), stream);
   knn_sv_large_kernel<<<grid, KL_THREADS, smem, stream>>>(p);

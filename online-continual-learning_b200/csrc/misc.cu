@@ -337,12 +337,7 @@ int b200ocl_stream_prepare(const uint8_t* src_hwc, const int64_t* perm, int n, i
   const size_t row = (size_t)h * w * 3;
   B200OCL_CHECK_ARG(row % 4 == 0 && (reinterpret_cast<uintptr_t>(src_hwc) & 3) == 0, "image rows must be 4-byte aligned");
   B200OCL_CHECK_ARG(row <= 200 * 1024, "image larger than shared memory");
-  static bool configured_dev[B200OCL_MAX_DEVICES] = {};
-  bool& configured = configured_dev[device_slot()];
-  if (!configured) {
-    B200OCL_CUDA(cudaFuncSetAttribute(stream_prepare_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    configured = true;
-  }
+  B200OCL_CUDA(raise_smem_limit<stream_prepare_kernel>(200 * 1024));
   B200OCL_PROF("stream_prepare", 5.0 * n * (double)row, stream);
   stream_prepare_kernel<<<n, 256, row, stream>>>(src_hwc, reinterpret_cast<const long long*>(perm), dst_chw, h * w);
   B200OCL_LAUNCHED();
@@ -357,10 +352,8 @@ int b200ocl_agem_project(const float* g, const float* g_ref, float* out, size_t 
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (n == 0) return B200OCL_OK;
   B200OCL_CHECK_ARG(g && g_ref && out, "null pointer");
-  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) || workspace_bytes < b200ocl_agem_project_workspace_bytes()) {
-    set_error("b200ocl_agem_project: workspace missing, misaligned or smaller than %zu bytes", b200ocl_agem_project_workspace_bytes());
-    return B200OCL_EWORKSPACE;
-  }
+  const int rc = check_workspace("b200ocl_agem_project", workspace, workspace_bytes, b200ocl_agem_project_workspace_bytes());
+  if (rc) return rc;
   int grid = 2 * sm_count();
   if (grid > 296) grid = 296;
   double* part = static_cast<double*>(workspace);
@@ -384,10 +377,8 @@ int b200ocl_grad_cosine(const float* mem_grads, const float* g, int K, size_t n,
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200OCL_CHECK_ARG(K >= 1 && K <= GC_MAX_K && n >= 1, "need 1 <= K <= 64 and n >= 1");
   B200OCL_CHECK_ARG(mem_grads && g && (cos_out || max_out), "null pointer");
-  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) || workspace_bytes < b200ocl_grad_cosine_workspace_bytes(K)) {
-    set_error("b200ocl_grad_cosine: workspace missing, misaligned or smaller than %zu bytes", b200ocl_grad_cosine_workspace_bytes(K));
-    return B200OCL_EWORKSPACE;
-  }
+  const int rc = check_workspace("b200ocl_grad_cosine", workspace, workspace_bytes, b200ocl_grad_cosine_workspace_bytes(K));
+  if (rc) return rc;
   int grid = 2 * sm_count();
   if (grid > 296) grid = 296;
   double* part = static_cast<double*>(workspace);

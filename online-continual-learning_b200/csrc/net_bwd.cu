@@ -19,15 +19,6 @@
 namespace b200ocl {
 namespace {
 
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src, int src_bytes) {
-  const unsigned int s = static_cast<unsigned int>(__cvta_generic_to_shared(smem_dst));
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem_src), "r"(src_bytes));
-}
-__device__ __forceinline__ void cp_async_commit_wait_all() {
-  asm volatile("cp.async.commit_group;\n" ::);
-  asm volatile("cp.async.wait_group 0;\n" ::);
-}
-
 // ----------------------------------------------------------------------------- BN backward
 struct BnBwdArgs {
   const float* dA;     // gradient w.r.t. the activated output, NHWC [M][C]
@@ -327,43 +318,17 @@ __global__ void __launch_bounds__(256, 1) bn_bwd_fused_kernel(BnBwdArgs a) {
 }
 
 int launch_bn_bwd(BnBwdArgs a, cudaStream_t stream) {
-  {
-    // fused path: rows split evenly over at most one CTA per SM, all of a CTA's rows resident in shared memory
-    const int cols = a.C / 4;
-    const int R = 256 / cols;
-    const int sms = sm_count();
-    int rows = (a.M + sms - 1) / sms;
-    if (rows < 4 * R) rows = 4 * R;
-    rows = (rows + R - 1) / R * R;
-    const int grid = (a.M + rows - 1) / rows;
-    const int groups = 256 / a.C > 0 ? 256 / a.C : 1;
-    const int srows = R > groups ? R : groups;
-    const size_t smem = (size_t)srows * a.C * 2 * sizeof(double) + (size_t)rows * a.C * 2 * sizeof(float);
-    if (a.ready && grid <= sms && smem <= 200 * 1024 &&
-        (size_t)grid * a.C * 2 * sizeof(double) <= (size_t)bn_bwd_part_capacity(a.M, a.C, sms)) {
-      static bool configured_dev[B200OCL_MAX_DEVICES] = {};
-      bool& configured = configured_dev[device_slot()];
-      if (!configured) {
-        B200OCL_CUDA(cudaFuncSetAttribute(bn_bwd_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        configured = true;
-      }
-      a.rows_per_cta = rows;
-      B200OCL_PROF("bn_bwd", (a.amask ? 16.0 : 12.0) * a.M * a.C + (a.gout ? 4.0 * a.M * a.C : 0.0), stream);
-      bn_bwd_fused_kernel<<<grid, 256, smem, stream>>>(a);
-      B200OCL_LAUNCHED();
-      return B200OCL_OK;
-    }
+  const BnBwdGeom g = bn_bwd_geom(a.M, a.C, sm_count(), a.ready != nullptr);
+  a.rows_per_cta = g.rows;
+  if (g.fused) {
+    B200OCL_CUDA(raise_smem_limit<bn_bwd_fused_kernel>(200 * 1024));
+    B200OCL_PROF("bn_bwd", (a.amask ? 16.0 : 12.0) * a.M * a.C + (a.gout ? 4.0 * a.M * a.C : 0.0), stream);
+    bn_bwd_fused_kernel<<<g.grid, 256, g.smem, stream>>>(a);
+    B200OCL_LAUNCHED();
+    return B200OCL_OK;
   }
-  const int cols = a.C / 4;
-  const int R = 256 / cols;
-  const int rows = bn_bwd_rows_per_cta(a.M, a.C, sm_count());
-  a.rows_per_cta = rows;
-  const int grid = (a.M + rows - 1) / rows;
-  const int groups = 256 / a.C > 0 ? 256 / a.C : 1;
-  const int srows = R > groups ? R : groups;
-  const size_t smem = (size_t)srows * a.C * 2 * sizeof(double);
   B200OCL_PROF("bn_bwd", (a.amask ? 12.0 : 8.0) * a.M * a.C, stream);
-  bn_bwd_reduce_kernel<<<grid, 256, smem, stream>>>(a);
+  bn_bwd_reduce_kernel<<<g.grid, 256, g.smem, stream>>>(a);
   B200OCL_LAUNCHED();
   size_t blocks = ((size_t)a.M * a.C / 4 + 255) / 256;
   const size_t cap = (size_t)16 * sm_count();
@@ -476,14 +441,14 @@ __global__ void __launch_bounds__(128, 3) wgrad_kernel(WgradArgs a) {
 #pragma unroll
   for (int st = 0; st < WG_NST - 1; ++st) {
     if (st < nch) gather(st);
-    asm volatile("cp.async.commit_group;\n" ::);
+    cp_async_commit();
   }
   for (int c = 0; c < nch; ++c) {
-    asm volatile("cp.async.wait_group %0;\n" ::"n"(WG_NST - 2));
+    cp_async_wait<WG_NST - 2>();
     __syncthreads();
     rowinfo(c + WG_NST);                       // consumed by the gather of the NEXT iteration
     if (c + WG_NST - 1 < nch) gather(c + WG_NST - 1);
-    asm volatile("cp.async.commit_group;\n" ::);
+    cp_async_commit();
     const float* pA = sbuf + (c % WG_NST) * stage_f + kwi * 128 + lane * 4;
     const float* pG = sbuf + (c % WG_NST) * stage_f + WG_MC * KS + nwi * 20;
 #pragma unroll 4
@@ -502,7 +467,7 @@ __global__ void __launch_bounds__(128, 3) wgrad_kernel(WgradArgs a) {
       }
     }
   }
-  asm volatile("cp.async.wait_group 0;\n" ::);
+  cp_async_wait<0>();
   const int g4 = g4_base + kwi * 32 + lane;
   const int co = co_base + nwi * 20;
   if (g4 < a.k4_groups && co < a.Cout) {
@@ -521,7 +486,7 @@ __global__ void __launch_bounds__(128, 3) wgrad_kernel(WgradArgs a) {
 // staged in shared memory (coalesced), then 225 threads = 5 pixel slices x (9 taps x 5 channel quads)
 // accumulate 3 ci x 4 co each; the slices meet in shared memory in fixed order and the CTA writes one
 // partial [27][20].
-constexpr int SW_PX = 128, SW_LD = SW_PX + 4, SW_SLICES = 5;
+constexpr int SW_LD = SW_PX + 4, SW_SLICES = 5;   // SW_PX: net_ws.cuh
 
 __global__ void __launch_bounds__(256) stem_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dz,
                                                          float* __restrict__ part, int N, int H, int W, int M,
@@ -819,11 +784,8 @@ extern "C" int b200ocl_net_backward(const b200ocl_net_desc* desc, const b200ocl_
     return rc;
   }
   B200OCL_CHECK_ARG(N >= 1 && dout && x, "need N >= 1, x and dout");
-  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) ||
-      workspace_bytes < b200ocl_net_train_workspace_bytes(desc, N)) {
-    set_error("b200ocl_net_backward: workspace missing, misaligned or too small");
-    return B200OCL_EWORKSPACE;
-  }
+  if ((rc = check_workspace("b200ocl_net_backward", workspace, workspace_bytes,
+                            b200ocl_net_train_workspace_bytes(desc, N)))) return rc;
   const int eval_stats = (accumulate >> 1) & 1;   // bit 1 of `accumulate`: backward of b200ocl_net_forward_evalgrad
   accumulate &= 1;
   const int sms = sm_count();
@@ -888,22 +850,28 @@ extern "C" int b200ocl_net_backward(const b200ocl_net_desc* desc, const b200ocl_
   };
   auto wgrad_on = [&](int ci, const float* x, const float* dz, cudaStream_t stream) -> int {
     const ConvL& c = p.conv[ci];
-    {
-      // 3x3 stride-1 layers on 4..32-wide maps: wgmma with the activation read in place from a strip (wgrad_tc.cu)
-      const WgradTcCfg tg = wgrad_tc_cfg(N, c.hin, c.win, c.ks, c.stride, c.pad, c.cin, c.cout, sms);
-      if (tg.eligible) {
-        WgradTcArgs ta{};
-        ta.x = x; ta.dz = dz;
-        ta.part = w.wg_part + w.wg_off[ci];
-        ta.N = N; ta.H = c.hin; ta.W = c.win; ta.Cin = c.cin; ta.Cout = c.cout;
-        ta.tpc = tg.tpc; ta.chains = tg.chains; ta.chains_per_cta = tg.chains_per_cta;
-        return launch_wgrad_tc(ta, tg, stream);
-      }
+    const WgradPlan wp = wgrad_plan(p, ci, N, sms);
+    float* part = w.wg_part + w.wg_off[ci];
+    if (wp.kernel == WGRAD_STEM) {
+      const int M = N * p.in_h * p.in_w;
+      B200OCL_PROF("wgrad", 2.0 * M * 540.0, stream);
+      stem_wgrad_kernel<<<wp.splits, 256, 0, stream>>>(x, dz, part, N, p.in_h, p.in_w, M, wp.stem_ppc);
+      B200OCL_LAUNCHED();
+      return B200OCL_OK;
     }
-    const WgradCfg g = wgrad_cfg(c, N, sms);
+    if (wp.kernel == WGRAD_TC) {
+      const WgradTcCfg& tg = wp.tc;
+      WgradTcArgs ta{};
+      ta.x = x; ta.dz = dz;
+      ta.part = part;
+      ta.N = N; ta.H = c.hin; ta.W = c.win; ta.Cin = c.cin; ta.Cout = c.cout;
+      ta.tpc = tg.tpc; ta.chains = tg.chains; ta.chains_per_cta = tg.chains_per_cta;
+      return launch_wgrad_tc(ta, tg, stream);
+    }
+    const WgradCfg& g = wp.fp32;
     WgradArgs a{};
     a.x = x; a.dz = dz;
-    a.part = w.wg_part + w.wg_off[ci];
+    a.part = part;
     a.N = N; a.Hin = c.hin; a.Win = c.win; a.Cin = c.cin;
     a.Hout = c.hout; a.Wout = c.wout; a.Cout = c.cout;
     a.ks = c.ks; a.stride = c.stride; a.pad = c.pad;
@@ -912,47 +880,15 @@ extern "C" int b200ocl_net_backward(const b200ocl_net_desc* desc, const b200ocl_
     a.pix_per_split = g.pix_per_split;
     const size_t smem = (size_t)WG_NST * WG_MC * (g.kw * 128 + g.nw * 20) * sizeof(float) +
                         (size_t)(WG_NST + 1) * 3 * WG_MC * sizeof(int);
-    static bool configured_dev[B200OCL_MAX_DEVICES] = {};
-  bool& configured = configured_dev[b200ocl::device_slot()];
-    if (!configured) {
-      B200OCL_CUDA(cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-      configured = true;
-    }
+    B200OCL_CUDA(raise_smem_limit<wgrad_kernel>(64 * 1024));
     B200OCL_PROF("wgrad", 2.0 * a.M * (double)a.k_total * a.Cout, stream);
     wgrad_kernel<<<dim3(g.grid_k, g.grid_n, g.splits), 32 * g.kw * g.nw, smem, stream>>>(a);
     B200OCL_LAUNCHED();
     return B200OCL_OK;
   };
   auto dgrad = [&](int ci, const float* dz, float* dx, int accum) -> int {
-    const ConvL& c = p.conv[ci];
-    ConvArgs a{};
-    a.in = dz;
-    a.w = st->packed + c.pkd_off;
-    a.out = dx;
-    a.N = N;
-    a.Hin = c.hout; a.Win = c.wout; a.CK = c.cout;
-    a.Hout = c.hin; a.Wout = c.win; a.CN = c.cin;
-    a.ks = c.ks; a.stride = c.stride; a.pad = c.pad;
-    a.M = N * c.hin * c.win;
+    ConvArgs a = conv_layer_args(p.conv[ci], N, dz, st->packed, dx, true);
     a.mode = accum ? CONV_ACCUM : CONV_RAW;
-    if (c.stride == 1) {
-      // dx[h,w] = sum_taps dz[h+1-kh, w+1-kw] W[kh,kw]: a forward-style correlation with flipped taps
-      a.transposed = 0;
-      a.flip = 1;
-      if (c.tc_kb_d) {
-        a.w_tc = st->packed + c.tc_d_off;
-        a.tc_kb = c.tc_kb_d;
-        a.tc_bn = c.tc_bn_d;
-      }
-      if (c.tp_sl_d) {
-        a.w_tp = st->packed + c.tp_d_off;
-        a.tp_bn = c.tp_bn_d;
-        a.tp_slices = c.tp_sl_d;
-      }
-    } else {
-      a.transposed = 1;
-      a.parity_order = (c.stride == 2 && c.hin % 2 == 0 && c.win % 2 == 0) ? 1 : 0;
-    }
     return launch_conv(a, stream);
   };
 
@@ -1017,41 +953,27 @@ extern "C" int b200ocl_net_backward(const b200ocl_net_desc* desc, const b200ocl_
   // stem
   if (!(dz = next_dz())) return B200OCL_ECUDA;
   if ((rc = bn_backward(0, g0, w.a + (size_t)N * p.conv[0].act_off, dz, nullptr))) return rc;
-  {
-    const int M = N * p.in_h * p.in_w;
-    int ctas = (M + SW_PX - 1) / SW_PX;
-    if (ctas > 2 * sms) ctas = 2 * sms;
-    const int ppc = ((M + ctas - 1) / ctas + SW_PX - 1) / SW_PX * SW_PX;
-    const int grid = (M + ppc - 1) / ppc;
-    B200OCL_PROF("wgrad", 2.0 * M * 540.0, stream);
-    stem_wgrad_kernel<<<grid, 256, 0, stream>>>(x, dz, w.wg_part + w.wg_off[0], N, p.in_h, p.in_w, M, ppc);
-    B200OCL_LAUNCHED();
-    if ((rc = join_side())) return rc;            // every weight-gradient partial is in place
-    WgFinalTable t{};
-    t.n = p.n_conv;
-    unsigned int blocks = 0;
-    for (int i = 0; i < p.n_conv; ++i) {
-      auto& e = t.e[i];
-      e.part_off = w.wg_off[i];
-      e.w_off = (unsigned)p.conv[i].w_off;
-      e.cin = p.conv[i].cin;
-      e.cout = p.conv[i].cout;
-      e.taps = p.conv[i].ks * p.conv[i].ks;
-      e.splits = (i == 0) ? grid : wgrad_cfg(p.conv[i], N, sms).splits;
-      if (i > 0) {
-        const ConvL& ci_ = p.conv[i];
-        const WgradTcCfg tg = wgrad_tc_cfg(N, ci_.hin, ci_.win, ci_.ks, ci_.stride, ci_.pad, ci_.cin, ci_.cout, sms);
-        if (tg.eligible) e.splits = tg.chains;
-      }
-      e.sg_log2 = e.splits >= 256 ? 5 : (e.splits >= 64 ? 4 : (e.splits >= 16 ? 3 : 2));
-      e.blk_start = blocks;
-      const int epb = 256 >> e.sg_log2;
-      blocks += (unsigned)((e.cin * e.taps * e.cout + epb - 1) / epb);
-    }
-    t.n_blocks = blocks;
-    B200OCL_PROF("wgrad_finalize", 8.0 * p.n_packed / 2, stream);
-    wgrad_finalize_kernel<<<blocks, 256, 0, stream>>>(t, w.wg_part, st->grads, accumulate);
-    B200OCL_LAUNCHED();
+  if ((rc = wgrad_on(0, x, dz, stream))) return rc;   // on the caller stream: nothing is left to overlap it with
+  if ((rc = join_side())) return rc;                   // every weight-gradient partial is in place
+  WgFinalTable t{};
+  t.n = p.n_conv;
+  unsigned int blocks = 0;
+  for (int i = 0; i < p.n_conv; ++i) {
+    auto& e = t.e[i];
+    e.part_off = w.wg_off[i];
+    e.w_off = (unsigned)p.conv[i].w_off;
+    e.cin = p.conv[i].cin;
+    e.cout = p.conv[i].cout;
+    e.taps = p.conv[i].ks * p.conv[i].ks;
+    e.splits = wgrad_plan(p, i, N, sms).splits;
+    e.sg_log2 = e.splits >= 256 ? 5 : (e.splits >= 64 ? 4 : (e.splits >= 16 ? 3 : 2));
+    e.blk_start = blocks;
+    const int epb = 256 >> e.sg_log2;
+    blocks += (unsigned)((e.cin * e.taps * e.cout + epb - 1) / epb);
   }
+  t.n_blocks = blocks;
+  B200OCL_PROF("wgrad_finalize", 8.0 * p.n_packed / 2, stream);
+  wgrad_finalize_kernel<<<blocks, 256, 0, stream>>>(t, w.wg_part, st->grads, accumulate);
+  B200OCL_LAUNCHED();
   return B200OCL_OK;
 }

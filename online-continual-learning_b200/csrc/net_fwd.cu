@@ -519,37 +519,13 @@ __global__ void __launch_bounds__(256) cls_loss_kernel(ClsLossArgs a) {
 }
 
 // ----------------------------------------------------------------------------- orchestration
-void fill_conv_common(ConvArgs& a, const ConvL& c, int N, const float* in, const float* packed, float* out) {
-  a = ConvArgs{};
-  a.in = in;
-  a.w = packed + c.pkf_off;
-  a.out = out;
-  a.N = N;
-  a.Hin = c.hin; a.Win = c.win; a.CK = c.cin;
-  a.Hout = c.hout; a.Wout = c.wout; a.CN = c.cout;
-  a.ks = c.ks; a.stride = c.stride; a.pad = c.pad;
-  a.transposed = 0;
-  a.M = N * c.hout * c.wout;
-  a.eps = NET_BN_EPS;
-  a.momentum = NET_BN_MOMENTUM;
-  if (c.tc_kb_f) {
-    a.w_tc = packed + c.tc_f_off;
-    a.tc_kb = c.tc_kb_f;
-    a.tc_bn = c.tc_bn_f;
-  }
-  if (c.tp_sl_f) {
-    a.w_tp = packed + c.tp_f_off;
-    a.tp_bn = c.tp_bn_f;
-    a.tp_slices = c.tp_sl_f;
-  }
-}
-
 int conv_eval(const NetPlan& p, const b200ocl_net_state& st, int ci, int N, const float* in, float* out,
               const float* residual, int relu, cudaStream_t stream) {
-  ConvArgs a;
-  fill_conv_common(a, p.conv[ci], N, in, st.packed, out);
+  ConvArgs a = conv_layer_args(p.conv[ci], N, in, st.packed, out, false);
   const BnL& b = p.bn[ci];
   a.mode = CONV_EVAL;
+  a.eps = NET_BN_EPS;
+  a.momentum = NET_BN_MOMENTUM;
   a.gamma = st.params + b.g_off;
   a.beta = st.params + b.b_off;
   a.rmean = st.bn_stats + b.stat_off;
@@ -584,11 +560,12 @@ enum { STATS_RUNNING = 0, STATS_EVAL = 1, STATS_DEFER = 2 };
 int conv_train(const NetPlan& p, const b200ocl_net_state& st, const TrainWs& w, int ci, int N, const float* in,
                cudaStream_t stream, int stats = STATS_RUNNING) {
   const bool eval_stats = stats == STATS_EVAL;
-  ConvArgs a;
   const ConvL& c = p.conv[ci];
-  fill_conv_common(a, c, N, in, st.packed, w.z + (size_t)N * c.act_off);
+  ConvArgs a = conv_layer_args(c, N, in, st.packed, w.z + (size_t)N * c.act_off, false);
   const BnL& b = p.bn[ci];
   a.mode = CONV_TRAIN;
+  a.eps = NET_BN_EPS;
+  a.momentum = NET_BN_MOMENTUM;
   a.stat_part = w.stat_part;
   a.counter = w.counters + 8 * ci;   // up to 8 channel tiles per conv (160 = 8 x 20)
   a.save_mean = w.save + b.save_off;
@@ -788,15 +765,7 @@ int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N
   unsigned int* counters = reinterpret_cast<unsigned int*>(reinterpret_cast<unsigned char*>(stat_part) + align_up(stat, 256));
   int rc = launch_pack(p, w_oihw, packed, stream);
   if (rc) return rc;
-  const ConvL& c = p.conv[0];
-  ConvArgs a{};
-  a.in = x;
-  a.out = out;
-  a.N = N;
-  a.Hin = H; a.Win = W;
-  a.Hout = c.hout; a.Wout = c.wout;
-  a.ks = ks; a.stride = stride; a.pad = c.pad;
-  a.M = N * c.hout * c.wout;
+  ConvArgs a = conv_layer_args(p.conv[0], N, x, packed, out, dgrad);
   a.mode = mode == 2 ? CONV_TRAIN : (mode == 1 ? CONV_ACCUM : CONV_RAW);
   a.force_path = path;
   a.eps = NET_BN_EPS;
@@ -810,18 +779,6 @@ int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N
     a.save_invstd = stats_out + cout;
     a.run_mean = stats_out + 2 * cout;
     a.run_var = stats_out + 3 * cout;
-  }
-  if (!dgrad) {
-    a.CK = cin; a.CN = cout;
-    a.w = packed + c.pkf_off;
-    if (c.tc_kb_f) { a.w_tc = packed + c.tc_f_off; a.tc_kb = c.tc_kb_f; a.tc_bn = c.tc_bn_f; }
-    if (c.tp_sl_f) { a.w_tp = packed + c.tp_f_off; a.tp_bn = c.tp_bn_f; a.tp_slices = c.tp_sl_f; }
-  } else {
-    a.CK = cout; a.CN = cin;
-    a.w = packed + c.pkd_off;
-    a.flip = 1;
-    if (c.tc_kb_d) { a.w_tc = packed + c.tc_d_off; a.tc_kb = c.tc_kb_d; a.tc_bn = c.tc_bn_d; }
-    if (c.tp_sl_d) { a.w_tp = packed + c.tp_d_off; a.tp_bn = c.tp_bn_d; a.tp_slices = c.tp_sl_d; }
   }
   return launch_conv(a, stream);
 }
@@ -869,11 +826,8 @@ int b200ocl_net_features_eval(const b200ocl_net_desc* desc, const b200ocl_net_st
   B200OCL_CHECK_ARG(N >= 0, "negative batch");
   if (N == 0) return B200OCL_OK;
   B200OCL_CHECK_ARG(x && feat, "null pointer");
-  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) ||
-      workspace_bytes < b200ocl_net_eval_workspace_bytes(desc, N)) {
-    set_error("b200ocl_net_features_eval: workspace missing, misaligned or too small");
-    return B200OCL_EWORKSPACE;
-  }
+  if ((rc = check_workspace("b200ocl_net_features_eval", workspace, workspace_bytes,
+                            b200ocl_net_eval_workspace_bytes(desc, N)))) return rc;
   EvalWs w = eval_ws(p, N, workspace);
   float* cur = w.buf[0];
   float* t1 = w.buf[1];
@@ -914,11 +868,8 @@ static int net_forward_impl(const b200ocl_net_desc* desc, const b200ocl_net_stat
   int rc = check_state(desc, st, p);
   if (rc) return rc;
   B200OCL_CHECK_ARG(N >= 1 && x && out, "need N >= 1 and non-null x/out");
-  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) ||
-      workspace_bytes < b200ocl_net_train_workspace_bytes(desc, N)) {
-    set_error("b200ocl_net_forward_train: workspace missing, misaligned or too small");
-    return B200OCL_EWORKSPACE;
-  }
+  if ((rc = check_workspace("b200ocl_net_forward_train", workspace, workspace_bytes,
+                            b200ocl_net_train_workspace_bytes(desc, N)))) return rc;
   TrainWs w = train_ws(p, N, workspace, sm_count());
   B200OCL_CUDA(cudaMemsetAsync(w.counters, 0, NET_COUNTERS * sizeof(unsigned int), stream));
   if (ev == STATS_DEFER) B200OCL_CUDA(cudaMemsetAsync(w.run_defer, 0, p.n_stats * sizeof(float), stream));
@@ -975,11 +926,8 @@ int b200ocl_net_apply_running_stats(const b200ocl_net_desc* desc, const b200ocl_
   int rc = check_state(desc, st, p);
   if (rc) return rc;
   B200OCL_CHECK_ARG(N >= 1, "need N >= 1");
-  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) ||
-      workspace_bytes < b200ocl_net_train_workspace_bytes(desc, N)) {
-    set_error("b200ocl_net_apply_running_stats: workspace missing, misaligned or too small");
-    return B200OCL_EWORKSPACE;
-  }
+  if ((rc = check_workspace("b200ocl_net_apply_running_stats", workspace, workspace_bytes,
+                            b200ocl_net_train_workspace_bytes(desc, N)))) return rc;
   TrainWs w = train_ws(p, N, workspace, sm_count());
   const int n = (int)p.n_stats;
   B200OCL_PROF("misc", 12.0 * n, stream);

@@ -12,6 +12,7 @@
 #include <string.h>
 
 #include "../../include/b200ocl.h"
+#include "conv.cuh"
 
 namespace b200ocl {
 
@@ -78,7 +79,7 @@ inline int conv_out(int x, int ks, int stride, int pad) { return (x + 2 * pad - 
 
 // Packed-arena layout of one convolution (kernel-side weight copies); c.cin/cout/ks/stride/hin/win set.
 inline void conv_pack_layout(ConvL& c, size_t& pk) {
-  const int cin = c.cin, cout = c.cout, ks = c.ks, stride = c.stride, hin = c.hin, win = c.win;
+  const int cin = c.cin, cout = c.cout, ks = c.ks, stride = c.stride, win = c.win;
   c.pkf_off = pk; pk += (size_t)cout * cin * ks * ks;
   c.pkd_off = pk; pk += (size_t)cout * cin * ks * ks;
   c.tc_kb_f = c.tc_kb_d = c.tp_sl_f = c.tp_sl_d = 0;
@@ -90,8 +91,8 @@ inline void conv_pack_layout(ConvL& c, size_t& pk) {
     c.tc_f_off = pk; pk += (size_t)(cout / c.tc_bn_f) * c.tc_kb_f * 2 * tc_nt(c.tc_bn_f) * 32;
     c.tc_d_off = pk; pk += (size_t)(cin / c.tc_bn_d) * c.tc_kb_d * 2 * tc_nt(c.tc_bn_d) * 32;
   }
-  // conv_tcp.cu: images for the 3x3 stride-1 convolutions on maps with W <= 37 (forward + data gradient)
-  if (ks == 3 && stride == 1 && c.pad == 1 && cin % 20 == 0 && win <= 37) {
+  // conv_tcp.cu: images for the 3x3 stride-1 convolutions on maps its strip holds (forward + data gradient)
+  if (ks == 3 && stride == 1 && c.pad == 1 && cin % 20 == 0 && tcp_strip_fits(win)) {
     c.tp_bn_f = cout < 40 ? cout : 40;
     c.tp_sl_f = (cin + 31) / 32;
     c.tp_f_off = pk; pk += (size_t)(cout / c.tp_bn_f) * c.tp_sl_f * 9 * 2 * tc_nt(c.tp_bn_f) * 32;
@@ -99,6 +100,39 @@ inline void conv_pack_layout(ConvL& c, size_t& pk) {
     c.tp_sl_d = (cout + 31) / 32;
     c.tp_d_off = pk; pk += (size_t)(cin / c.tp_bn_d) * c.tp_sl_d * 9 * 2 * tc_nt(c.tp_bn_d) * 32;
   }
+}
+
+// Argument block of layer c's forward (dgrad = false) or data-gradient launch over N images: geometry, the weight
+// images of `packed`, flip / transposed / parity_order.  The caller adds the mode and the BatchNorm fields.
+inline ConvArgs conv_layer_args(const ConvL& c, int N, const float* in, const float* packed, float* out, bool dgrad) {
+  ConvArgs a{};
+  a.in = in;
+  a.out = out;
+  a.N = N;
+  a.ks = c.ks; a.stride = c.stride; a.pad = c.pad;
+  if (!dgrad) {
+    a.w = packed + c.pkf_off;
+    a.Hin = c.hin; a.Win = c.win; a.CK = c.cin;
+    a.Hout = c.hout; a.Wout = c.wout; a.CN = c.cout;
+    a.M = N * c.hout * c.wout;
+    if (c.tc_kb_f) { a.w_tc = packed + c.tc_f_off; a.tc_kb = c.tc_kb_f; a.tc_bn = c.tc_bn_f; }
+    if (c.tp_sl_f) { a.w_tp = packed + c.tp_f_off; a.tp_bn = c.tp_bn_f; a.tp_slices = c.tp_sl_f; }
+    return a;
+  }
+  a.w = packed + c.pkd_off;
+  a.Hin = c.hout; a.Win = c.wout; a.CK = c.cout;
+  a.Hout = c.hin; a.Wout = c.win; a.CN = c.cin;
+  a.M = N * c.hin * c.win;
+  if (c.stride == 1) {
+    // dx[h,w] = sum_taps dz[h+1-kh, w+1-kw] W[kh,kw]: a forward-style correlation with flipped taps
+    a.flip = 1;
+    if (c.tc_kb_d) { a.w_tc = packed + c.tc_d_off; a.tc_kb = c.tc_kb_d; a.tc_bn = c.tc_bn_d; }
+    if (c.tp_sl_d) { a.w_tp = packed + c.tp_d_off; a.tp_bn = c.tp_bn_d; a.tp_slices = c.tp_sl_d; }
+  } else {
+    a.transposed = 1;
+    a.parity_order = (c.stride == 2 && c.hin % 2 == 0 && c.win % 2 == 0) ? 1 : 0;
+  }
+  return a;
 }
 
 // Returns 0 on success, a B200OCL_E* code otherwise.

@@ -22,7 +22,7 @@ inline EvalWs eval_ws(const NetPlan& p, int N, void* base) {
   return w;
 }
 
-// Weight-gradient tiling of conv layer c (shared by the workspace sizing and the launcher).
+// Tiling of the fp32 weight-gradient kernel (wgrad_kernel, net_bwd.cu) over conv layer c.
 struct WgradCfg {
   int k_total;    // ks*ks*cin
   int k4_groups;  // k_total / 4
@@ -58,18 +58,79 @@ inline WgradCfg wgrad_cfg(const ConvL& c, int N, int sms) {
   return g;
 }
 
-// Grid of the BN-backward reduction over M pixels x C channels (shared by sizing and launch).
-inline int bn_bwd_rows_per_cta(int M, int C, int sms) {
-  const int R = 256 / (C / 4);
-  constexpr int per_sm = 2;   // CTAs per SM the row split aims for
-  int rows = (M + per_sm * sms - 1) / (per_sm * sms);
-  if (rows < 4 * R) rows = 4 * R;
-  return (rows + R - 1) / R * R;
+constexpr int SW_PX = 128;   // pixels per chunk of the stem weight-gradient kernel (stem_wgrad_kernel, net_bwd.cu)
+
+// Which kernel computes the weight gradient of conv layer ci, with what configuration, and how many partials it writes.
+// The workspace sizing (train_ws), the launch and the finalize table of b200ocl_net_backward all read it.
+enum WgradKernel { WGRAD_STEM, WGRAD_TC, WGRAD_FP32 };
+struct WgradPlan {
+  WgradKernel kernel;
+  WgradTcCfg tc;      // WGRAD_TC (wgrad_tc.cu)
+  WgradCfg fp32;      // WGRAD_FP32 (wgrad_kernel)
+  int stem_ppc;       // WGRAD_STEM: pixels per CTA
+  int splits;         // partials of [ks*ks*cin][cout] floats the kernel writes; the finalize sums exactly these
+};
+
+inline WgradPlan wgrad_plan(const NetPlan& p, int ci, int N, int sms) {
+  WgradPlan w{};
+  const ConvL& c = p.conv[ci];
+  if (ci == 0) {
+    // one partial per CTA, at most two CTAs per SM
+    w.kernel = WGRAD_STEM;
+    const int M = N * p.in_h * p.in_w;
+    int ctas = (M + SW_PX - 1) / SW_PX;
+    if (ctas > 2 * sms) ctas = 2 * sms;
+    w.stem_ppc = ((M + ctas - 1) / ctas + SW_PX - 1) / SW_PX * SW_PX;
+    w.splits = (M + w.stem_ppc - 1) / w.stem_ppc;
+    return w;
+  }
+  // 3x3 stride-1 layers on maps the strip holds: wgmma with the activation read in place from a strip
+  w.tc = wgrad_tc_cfg(N, c.hin, c.win, c.ks, c.stride, c.pad, c.cin, c.cout, sms);
+  if (w.tc.eligible) {
+    w.kernel = WGRAD_TC;
+    w.splits = w.tc.chains;
+    return w;
+  }
+  w.kernel = WGRAD_FP32;
+  w.fp32 = wgrad_cfg(c, N, sms);
+  w.splits = w.fp32.splits;
+  return w;
 }
-// bytes of BN-backward partials the workspace holds for a layer (the fused kernel's grid must fit as well)
-inline size_t bn_bwd_part_capacity(int M, int C, int sms) {
-  const int rows = bn_bwd_rows_per_cta(M, C, sms);
-  return (size_t)((M + rows - 1) / rows) * C * 2 * sizeof(double);
+
+// Launch geometry of the BN backward over M pixels x C channels (launch_bn_bwd, net_bwd.cu).  With fused_ok (the
+// caller has a ready counter) it is the fused kernel when its grid is co-resident (at most one CTA per SM) and its
+// rows fit in shared memory; otherwise the two-phase reduce + apply.  The fused rows are split over sms CTAs, the
+// two-phase rows over 2 * sms, so the fused rows are never fewer and its grid never larger: the two-phase grid
+// bounds the partials either path writes (train_ws).
+struct BnBwdGeom {
+  bool fused;
+  int rows;       // rows per CTA, a multiple of the rows a CTA covers per pass
+  int grid;
+  size_t smem;    // dynamic shared memory of the fused or the reduce kernel
+};
+
+inline BnBwdGeom bn_bwd_geom(int M, int C, int sms, bool fused_ok) {
+  const int R = 256 / (C / 4);                     // rows per pass: 256 threads over C / 4 float4 columns
+  const int groups = 256 / C > 0 ? 256 / C : 1;    // thread groups of the final reduction
+  const size_t sred = (size_t)(R > groups ? R : groups) * C * 2 * sizeof(double);
+  auto split = [&](int ctas) {
+    int rows = (M + ctas - 1) / ctas;
+    if (rows < 4 * R) rows = 4 * R;
+    return (rows + R - 1) / R * R;
+  };
+  BnBwdGeom g{};
+  if (fused_ok) {
+    g.rows = split(sms);
+    g.grid = (M + g.rows - 1) / g.rows;
+    g.smem = sred + (size_t)g.rows * C * 2 * sizeof(float);   // all of a CTA's rows stay resident
+    g.fused = g.grid <= sms && g.smem <= 200 * 1024;
+    if (g.fused) return g;
+  }
+  constexpr int per_sm = 2;   // CTAs per SM the two-phase row split aims for
+  g.rows = split(per_sm * sms);
+  g.grid = (M + g.rows - 1) / g.rows;
+  g.smem = sred;
+  return g;
 }
 constexpr int NET_COEF_DOUBLES = 512;  // 3 x 160 floats of BN-backward coefficients fit in front of the partials
 
@@ -112,8 +173,8 @@ inline TrainWs train_ws(const NetPlan& p, int N, void* base, int sms) {
     const size_t M = (size_t)N * p.conv[i].hout * p.conv[i].wout;
     const size_t s = (size_t)conv_max_grid_m((int)M) * p.conv[i].cout * 2 * sizeof(double);
     if (s > stat_max) stat_max = s;
-    const int rows = bn_bwd_rows_per_cta((int)M, p.conv[i].cout, sms);
-    const size_t sb = ((M + rows - 1) / rows * p.conv[i].cout * 2 + NET_COEF_DOUBLES) * sizeof(double);
+    const int grid = bn_bwd_geom((int)M, p.conv[i].cout, sms, false).grid;
+    const size_t sb = ((size_t)grid * p.conv[i].cout * 2 + NET_COEF_DOUBLES) * sizeof(double);
     if (sb > stat_max) stat_max = sb;
   }
   w.stat_part = reinterpret_cast<double*>(take(stat_max));
@@ -136,16 +197,9 @@ inline TrainWs train_ws(const NetPlan& p, int N, void* base, int sms) {
   w.dproj = reinterpret_cast<float*>(take((size_t)N * p.out_dim * sizeof(float)));
   size_t wg = 0;
   for (int i = 0; i < p.n_conv; ++i) {
+    const ConvL& c = p.conv[i];
     w.wg_off[i] = wg;
-    if (i == 0) {
-      wg += (size_t)(8 * sms) * 27 * 20;  // stem: one partial per CTA
-    } else {
-      const WgradCfg g = wgrad_cfg(p.conv[i], N, sms);
-      const ConvL& c = p.conv[i];
-      const WgradTcCfg tg = wgrad_tc_cfg(N, c.hin, c.win, c.ks, c.stride, c.pad, c.cin, c.cout, sms);   // wgrad_tc.cu
-      const int splits = (tg.eligible && tg.chains > g.splits) ? tg.chains : g.splits;
-      wg += (size_t)splits * g.k_total * p.conv[i].cout;
-    }
+    wg += (size_t)wgrad_plan(p, i, N, sms).splits * c.ks * c.ks * c.cin * c.cout;
   }
   w.wg_part = reinterpret_cast<float*>(take(wg * sizeof(float)));
   w.bytes = off;

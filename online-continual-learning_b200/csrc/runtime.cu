@@ -20,6 +20,12 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
+int check_workspace(const char* entry, const void* ws, size_t ws_bytes, size_t need) {
+  if (ws && !(reinterpret_cast<uintptr_t>(ws) & 255) && ws_bytes >= need) return B200OCL_OK;
+  set_error("%s: workspace missing, misaligned or smaller than %zu bytes", entry, need);
+  return B200OCL_EWORKSPACE;
+}
+
 bool g_prof_on = false;
 namespace {
 struct ProfRec {

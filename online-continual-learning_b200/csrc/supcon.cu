@@ -519,12 +519,7 @@ template <int RM, int RN, int NC, bool RES>
 int launch_fused(SupconParams p, cudaStream_t stream) {
   constexpr int TM = 16 * RM;
   const size_t smem = fused_smem_bytes<RM, RN, NC, RES>(p.A, p.d);
-  static bool configured_dev[B200OCL_MAX_DEVICES] = {};
-  bool& configured = configured_dev[device_slot()];
-  if (!configured) {
-    B200OCL_CUDA(cudaFuncSetAttribute(supcon_fused_kernel<RM, RN, NC, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    configured = true;
-  }
+  B200OCL_CUDA((raise_smem_limit<supcon_fused_kernel<RM, RN, NC, RES>>(227 * 1024)));
   p.n_units = (p.A + TM - 1) / TM;
   // the grid-wide wait needs every CTA resident: one CTA per SM
   int per_sm = 0;
@@ -574,12 +569,8 @@ int b200ocl_supcon(const float* feats, const int64_t* labels, int B, int V, int 
     set_error("b200ocl_supcon: d=%d exceeds the kernel's limit of 1024", d);
     return B200OCL_EUNSUPPORTED;
   }
-  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) ||
-      workspace_bytes < b200ocl_supcon_workspace_bytes(B, V, d)) {
-    set_error("b200ocl_supcon: workspace missing, misaligned or smaller than %zu bytes",
-              b200ocl_supcon_workspace_bytes(B, V, d));
-    return B200OCL_EWORKSPACE;
-  }
+  const int rc = check_workspace("b200ocl_supcon", workspace, workspace_bytes, b200ocl_supcon_workspace_bytes(B, V, d));
+  if (rc) return rc;
   SupconParams p{};
   p.feats = feats;
   p.labels = reinterpret_cast<const long long*>(labels);
@@ -607,17 +598,9 @@ int b200ocl_supcon(const float* feats, const int64_t* labels, int B, int V, int 
     // the 4 x 4 register tile with the least shared-memory traffic per FMA is used.
     return launch_fused_nc<4, 4, false>(p, stream);
   }
-  static bool configured_dev[B200OCL_MAX_DEVICES] = {};
-  bool& configured = configured_dev[b200ocl::device_slot()];
-  if (!configured) {
-    const int max_smem = 200 * 1024;  // d = 1024 needs 165 KB; static smem takes a little of the 227 KB
-    B200OCL_CUDA(cudaFuncSetAttribute(supcon_stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200OCL_CUDA(cudaFuncSetAttribute(supcon_grad_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200OCL_CUDA(cudaFuncSetAttribute(supcon_grad_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200OCL_CUDA(cudaFuncSetAttribute(supcon_grad_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    B200OCL_CUDA(cudaFuncSetAttribute(supcon_grad_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    configured = true;
-  }
+  // d = 1024 needs 165 KB; static smem takes a little of the 227 KB
+  B200OCL_CUDA((raise_smem_limit<supcon_stats_kernel, supcon_grad_kernel<4>, supcon_grad_kernel<8>, supcon_grad_kernel<16>,
+                                 supcon_grad_kernel<32>>(200 * 1024)));
   B200OCL_PROF("supcon", 4.0 * p.A * d + 8.0 * B + 8.0 * p.A, stream);
   supcon_stats_kernel<<<grid, SC_THREADS, smem_stats, stream>>>(p);
   B200OCL_LAUNCHED();

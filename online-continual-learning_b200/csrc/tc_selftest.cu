@@ -139,7 +139,7 @@ extern "C" int b200ocl_selftest_umma_window(const float* P, const float* B, floa
                         start_row + 15 * sbo_rows + 8 <= rows,
                     "window exceeds the patch");
   const size_t smem = (size_t)((rows + 7) / 8 * 8 + 256) * 32 * sizeof(float) + 1024;
-  B200OCL_CUDA(cudaFuncSetAttribute(wgmma_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  B200OCL_CUDA(raise_smem_limit<wgmma_window_kernel>(smem));
   B200OCL_CUDA(cudaMemsetAsync(status, 0, sizeof(int), stream));
   wgmma_window_kernel<<<1, 128, smem, stream>>>(P, B, D, rows, start_row, sbo_rows, base_off_mode, N);
   B200OCL_LAUNCHED();

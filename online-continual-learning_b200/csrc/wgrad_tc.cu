@@ -33,7 +33,6 @@ namespace {
 
 constexpr int WT_THREADS = 32 * 14;
 constexpr int WT_PS = 2;
-constexpr int WT_LD_MAX = 13;             // x rows a loader thread stages per tile (16 rows per pass)
 constexpr int WT_XP = 40;                 // floats per x row in shared memory (32 channels + 8: conflict-free fragments)
 constexpr int WT_DZ_BYTES = 128 * 128;    // one dz half (hi or lo) of a tile: 4 K-major [32 co][32 positions] tiles
 
@@ -267,12 +266,7 @@ __global__ void wgrad_tc_reduce_kernel(const float* __restrict__ part, int chain
 int launch_wgrad_tc(const WgradTcArgs& a, const WgradTcCfg& g, cudaStream_t stream) {
   const WtGeom G = wt_geom(a.H, a.W);
   const size_t smem = (size_t)WT_PS * (2 * WT_DZ_BYTES + (size_t)G.xbytes) + 1024;
-  static size_t configured_dev[B200OCL_MAX_DEVICES] = {};
-  size_t& configured = configured_dev[device_slot()];
-  if (smem > configured) {
-    B200OCL_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = smem;
-  }
+  B200OCL_CUDA(raise_smem_limit<wgrad_tc_kernel>(smem));
   const double M = (double)a.N * a.H * a.W;
   B200OCL_PROF("wgrad_tc", 2.0 * M * 9.0 * a.Cin * a.Cout, stream);
   wgrad_tc_kernel<<<dim3(g.ctas_x, g.slices, g.cout_blocks), WT_THREADS, smem, stream>>>(a, g.tiles);
@@ -300,17 +294,14 @@ extern "C" int b200ocl_wgrad_tc_selftest(const float* x, const float* dz, float*
     set_error("b200ocl_wgrad_tc_selftest: geometry not covered (3x3 stride 1, W <= 37, channels %% 4 == 0)");
     return B200OCL_EUNSUPPORTED;
   }
-  if (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 255) ||
-      workspace_bytes < b200ocl_wgrad_tc_selftest_workspace_bytes(N, H, W, cin, cout)) {
-    set_error("b200ocl_wgrad_tc_selftest: workspace missing, misaligned or too small");
-    return B200OCL_EWORKSPACE;
-  }
+  int rc = check_workspace("b200ocl_wgrad_tc_selftest", workspace, workspace_bytes,
+                           b200ocl_wgrad_tc_selftest_workspace_bytes(N, H, W, cin, cout));
+  if (rc) return rc;
   WgradTcArgs a{};
   a.x = x; a.dz = dz; a.part = static_cast<float*>(workspace);
   a.N = N; a.H = H; a.W = W; a.Cin = cin; a.Cout = cout;
   a.tpc = g.tpc; a.chains = g.chains; a.chains_per_cta = g.chains_per_cta;
-  const int rc = launch_wgrad_tc(a, g, stream);
-  if (rc) return rc;
+  if ((rc = launch_wgrad_tc(a, g, stream))) return rc;
   const int total = 9 * cin * cout;
   wgrad_tc_reduce_kernel<<<(total + 255) / 256, 256, 0, stream>>>(a.part, g.chains, cin, cout, dw_oihw);
   B200OCL_LAUNCHED();

@@ -1,9 +1,12 @@
-// wgrad_tc.cuh -- weight gradient of a 3x3 stride-1 convolution on wgmma (wgrad_tc.cu): configuration shared by the
-// workspace sizing (net_ws.cuh), the launcher and the backward driver (net_bwd.cu).
+// wgrad_tc.cuh -- weight gradient of a 3x3 stride-1 convolution on wgmma (wgrad_tc.cu): its configuration, which the
+// network's weight-gradient plan (wgrad_plan, net_ws.cuh) and the self-test read.
 #pragma once
 #include <cuda_runtime.h>
 
 namespace b200ocl {
+
+// x rows a wgrad_tc loader thread stages per tile (16 rows per pass): bounds the strip of 128 + 2 * (W + 2) + 2 rows
+constexpr int WT_LD_MAX = 13;
 
 struct WgradTcCfg {
   int eligible;        // geometry covered (3x3, stride 1, pad 1, W <= 37, channels % 4 == 0)
@@ -25,7 +28,7 @@ inline int wgrad_tc_tiles(int N, int H, int W) {
 inline WgradTcCfg wgrad_tc_cfg(int N, int H, int W, int ks, int stride, int pad, int cin, int cout, int sms) {
   WgradTcCfg g{};
   g.eligible = (ks == 3 && stride == 1 && pad == 1 && cin % 4 == 0 && cout % 4 == 0 && cin >= 4 && cout >= 4 &&
-                128 + 2 * (W + 2) + 2 <= 16 * 13 && (long)N * (H + 2) * (W + 2) < 2000000000L) ? 1 : 0;
+                128 + 2 * (W + 2) + 2 <= 16 * WT_LD_MAX && (long)N * (H + 2) * (W + 2) < 2000000000L) ? 1 : 0;
   if (!g.eligible) return g;
   g.slices = (cin + 31) / 32;
   g.cout_blocks = (cout + 31) / 32;

@@ -54,7 +54,7 @@ def test_weight_gradient_workspace_query_follows_the_kernel_geometry():
 
 def test_train_workspace_grows_with_the_batch():
     """Host-only: b200ocl_net_train_workspace_bytes is monotonic in N and covers the partial buffers of both weight-gradient
-    kernels (the larger of the two split counts per layer)."""
+    kernels (the split count of the kernel each layer runs)."""
     from b200ocl import engine
     import ctypes
     from b200ocl import _native
