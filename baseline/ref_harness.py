@@ -120,6 +120,8 @@ def make_params(kind, **over):
         base.update(agent='SCR', retrieve='ASER', update='ASER', eps_mem_batch=100)
     elif kind == 'lwf':
         base.update(agent='LWF', retrieve='random', update='random', eps_mem_batch=10)
+    elif kind == 'icarl':
+        base.update(agent='ICARL', retrieve='random', update='random', eps_mem_batch=10)
     else:
         raise ValueError(kind)
     base.update(over)

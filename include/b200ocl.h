@@ -256,6 +256,19 @@ int b200ocl_cls_loss(const float* logits, const int64_t* labels, int N, int C, i
                      int n_cols, int n_old, const int64_t* pos_table, int table_len, const float* teacher, float w_ce,
                      float w_kd, float* loss, float* dlogits, int64_t* n_correct, int* err_flag, void* stream);
 
+/* iCaRL's criterion (agents/icarl.py:42-62) over logits [N,C] in one launch:
+ *   loss[1] = (1/N) sum_i sum_{j<K} [max(z,0) - z*t + log1p(exp(-|z|))]   (BCE with logits, summed over the K columns,
+ *   averaged over the rows), dlogits [N,C] = (sigmoid(z) - t)/N for j < K and 0 for j >= K (nullable).
+ * Targets t: rows i < n_stream are the stream batch, one-hot at pos_table[labels[i]] (pos_len entries, the
+ * lbl_inv_map of this task); rows i >= n_stream are the memory rows, target 0; in the columns j < n_old the target is
+ * sigmoid(teacher[i,j]) for every row (teacher [N,C], the previous model's logits; NULL only when n_old == 0).
+ * Needs 0 <= n_old <= K <= C, K >= 1 and 0 <= n_stream <= N.  A stream label outside the table, or whose position lies
+ * outside [n_old, K), sets *err_flag = 1 (nullable, never cleared) and its row adds nothing to the loss or gradient.
+ * One CTA, fixed-order sums, no atomics: repeated launches are bit-identical. */
+int b200ocl_icarl_loss(const float* logits, const float* teacher, const int64_t* labels, const int64_t* pos_table,
+                       int pos_len, int N, int n_stream, int C, int K, int n_old, float* loss, float* dlogits,
+                       int* err_flag, void* stream);
+
 /* ---------------------------------------------------------------- SCR augmentation
  * The second view of agents/scr.py:18-24,54 (kornia RandomResizedCrop -> RandomHorizontalFlip ->
  * ColorJitter -> RandomGrayscale) in one kernel over NCHW fp32 images in [0,1].

@@ -48,6 +48,7 @@ SIGNATURES = {
     'b200ocl_ce_loss': (c_int, [P, P, c_int, c_int, P, P, P, P, P]),
     'b200ocl_cls_loss': (c_int, [P, P, c_int, c_int, c_int, P, c_int, c_int, P, c_int, P, c_float, c_float, P, P, P, P,
                                  P]),
+    'b200ocl_icarl_loss': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, P, P, P, P]),
     'b200ocl_scr_augment': (c_int, [P, P, P, c_int, c_int, c_int, P]),
     'b200ocl_aser_replace': (c_int, [P, c_int, c_int, P, P, P, c_int, c_size_t, P, P, P, P]),
     'b200ocl_conv_selftest_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int, c_int]),

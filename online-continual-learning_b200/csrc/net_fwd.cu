@@ -518,6 +518,67 @@ __global__ void __launch_bounds__(256) cls_loss_kernel(ClsLossArgs a) {
   }
 }
 
+// ----------------------------------------------------------------------------- iCaRL's criterion
+// F.binary_cross_entropy_with_logits(logits[:, :K], target, reduction='none').sum(1).mean() of agents/icarl.py:42-62
+// and its gradient.  The target is one-hot at the label's position for the stream rows and zero for the memory rows,
+// with the teacher's sigmoids in the first n_old columns of every row.  Like ce_kernel: one CTA, a fixed assignment of
+// rows to warps and fixed-order sums, so repeated launches give identical bits.
+struct IcarlLossArgs {
+  const float* logits;
+  const float* teacher;      // previous model's logits [N,C]; nullable when n_old == 0
+  const long long* labels;   // [n_stream]
+  const long long* pos;      // label -> position (lbl_inv_map), -1 where unmapped
+  int n_pos, N, n_stream, C, K, n_old;
+  float* loss;
+  float* dlogits;
+  int* err;
+};
+
+__device__ __forceinline__ float sigmoid_f(float z) { return 1.f / (1.f + expf(-z)); }
+
+__global__ void __launch_bounds__(256) icarl_loss_kernel(IcarlLossArgs a) {
+  __shared__ float s_loss[8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int C = a.C, K = a.K, n_old = a.n_old;
+  const float invN = 1.f / (float)a.N;
+  float lsum = 0.f;
+  for (int n = warp; n < a.N; n += 8) {
+    const float* lr = a.logits + (size_t)n * C;
+    const float* tr = a.teacher ? a.teacher + (size_t)n * C : nullptr;
+    float* dr = a.dlogits ? a.dlogits + (size_t)n * C : nullptr;
+    int p = -1;                          // the one-hot column; memory rows have none
+    if (n < a.n_stream) {
+      const long long y = a.labels[n];
+      const long long q = (y >= 0 && y < a.n_pos) ? a.pos[y] : -1;
+      if (q < n_old || q >= K) {         // not a label of this task (icarl.py:44 raises); the row adds nothing
+        if (lane == 0 && a.err) *a.err = 1;
+        if (dr)
+          for (int c = lane; c < C; c += 32) dr[c] = 0.f;
+        continue;
+      }
+      p = (int)q;
+    }
+    // max(z,0) - z*t + log1p(exp(-|z|)): finite for any finite z
+    float s = 0.f;
+    for (int c = lane; c < K; c += 32) {
+      const float z = __ldg(lr + c);
+      const float t = c < n_old ? sigmoid_f(__ldg(tr + c)) : (c == p ? 1.f : 0.f);
+      s += fmaxf(z, 0.f) - z * t + log1pf(expf(-fabsf(z)));
+      if (dr) dr[c] = (sigmoid_f(z) - t) * invN;
+    }
+    if (dr)
+      for (int c = K + lane; c < C; c += 32) dr[c] = 0.f;
+    lsum += warp_sum(s);
+  }
+  if (lane == 0) s_loss[warp] = lsum;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int w = 0; w < 8; ++w) t += s_loss[w];
+    if (a.loss) *a.loss = t / (float)a.N;
+  }
+}
+
 // ----------------------------------------------------------------------------- orchestration
 int conv_eval(const NetPlan& p, const b200ocl_net_state& st, int ci, int N, const float* in, float* out,
               const float* residual, int relu, cudaStream_t stream) {
@@ -970,6 +1031,26 @@ int b200ocl_cls_loss(const float* logits, const int64_t* labels, int N, int C, i
   const size_t smem = mode == B200OCL_CLS_LABELS ? (size_t)C * sizeof(int) : 0;
   B200OCL_PROF("cls_loss", (teacher ? 12.0 : 8.0) * N * C, stream);
   cls_loss_kernel<<<1, 256, smem, stream>>>(a);
+  B200OCL_LAUNCHED();
+  return B200OCL_OK;
+}
+
+int b200ocl_icarl_loss(const float* logits, const float* teacher, const int64_t* labels, const int64_t* pos_table,
+                       int pos_len, int N, int n_stream, int C, int K, int n_old, float* loss, float* dlogits,
+                       int* err_flag, void* stream_) {
+  using namespace b200ocl;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200OCL_CHECK_ARG(logits && N >= 1 && C >= 1, "need logits, N >= 1, C >= 1");
+  B200OCL_CHECK_ARG(n_stream >= 0 && n_stream <= N, "need 0 <= n_stream <= N");
+  B200OCL_CHECK_ARG(n_stream == 0 || (labels && pos_table && pos_len >= 0), "stream rows need labels and a position table");
+  B200OCL_CHECK_ARG(K >= 1 && K <= C, "need 1 <= K <= C");
+  B200OCL_CHECK_ARG(n_old >= 0 && n_old <= K, "need 0 <= n_old <= K");
+  B200OCL_CHECK_ARG(teacher || n_old == 0, "n_old > 0 needs the teacher's logits");
+  IcarlLossArgs a{logits, teacher, reinterpret_cast<const long long*>(labels),
+                  reinterpret_cast<const long long*>(pos_table), pos_len, N, n_stream, C, K, n_old, loss, dlogits,
+                  err_flag};
+  B200OCL_PROF("icarl_loss", 4.0 * N * (K + n_old) + (dlogits ? 4.0 * N * C : 0.0), stream);
+  icarl_loss_kernel<<<1, 256, 0, stream>>>(a);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }

@@ -405,3 +405,28 @@ def cls_loss(logits, labels, mode='ce', cols=None, n_old=0, pos_table=None, teac
                                  out['loss'].data_ptr(), ptr(out['dlogits']), ptr(out['n_correct']), ptr(err), _stream())
     _native.check(rc, 'b200ocl_cls_loss')
     return out
+
+
+def icarl_loss(logits, labels, pos_table, K, n_old, teacher=None, err=None, want_grad=True):
+    """iCaRL's criterion (b200ocl_icarl_loss, agents/icarl.py:42-62): BCE with logits over the first K columns, summed
+    over the columns and averaged over the N rows; returns dict(loss[1], dlogits).  The first labels.numel() rows are the
+    stream batch (one-hot at pos_table[label], the int64 device table of lbl_inv_map, -1 unmapped), the rest are memory
+    rows (zero target).  teacher: the previous model's logits; their sigmoids are the targets of the first n_old columns
+    (None needs n_old == 0).  err: int32 device flag [1] set to 1 by a label whose position is not in [n_old, K)."""
+    _need_cuda(logits, labels, pos_table, teacher, err)
+    logits = logits.detach().to(torch.float32).contiguous()
+    labels = labels.detach().to(torch.int64).contiguous()
+    pos_table = pos_table.to(torch.int64).contiguous()
+    n, c = logits.shape
+    if teacher is not None:
+        teacher = teacher.detach().to(torch.float32).contiguous()
+        if teacher.shape != logits.shape:
+            raise ValueError('teacher logits must match the logits in shape')
+    out = {'loss': torch.empty(1, dtype=torch.float32, device=logits.device)}
+    out['dlogits'] = torch.empty_like(logits) if want_grad else None
+    ptr = lambda t: 0 if t is None else t.data_ptr()
+    rc = _lib().b200ocl_icarl_loss(logits.data_ptr(), ptr(teacher), labels.data_ptr(), pos_table.data_ptr(),
+                                   pos_table.numel(), n, labels.numel(), c, int(K), int(n_old), out['loss'].data_ptr(),
+                                   ptr(out['dlogits']), ptr(err), _stream())
+    _native.check(rc, 'b200ocl_icarl_loss')
+    return out

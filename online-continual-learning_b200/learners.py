@@ -1,8 +1,8 @@
 """Agents of the replay path with the reference surface `cls(model, opt, params)`,
 `.train_learner(x_train, y_train)`, `.evaluate(test_loaders)`:
 ExperienceReplay (agents/exp_replay.py:10-104: ER / MIR / ASER), SupContrastReplay (agents/scr.py:11-69), AGEM
-(agents/agem.py) and Lwf (agents/lwf.py), over ContinualLearner (agents/base.py:14-113) with its training tricks
-(labels trick, separated softmax, kd_trick / kd_trick_star, review trick).
+(agents/agem.py), Lwf (agents/lwf.py) and Icarl (agents/icarl.py), over ContinualLearner (agents/base.py:14-113) with
+its training tricks (labels trick, separated softmax, kd_trick / kd_trick_star, review trick).
 
 The loop structure, the order of train-mode forwards (they move BN running statistics) and the
 order of buffer operations follow the reference step exactly; what changes is who does the
@@ -15,16 +15,16 @@ import torch
 
 from . import memory, ops
 from .augment import SCRTransform
-from .engine import ce_loss, cls_loss
+from .engine import ce_loss, cls_loss, icarl_loss
 from .memory import Buffer, input_size_match
 from .nets import adopt, engine_of, EngineModel
 
 
 # The train-mode passes of one replay step only interact through the BatchNorm running statistics and the gradient arena.
 # With this switch on (default; B200OCL_CONCURRENT=0 turns it off) independent passes are issued on two streams -- SCR's two
-# views (forward and backward), the memory / combined forwards of the ASER branch -- with deferred statistics applied in the
-# reference's order and the second backward pass into a second gradient arena: most launches of this network fill a
-# fraction of the GPU (tools/overlap_probe.py times the overlap).
+# views (forward and backward), the memory / combined forwards of the ASER branch, iCaRL's teacher and student forwards --
+# with deferred statistics applied in the reference's order and the second backward pass into a second gradient arena:
+# most launches of this network fill a fraction of the GPU (tools/overlap_probe.py times the overlap).
 import os as _os
 _CONCURRENT = _os.environ.get('B200OCL_CONCURRENT', '1') != '0'
 
@@ -599,5 +599,98 @@ class Lwf(ContinualLearner):
                 if i % 100 == 1 and self.verbose:
                     print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
                           .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
+        self._raise_label_errors()
+        self.after_train()
+
+
+class Icarl(ContinualLearner):
+    """iCaRL (agents/icarl.py:15-65) on the engine.  Per batch of B stream rows: from the second task on, B memory rows
+    drawn uniformly from the slots this train_learner call has not written yet are appended; one train-mode forward of
+    the student and, with a previous model, one of the teacher arena (the reference's deep copy, taken at the end of
+    each call before after_train and its review trick, so it holds the pre-review weights); BCE with logits against
+    one-hot targets whose first n_old columns are the teacher's sigmoids (one fused kernel, b200ocl_icarl_loss); one
+    backward pass and one SGD step; then the reservoir update, whose written slots are excluded from the later draws of
+    the call.  Evaluation is the inherited nearest-class-mean path."""
+
+    def __init__(self, model, opt, params):
+        if params.update != 'random':
+            # icarl.py:65 extends a list with what buffer.update returns; only the reservoir returns its slots
+            raise NotImplementedError('iCaRL runs with the reservoir update (update=random), not %r' % params.update)
+        super().__init__(model, opt, params)
+        self.mem_size = params.mem_size
+        self.buffer = Buffer(model, params)
+        self._takes_teacher = False      # the previous model is taken in train_learner; kd_trick's teacher is never read
+        self._prev_live = False
+        self._updated = np.zeros(params.mem_size, dtype=bool)   # icarl.py:35 updated_idx, as a mask over the slots
+        self._pos = None                 # (label -> position table on the device, n_old, K), one upload per task
+        # device flag: a stream label that is not one of this task's labels.  Kept apart from the criterion's _err:
+        # the reference fails here in list.index (ValueError, icarl.py:44), not in a dict lookup (KeyError, base.py:105)
+        self._pos_err = None
+
+    def _task_tables(self):
+        super()._task_tables()
+        if not self.new_labels:
+            return
+        _, n_old, pos = separated_softmax_table(self.old_labels, self.new_labels, self.lbl_inv_map)
+        self._pos = (torch.from_numpy(pos).to(self.device), n_old, n_old + len(self.new_labels))
+
+    def replay_step(self, batch_x, batch_y, batch_y_host, meters=None):
+        """One iteration of icarl.py:37-65."""
+        eng = self.engine
+        lr, wd = self._lr_wd()
+        pos, n_old, K = self._pos
+        B = batch_x.size(0)
+        if K > eng.out_dim:
+            # recurring labels count again in K = len(old_labels) + len(new_labels) (icarl.py:45,62 fail here)
+            raise ValueError('iCaRL: %d label positions exceed the %d logits' % (K, eng.out_dim))
+        if self._pos_err is None:
+            self._pos_err = torch.zeros(1, dtype=torch.int32, device=self.device)
+        teacher = None
+        if self._prev_live:
+            n = self.buffer.current_index
+            excl = np.flatnonzero(self._updated[:n])
+            if min(self.batch, n - excl.size) != B:
+                # icarl.py:52 pads the target with B zero rows whatever the retrieval returned
+                raise ValueError('iCaRL: %d memory rows can be drawn for a batch of %d (%d of %d filled slots were '
+                                 'written in this call)' % (n - excl.size, B, excl.size, n))
+            idx = memory.uniform_indices(n, self.batch, excl)                        # icarl.py:48-49
+            mem_x = ops.gather_rows(self.buffer.buffer_img, memory.to_device_i64(idx, self.device))
+            x = torch.cat((batch_x, mem_x))                                          # :51
+            if _CONCURRENT:
+                # the teacher's forward runs over its own arenas and workspace, side by side with the student's
+                main, side = self._fork()
+                with torch.cuda.stream(side):
+                    teacher = eng.teacher_forward(x)                                 # :58-59
+                logits, ws = eng.forward_train(x, slot=0)                            # :55
+                main.wait_stream(side)
+            else:
+                logits, ws = eng.forward_train(x, slot=0)
+                teacher = eng.teacher_forward(x)
+        else:
+            x = batch_x
+            logits, ws = eng.forward_train(x, slot=0)
+        out = icarl_loss(logits, batch_y, pos, K, n_old if teacher is not None else 0, teacher=teacher,
+                         err=self._pos_err)                                          # :43-62
+        eng.backward(x, out['dlogits'], ws)                                          # :63
+        self._optimizer_step(lr, wd)                                                 # :64
+        self.last_loss = out['loss']
+        slots = self.buffer.update(batch_x, batch_y, y_host=batch_y_host)            # :65
+        self._updated[np.asarray(slots, dtype=np.int64)] = True
+        self._throttle()
+
+    def train_learner(self, x_train, y_train):
+        self.before_train(x_train, y_train)
+        self.engine.pack()
+        self.model = self.model.train()
+        self._updated[:] = False                                                     # icarl.py:35, once per call
+        for ep in range(self.epoch):
+            stream = StreamFeeder(x_train, y_train, self.batch, self.device)
+            for batch_x, batch_y, y_host in stream:
+                self.replay_step(batch_x, batch_y, y_host)
+        if self._pos_err is not None and int(self._pos_err.item()):
+            self._pos_err.zero_()
+            raise ValueError("iCaRL trained on a label outside the task's labels (icarl.py:44 raises there)")
+        self.engine.update_teacher()                                                 # icarl.py:31, before after_train
+        self._prev_live = True
         self._raise_label_errors()
         self.after_train()

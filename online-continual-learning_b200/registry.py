@@ -9,7 +9,7 @@ already hold), so `general_main.py` runs unchanged:
 
 Every other agent / plugin of the reference stays registered and untouched.
 """
-from .learners import AGEM, ExperienceReplay, Lwf, SupContrastReplay
+from .learners import AGEM, ExperienceReplay, Icarl, Lwf, SupContrastReplay
 from .retrieve import ASER_retrieve, MIR_retrieve, Random_retrieve
 from .update import ASER_update, GSSGreedyUpdate, Reservoir_update
 
@@ -18,6 +18,7 @@ agents = {
     'SCR': SupContrastReplay,
     'AGEM': AGEM,
     'LWF': Lwf,
+    'ICARL': Icarl,
 }
 
 retrieve_methods = {
