@@ -122,6 +122,9 @@ def make_params(kind, **over):
         base.update(agent='LWF', retrieve='random', update='random', eps_mem_batch=10)
     elif kind == 'icarl':
         base.update(agent='ICARL', retrieve='random', update='random', eps_mem_batch=10)
+    elif kind == 'gdumb':      # config/agent/gdumb/gdumb_5k.yml
+        base.update(agent='GDUMB', retrieve='random', update='random', eps_mem_batch=10, mem_epoch=30, clip=10.0,
+                    minlr=0.0005)
     else:
         raise ValueError(kind)
     base.update(over)

@@ -227,6 +227,20 @@ int b200ocl_net_backward(const b200ocl_net_desc* desc, const b200ocl_net_state* 
 int b200ocl_net_sgd_step(const b200ocl_net_desc* desc, const b200ocl_net_state* st, float lr, float weight_decay,
                          const b200ocl_net_state* dst, void* stream);
 
+/* GDumb's step (agents/gdumb.py:82-83): torch.nn.utils.clip_grad_norm_(parameters, max_norm) then opt.step().
+ * Launch 1 takes the L2 norm of every tensor that has a gradient (the tensors b200ocl_net_sgd_step skips are left out)
+ * and the coefficient coef = min(max_norm / (norm + 1e-6), 1) in fp32, rounded as torch/nn/utils/clip_grad.py
+ * (_clip_grads_with_norm_) rounds it: the division is Tensor.__rdiv__, (norm + 1e-6).reciprocal() * max_norm.  The
+ * norm comes from per-CTA fp64 partials reduced in CTA order by the last CTA, no floating-point atomics, so repeated
+ * launches are bit-identical.  Launch 2 writes g * coef back to the gradient arena (torch scales
+ * .grad in place, and by coef = 1 too) and applies the SGD update of b200ocl_net_sgd_step with it; then `packed` is
+ * refreshed.  The coefficient stays on the device.  norm_out (nullable, device): the norm before clipping.  workspace:
+ * b200ocl_net_sgd_step_clipped_workspace_bytes(desc) bytes of device memory, no initial contents needed. */
+size_t b200ocl_net_sgd_step_clipped_workspace_bytes(const b200ocl_net_desc* desc);
+int b200ocl_net_sgd_step_clipped(const b200ocl_net_desc* desc, const b200ocl_net_state* st, float lr,
+                                 float weight_decay, float max_norm, float* norm_out, void* workspace,
+                                 size_t workspace_bytes, void* stream);
+
 /* Mean cross-entropy (agents/base.py:95,113) over logits [N,C], labels [N]:
  * loss[1]; per_sample [N] (F.cross_entropy(reduction='none'), mir_retrieve.py:26-27);
  * dlogits [N,C] = d(mean CE)/dlogits; n_correct[1] = #(argmax == label).  Each output nullable. */

@@ -45,6 +45,8 @@ SIGNATURES = {
     'b200ocl_net_apply_running_stats': (c_int, [P, P, c_int, P, c_size_t, P]),
     'b200ocl_net_backward': (c_int, [P, P, P, P, c_int, P, c_size_t, c_int, P]),
     'b200ocl_net_sgd_step': (c_int, [P, P, c_float, c_float, P, P]),
+    'b200ocl_net_sgd_step_clipped_workspace_bytes': (c_size_t, [P]),
+    'b200ocl_net_sgd_step_clipped': (c_int, [P, P, c_float, c_float, c_float, P, P, c_size_t, P]),
     'b200ocl_ce_loss': (c_int, [P, P, c_int, c_int, P, P, P, P, P]),
     'b200ocl_cls_loss': (c_int, [P, P, c_int, c_int, c_int, P, c_int, c_int, P, c_int, P, c_float, c_float, P, P, P, P,
                                  P]),

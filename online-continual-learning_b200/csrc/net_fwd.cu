@@ -191,10 +191,16 @@ int launch_pack(const NetPlan& p, const float* params, float* packed, cudaStream
 }
 
 // ----------------------------------------------------------------------------- SGD over the arena
+// CLIP: the gradient is first scaled by the clipping coefficient *coef (grad_norm_kernel) and the scaled value is
+// written back to the gradient arena through g_out (== g).  Each element is read and then written by one thread only,
+// so the read-only load of g cannot see a stale value.
+template <bool CLIP>
 __global__ void __launch_bounds__(256) net_sgd_kernel(const float* __restrict__ p, const float* __restrict__ g,
                                                       float* __restrict__ out, size_t n, float lr, float wd,
-                                                      size_t skip_lo, size_t skip_hi) {
+                                                      size_t skip_lo, size_t skip_hi, const float* coef, float* g_out) {
   const size_t stride = (size_t)gridDim.x * blockDim.x;
+  float c = 1.f;
+  if (CLIP) c = *coef;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const float w = p[i];
     if (i >= skip_lo && i < skip_hi) {  // tensors that never receive a gradient: torch skips them
@@ -202,8 +208,56 @@ __global__ void __launch_bounds__(256) net_sgd_kernel(const float* __restrict__ 
       continue;
     }
     float gi = g[i];
+    if (CLIP) {
+      gi = gi * c;                      // torch._foreach_mul_(grads, clip_coef_clamped)
+      g_out[i] = gi;
+    }
     if (wd != 0.f) gi = fmaf(wd, w, gi);
     out[i] = w - lr * gi;
+  }
+}
+
+// L2 norm of the gradient arena outside [skip_lo, skip_hi) and torch's clipping coefficient
+// (torch/nn/utils/clip_grad.py, _clip_grads_with_norm_): coef = min(max_norm / (norm + 1e-6), 1) in fp32, with torch's roundings.
+// Per-CTA fp64 partial sums of squares in a fixed order; the last CTA to arrive adds them in CTA order.
+constexpr int NORM_MAX_GRID = 1024;
+
+__global__ void __launch_bounds__(256) grad_norm_kernel(const float* __restrict__ g, size_t n, size_t skip_lo,
+                                                        size_t skip_hi, float max_norm, double* __restrict__ part,
+                                                        unsigned int* counter, float* coef, float* norm_out) {
+  __shared__ double s_red[8];
+  __shared__ bool is_last;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double acc = 0.0;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if (i >= skip_lo && i < skip_hi) continue;
+    const double v = (double)g[i];
+    acc = fma(v, v, acc);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(FULL_MASK, acc, o);
+  if (lane == 0) s_red[warp] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) t += s_red[w];
+    part[blockIdx.x] = t;
+    __threadfence();
+    is_last = (atomicAdd(counter, 1u) == gridDim.x - 1);
+  }
+  __syncthreads();
+  if (is_last && threadIdx.x == 0) {
+    __threadfence();
+    double t = 0.0;
+    for (unsigned int b = 0; b < gridDim.x; ++b) t += __ldcg(part + b);
+    const float norm = (float)sqrt(t);
+    // torch forms max_norm / (norm + 1e-6) as Tensor.__rdiv__: (norm + 1e-6).reciprocal() * max_norm, two roundings
+    const float q = __fmul_rn(__frcp_rn(norm + 1e-6f), max_norm);
+    *coef = q > 1.f ? 1.f : q;          // torch.clamp(max=1.0): a NaN norm stays NaN
+
+    if (norm_out) *norm_out = norm;
   }
 }
 
@@ -864,10 +918,55 @@ int b200ocl_net_sgd_step(const b200ocl_net_desc* desc, const b200ocl_net_state* 
   const size_t cap = (size_t)8 * sm_count();
   if (blocks > cap) blocks = cap;
   B200OCL_PROF("sgd", 12.0 * p.n_params, stream);
-  net_sgd_kernel<<<(unsigned)blocks, 256, 0, stream>>>(st->params, st->grads, out_params, p.n_params, lr, weight_decay,
-                                                       skip_lo, skip_hi);
+  net_sgd_kernel<false><<<(unsigned)blocks, 256, 0, stream>>>(st->params, st->grads, out_params, p.n_params, lr,
+                                                              weight_decay, skip_lo, skip_hi, nullptr, nullptr);
   B200OCL_LAUNCHED();
   return launch_pack(p, out_params, out_packed, stream);
+}
+
+size_t b200ocl_net_sgd_step_clipped_workspace_bytes(const b200ocl_net_desc* desc) {
+  using namespace b200ocl;
+  NetPlan p;
+  if (!desc || build_plan(*desc, p)) return 0;
+  return align_up((size_t)NORM_MAX_GRID * sizeof(double), 256) + 256;   // partials, then counter and coefficient
+}
+
+int b200ocl_net_sgd_step_clipped(const b200ocl_net_desc* desc, const b200ocl_net_state* st, float lr,
+                                 float weight_decay, float max_norm, float* norm_out, void* workspace,
+                                 size_t workspace_bytes, void* stream_) {
+  using namespace b200ocl;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  NetPlan p;
+  int rc = check_state(desc, st, p);
+  if (rc) return rc;
+  B200OCL_CHECK_ARG(st->grads, "state has no gradient arena");
+  if ((rc = check_workspace("b200ocl_net_sgd_step_clipped", workspace, workspace_bytes,
+                            b200ocl_net_sgd_step_clipped_workspace_bytes(desc)))) return rc;
+  unsigned char* base = static_cast<unsigned char*>(workspace);
+  double* part = reinterpret_cast<double*>(base);
+  unsigned int* counter = reinterpret_cast<unsigned int*>(base + align_up((size_t)NORM_MAX_GRID * sizeof(double), 256));
+  float* coef = reinterpret_cast<float*>(counter + 1);
+  size_t skip_lo = 0, skip_hi = 0;
+  if (p.head != 0) {
+    skip_lo = p.lin[0].w_off;
+    skip_hi = p.lin[0].b_off + p.lin[0].out;
+  }
+  size_t blocks = (p.n_params + 255) / 256;
+  size_t cap = (size_t)2 * sm_count();
+  if (cap > NORM_MAX_GRID) cap = NORM_MAX_GRID;
+  const unsigned norm_grid = (unsigned)(blocks < cap ? blocks : cap);
+  B200OCL_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), stream));
+  B200OCL_PROF("grad_norm", 4.0 * p.n_params, stream);
+  grad_norm_kernel<<<norm_grid, 256, 0, stream>>>(st->grads, p.n_params, skip_lo, skip_hi, max_norm, part, counter, coef,
+                                                  norm_out);
+  B200OCL_LAUNCHED();
+  cap = (size_t)8 * sm_count();
+  if (blocks > cap) blocks = cap;
+  B200OCL_PROF("sgd", 16.0 * p.n_params, stream);
+  net_sgd_kernel<true><<<(unsigned)blocks, 256, 0, stream>>>(st->params, st->grads, st->params, p.n_params, lr,
+                                                             weight_decay, skip_lo, skip_hi, coef, st->grads);
+  B200OCL_LAUNCHED();
+  return launch_pack(p, st->params, st->packed, stream);
 }
 
 size_t b200ocl_net_eval_workspace_bytes(const b200ocl_net_desc* desc, int N) {

@@ -355,6 +355,21 @@ class Engine:
                                          _stream())
         _native.check(rc, 'b200ocl_net_sgd_step')
 
+    def sgd_step_clipped(self, lr, weight_decay, max_norm):
+        """torch.nn.utils.clip_grad_norm_(parameters, max_norm) then opt.step() (agents/gdumb.py:82-83): the gradient
+        arena is scaled in place by min(max_norm / (norm + 1e-6), 1) and the SGD step uses it.  Returns the norm before
+        clipping as a device tensor [1]; the next call overwrites it.  Nothing is read back to the host."""
+        if getattr(self, '_clip', None) is None:
+            lib = _lib()
+            ws = _workspace(lib.b200ocl_net_sgd_step_clipped_workspace_bytes(ctypes.byref(self.desc)), self.device)
+            self._clip = (ws, torch.zeros(1, dtype=torch.float32, device=self.device))
+        ws, norm = self._clip
+        rc = _lib().b200ocl_net_sgd_step_clipped(ctypes.byref(self.desc), ctypes.byref(self.state.c), float(lr),
+                                                 float(weight_decay), float(max_norm), norm.data_ptr(), ws.data_ptr(),
+                                                 ws.numel(), _stream())
+        _native.check(rc, 'b200ocl_net_sgd_step_clipped')
+        return norm
+
 
 def ce_loss(logits, labels, want_grad=True, want_per_sample=False, want_correct=False):
     """Mean cross-entropy; returns dict(loss[1], dlogits, per_sample, n_correct[1])."""

@@ -1,7 +1,7 @@
 """Agents of the replay path with the reference surface `cls(model, opt, params)`,
 `.train_learner(x_train, y_train)`, `.evaluate(test_loaders)`:
 ExperienceReplay (agents/exp_replay.py:10-104: ER / MIR / ASER), SupContrastReplay (agents/scr.py:11-69), AGEM
-(agents/agem.py), Lwf (agents/lwf.py) and Icarl (agents/icarl.py), over ContinualLearner (agents/base.py:14-113) with
+(agents/agem.py), Lwf (agents/lwf.py), Icarl (agents/icarl.py) and Gdumb (agents/gdumb.py), over ContinualLearner (agents/base.py:14-113) with
 its training tricks (labels trick, separated softmax, kd_trick / kd_trick_star, review trick).
 
 The loop structure, the order of train-mode forwards (they move BN running statistics) and the
@@ -13,7 +13,7 @@ their forwards are kept for the BN side effect, their backwards are skipped.
 import numpy as np
 import torch
 
-from . import memory, ops
+from . import memory, nets, ops
 from .augment import SCRTransform
 from .engine import ce_loss, cls_loss, icarl_loss
 from .memory import Buffer, input_size_match
@@ -694,3 +694,68 @@ class Icarl(ContinualLearner):
         self._prev_live = True
         self._raise_label_errors()
         self.after_train()
+
+
+class Gdumb(ContinualLearner):
+    """GDumb (agents/gdumb.py:12-83) on the engine.  Per train_learner call: one pass over the stream in the reference's
+    batch order puts each sample through the greedy class-balanced memory (the decisions on the host, the rows moved by
+    one gather and one scatter); then train_mem() trains the network from a fresh initialisation, drawn as the
+    reference's setup_architecture draws it, over the whole memory for mem_epoch epochs: per batch one train-mode
+    forward, the criterion (the labels trick and separated softmax apply), one backward pass and one SGD step on the
+    gradient clipped to norm params.clip (b200ocl_net_sgd_step_clipped).  Evaluation is the inherited arg-max path."""
+
+    def __init__(self, model, opt, params):
+        if params.optimizer != 'SGD':
+            # train_mem builds its own optimizer with setup_opt(params.optimizer, ...) (gdumb.py:63); the engine steps SGD
+            raise NotImplementedError('GDumb on the b200ocl engine trains with SGD, not %r' % params.optimizer)
+        if (getattr(params, 'trick', None) or {}).get('ncm_trick'):
+            # the reference's nearest-class-mean evaluation reads self.buffer, which GDumb does not have
+            raise NotImplementedError('ncm_trick reads a buffer GDumb does not keep')
+        super().__init__(model, opt, params)
+        self._takes_teacher = False      # GDumb never reads a teacher
+        # not named `buffer`: after_train runs the review trick when the learner has one, and for GDumb the reference does not
+        self.memory = memory.GreedyBalancedMemory(params.mem_size, input_size_match[params.data][1], self.device)
+
+    @property
+    def mem_c(self):
+        """The reference's mem_c: label -> count in insertion order."""
+        return self.memory.mem_c
+
+    def train_mem(self):
+        """gdumb.py:52-83."""
+        if self.grad_sync is not None:
+            raise NotImplementedError('data-parallel GDumb: the clipping would have to follow the gradient all-reduce')
+        order = self.memory.order()
+        n = order.size
+        if n == 0:
+            raise RuntimeError('GDumb: the memory is empty (the reference fails in torch.stack, gdumb.py:57)')
+        eng = self.engine
+        params = nets.reference_init(self.data, eng.out_dim, eng.in_hw)                       # :61
+        eng.load(params, [(torch.zeros_like(rm), torch.ones_like(rv), 0) for rm, rv in eng.bn_views()])
+        self.model.train()
+        lr, wd = float(self.params.learning_rate), float(self.params.weight_decay)            # :63 setup_opt
+        clip = float(self.params.clip)
+        bs = self.batch
+        images, labels = self.memory.images, self.memory.labels
+        for _ in range(self.params.mem_epoch):
+            order = order[np.random.permutation(n)]                                            # :67-69, cumulative
+            order_t = memory.to_device_i64(order, self.device)
+            for j in range(n // bs):
+                idx = order_t[j * bs:(j + 1) * bs]
+                bx, by = ops.gather_rows(images, idx), ops.gather_rows(labels, idx)
+                logits, ws = eng.forward_train(bx, slot=0)                                     # :78
+                out = self.criterion(logits, by)                                               # :79
+                eng.backward(bx, out['dlogits'], ws)                                           # :80-81
+                eng.sgd_step_clipped(lr, wd, clip)                                             # :82-83
+                self.last_loss = out['loss']
+                self._throttle()
+
+    def train_learner(self, x_train, y_train):
+        self.before_train(x_train, y_train)
+        stream = StreamFeeder(x_train, y_train, self.batch, self.device)                       # :35-38 (drop_last)
+        n = len(stream) * self.batch
+        slots, sources = self.memory.plan(stream.y_host[:n])                                   # :40-47
+        self.memory.write(stream.x, stream.y_host, slots, sources)
+        self.train_mem()                                                                       # :49
+        self._raise_label_errors()
+        self.after_train()                                                                     # :50

@@ -1,4 +1,5 @@
-"""Replay memory: the Buffer tensor store, uniform retrieval and class-balanced sampling.
+"""Replay memory: the Buffer tensor store, uniform retrieval and class-balanced sampling, and GDumb's greedy
+class-balanced memory (GreedyBalancedMemory, agents/gdumb.py:19-31).
 
 Mirrors the reference surface (utils/buffer/buffer.py:8-41; utils/buffer/buffer_utils.py:9-26,
 74-160) with a different split of work:
@@ -9,6 +10,7 @@ Mirrors the reference surface (utils/buffer/buffer.py:8-41; utils/buffer/buffer_
   * rows move with the gather/scatter kernels of csrc/misc.cu.
 """
 import os
+import random
 from collections import defaultdict
 
 import numpy as np
@@ -409,6 +411,71 @@ class ClassBalancedRandomSampling:
                     cache[c].add(i)
             cls.class_index_cache = cache
             # the reference leaves class_num_cache untouched on this path (buffer_utils.py:155-160)
+
+
+# --------------------------------------------------------------------------- GDumb's memory
+class GreedyBalancedMemory(object):
+    """GDumb's greedy class-balanced memory (agents/gdumb.py:19-31) as a device pool of `mem_size` slots.
+
+    The reference keeps per-class Python lists of image tensors and counts; here the lists hold slot ids into a
+    [mem_size,3,H,W] fp32 image pool and a [mem_size] int64 label pool, and a stack keeps the free slots.  Every
+    decision is taken on the host by plan() with the reference's rule and its draws on Python's global `random`; write()
+    then moves the rows with one gather and one scatter."""
+
+    def __init__(self, mem_size, in_hw, device):
+        if int(mem_size) < 1:
+            raise ValueError('GDumb needs mem_size >= 1, got %d' % int(mem_size))
+        self.mem_size = int(mem_size)
+        self.device = torch.device(device)
+        self.images = torch.zeros((self.mem_size, 3, in_hw, in_hw), dtype=torch.float32, device=self.device)
+        self.labels = torch.zeros(self.mem_size, dtype=torch.int64, device=self.device)
+        self.mem_c = {}                   # label -> count, in the insertion order of the reference's mem_c / mem_img
+        self.slots = {}                   # label -> slot ids in the order of the reference's mem_img[label] list
+        self._free = list(range(self.mem_size - 1, -1, -1))    # stack of free slots (slot 0 on top)
+        self._labels_host = np.zeros(self.mem_size, dtype=np.int64)
+        self._size = 0
+
+    def __len__(self):
+        return self._size
+
+    def plan(self, labels):
+        """greedy_balancing_update (gdumb.py:19-31) for each label in order: (slots, sources), the slots this pass
+        writes and, for each, the position in `labels` of the sample that ends up there (a slot freed and refilled
+        within the pass keeps only its last source).  Updates mem_c and the slot lists."""
+        src_of = {}
+        for j, y in enumerate(np.asarray(labels, dtype=np.int64).tolist()):
+            k_c = self.mem_size // max(1, len(self.mem_c))
+            if y not in self.mem_c or self.mem_c[y] < k_c:
+                if self._size >= self.mem_size:
+                    cls_max = max(self.mem_c.items(), key=lambda kv: kv[1])[0]     # the first class of maximal count
+                    idx = random.randrange(self.mem_c[cls_max])
+                    self._free.append(self.slots[cls_max].pop(idx))
+                    self.mem_c[cls_max] -= 1
+                    self._size -= 1
+                if y not in self.mem_c:
+                    self.mem_c[y] = 0
+                    self.slots[y] = []
+                slot = self._free.pop()
+                self.slots[y].append(slot)
+                self.mem_c[y] += 1
+                self._size += 1
+                src_of[slot] = j
+        slots = np.fromiter(src_of.keys(), dtype=np.int64, count=len(src_of))
+        return slots, np.fromiter(src_of.values(), dtype=np.int64, count=len(src_of))
+
+    def write(self, x, y_host, slots, sources):
+        """images[slots] = x[sources] (one gather, one scatter) and labels[slots] = y_host[sources]."""
+        if slots.size == 0:
+            return
+        src_t = to_device_i64(sources, self.device)
+        ops.scatter_rows(self.images, to_device_i64(slots, self.device), ops.gather_rows(x, src_t))
+        self._labels_host[slots] = np.asarray(y_host, dtype=np.int64)[sources]
+        self.labels = to_device_i64(self._labels_host, self.device)
+
+    def order(self):
+        """Slot ids in train_mem's order (gdumb.py:53-58): classes in insertion order, each in its list order."""
+        parts = [np.asarray(self.slots[c], dtype=np.int64) for c in self.mem_c]
+        return np.concatenate(parts) if parts else np.zeros(0, dtype=np.int64)
 
 
 # --------------------------------------------------------------------------- buffer

@@ -145,6 +145,52 @@ def setup_architecture(params):
     raise NotImplementedError('dataset %s is outside the replay-path scope (SURVEY section 8)' % params.data)
 
 
+def reduced_resnet_dim_in(in_hw, nf=20):
+    """Flattened encoder feature size of Reduced_ResNet18 for in_hw x in_hw inputs: three stride-2 3x3 convolutions
+    (padding 1), then avg_pool2d(4) (models/resnet.py:90-103)."""
+    h = int(in_hw)
+    for _ in range(3):
+        h = (h - 1) // 2 + 1
+    return nf * 8 * (h // 4) ** 2
+
+
+def reference_init(data, num_classes, in_hw):
+    """The parameters a fresh setup_architecture(params) draws on the CPU (utils/setup_elements.py:46-68, as
+    agents/gdumb.py:61 calls it), in parameters() order, drawn in module construction order from torch's default CPU
+    generator by the torch.nn.init calls the layers' reset_parameters() make: kaiming_uniform_(a=sqrt(5)) for every
+    convolution and linear weight, uniform_(+-1/sqrt(fan_in)) for the linear bias; BatchNorm weights 1 and biases 0
+    take no draws.  For mini_imagenet the 160-input classifier Reduced_ResNet18 builds is drawn and then replaced by a
+    640-input one (setup_elements.py:63-66), so both are drawn and the first is discarded."""
+    dim_in = reduced_resnet_dim_in(in_hw)
+
+    def linear(fan_in):
+        w = torch.empty(num_classes, fan_in)
+        nn.init.kaiming_uniform_(w, a=math.sqrt(5))
+        b = torch.empty(num_classes)
+        f, _ = nn.init._calculate_fan_in_and_fan_out(w)
+        nn.init.uniform_(b, -1 / math.sqrt(f), 1 / math.sqrt(f))
+        return w, b
+
+    out = []
+    for name, shape in param_layout(dim_in, num_classes):
+        if name.startswith('linear.'):
+            continue
+        t = torch.empty(shape)
+        if len(shape) == 4:
+            nn.init.kaiming_uniform_(t, a=math.sqrt(5))
+        elif name.endswith('.weight'):
+            nn.init.ones_(t)
+        else:
+            nn.init.zeros_(t)
+        out.append(t)
+    w, b = linear(20 * 8)
+    if data == 'mini_imagenet':
+        w, b = linear(dim_in)
+    elif dim_in != 20 * 8:
+        raise NotImplementedError('reference_init: %dx%d inputs of %s are outside the replay path' % (in_hw, in_hw, data))
+    return out + [w, b]
+
+
 def adopt(module, in_hw):
     """Move a reference nn.Module (models.resnet.ResNet with BasicBlocks, or SupConResNet) onto
     the engine.  Its Parameters / BN buffers are re-pointed at the engine arenas, keeping the

@@ -7,9 +7,10 @@ already hold), so `general_main.py` runs unchanged:
 
     import b200ocl; b200ocl.install()          # before main(args); or:  python -m b200ocl.launch general_main.py ...
 
-Every other agent / plugin of the reference stays registered and untouched.
+The agents registered here are ER, SCR, AGEM, LWF, ICARL and GDUMB.  Every other agent / plugin of the reference
+(EWC, CNDPM, the match retrievals) stays registered and untouched.
 """
-from .learners import AGEM, ExperienceReplay, Icarl, Lwf, SupContrastReplay
+from .learners import AGEM, ExperienceReplay, Gdumb, Icarl, Lwf, SupContrastReplay
 from .retrieve import ASER_retrieve, MIR_retrieve, Random_retrieve
 from .update import ASER_update, GSSGreedyUpdate, Reservoir_update
 
@@ -19,6 +20,7 @@ agents = {
     'AGEM': AGEM,
     'LWF': Lwf,
     'ICARL': Icarl,
+    'GDUMB': Gdumb,
 }
 
 retrieve_methods = {
