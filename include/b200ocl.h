@@ -304,9 +304,11 @@ int b200ocl_selftest_umma_tf32(const float* A, const float* B, float* D, int N, 
  * family, NHWC fp32, weights OIHW: path 0 automatic, 1 CUDA-core kernels, 2 wgmma with im2col tiles
  * (conv_tc.cu), 3 wgmma fed from a halo strip (conv_tcp.cu).  mode 0 raw store, 1 accumulate into out, 2 train
  * (forward only): raw store plus stats_out[4*cout] = batch mean, 1/sqrt(var+eps), running mean, running var
- * updated from zero with momentum 0.1.  Exists so that tests can pin every convolution kernel against a reference
- * convolution; fails with B200OCL_EUNSUPPORTED when the path does not cover the shape.  Path 3 covers 3x3 stride-1
- * convolutions in modes 0 and 1 only: train mode, stride 2 and 1x1 return B200OCL_EUNSUPPORTED. */
+ * updated from zero with momentum 0.1; 3 eval (forward only): out = (conv - mean) * gamma / sqrt(var + eps) + beta
+ * with stats_out[4*cout] = mean, var, gamma, beta as input; 4 the same plus x as the residual, then ReLU (cin == cout).
+ * Exists so that tests can pin every convolution kernel against a reference convolution; fails with
+ * B200OCL_EUNSUPPORTED when the path does not cover the shape.  Path 3 covers 3x3 stride-1 convolutions in every mode
+ * but 2: train mode, stride 2 and 1x1 return B200OCL_EUNSUPPORTED. */
 size_t b200ocl_conv_selftest_workspace_bytes(int N, int cin, int cout, int H, int W, int ks, int stride);
 int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N, int H, int W, int cin, int cout,
                           int ks, int stride, int dgrad, int path, int mode, float* stats_out, void* workspace,

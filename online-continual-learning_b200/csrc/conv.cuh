@@ -70,8 +70,9 @@ __device__ __forceinline__ void bn_finalize(const ConvArgs& a, int c, double S, 
   a.run_var[c] = bn_running_update(a.run_var[c], (float)unbiased, a.momentum);
 }
 
-// conv_tcp.cu stages 128 + 2 * (W + 2) + 2 strip rows per tile, TP_LD_MAX per patch-loader thread (16 rows per pass):
-// maps up to W = 37 wide.  The network plan builds halo-strip weight images exactly for the maps that fit.
+// conv_tcp.cu stages 128 + 2 * (W + 1) + 2 strip rows per tile, TP_LD_MAX per patch-loader thread (16 rows per pass).
+// The bound still counts the 128 + 2 * (W + 2) + 2 rows of the earlier two-position halo, so the eligible maps stay
+// those up to W = 37 wide.  The network plan builds halo-strip weight images exactly for the maps that fit.
 constexpr int TP_LD_MAX = 13;
 inline bool tcp_strip_fits(int W) { return 128 + 2 * (W + 2) + 2 <= 16 * TP_LD_MAX; }
 

@@ -6,15 +6,19 @@
 // arrays (TF32 hi / lo) of one 128-byte row per patch pixel, and the A operand of every tap is that
 // same array read through a shifted shared-memory descriptor:
 //
-//   strip  = the zero-padded input of the whole batch, row-major: position s = (img*(H+2) + yp)*(W+2) + xp,
-//            one 128-byte row (32 channel slots) per position, the halo positions hold zeros
-//   tile   = 128 consecutive strip positions = the 128 rows of an MMA tile; row i is the output pixel
-//            (img, y = yp, x = xp) when yp < H and xp < W, a discarded by-product otherwise
-//   tap (kh, kw) of row i reads strip position  s_i + kh*(W+2) + kw  -> one descriptor per tap whose start
-//            address is the patch base + (kh*(W+2) + kw) * 128 bytes; rows stay consecutive, so the 8-row
+//   strip  = the input of the whole batch with a one-position zero halo shared between neighbours, row-major:
+//            row length W+1, image size (H+1)*(W+1); pixel (img, y, x) sits at position
+//            s = img*(H+1)*(W+1) + (y+1)*(W+1) + (x+1), one 128-byte row (32 channel slots) per position.
+//            Strip row 0 and strip column 0 of every image hold zeros: they are the neighbours above pixel row 0
+//            and left of pixel column 0; the right neighbour of pixel column W-1 is the next strip row's column 0,
+//            and the row below pixel row H-1 is the next image's strip row 0 (or the zero tail past the last image).
+//   tile   = 128 consecutive strip positions = the 128 rows of an MMA tile; row i at s_i = img*(H+1)*(W+1) +
+//            y*(W+1) + x is the output pixel (img, y, x) when y < H and x < W, a discarded by-product otherwise
+//   tap (kh, kw) of row i reads strip position  s_i + kh*(W+1) + kw  -> one descriptor per tap whose start
+//            address is the patch base + (kh*(W+1) + kw) * 128 bytes; rows stay consecutive, so the 8-row
 //            groups are the standard 1024 bytes apart.
-// A stage therefore holds 128 + 2*(W+2) + 2 strip rows.  Any H, W works; the share of useful rows is
-// H*W / ((H+2)*(W+2)): 89 % at 32x32, 79 % at 16x16, 64 % at 8x8, 44 % at 4x4 -- tensor-core time is not
+// A stage therefore holds 128 + 2*(W+1) + 2 strip rows.  Any H, W works; the share of useful rows is
+// H*W / ((H+1)*(W+1)): 94 % at 32x32, 89 % at 16x16, 79 % at 8x8, 64 % at 4x4 -- tensor-core time is not
 // what bounds the kernel, and no im2col or per-shape tiling is needed.
 //
 // The hardware applies the 128-byte swizzle to absolute address bits, so a window that starts at any
@@ -48,15 +52,15 @@ using umma::mbar_expect_tx;
 using umma::bulk_g2s;
 
 struct TileGeom {
-  int wp, pp;        // padded row length W + 2, padded image size (H + 2) * (W + 2)
+  int wp, pp;        // strip row length W + 1, strip image size (H + 1) * (W + 1)
   int tiles_m;       // tiles of 128 strip positions
   int prow;          // strip rows staged per tile: 128 + 2 * wp + 2
   int pbytes;        // bytes of one hi (or lo) patch, 1024-aligned
 };
 __host__ __device__ inline TileGeom tile_geom(int N, int H, int W) {
   TileGeom g;
-  g.wp = W + 2;
-  g.pp = (H + 2) * (W + 2);
+  g.wp = W + 1;
+  g.pp = (H + 1) * (W + 1);
   // the last useful position is the last real pixel of the last image
   const long last = (long)(N - 1) * g.pp + (long)(H - 1) * g.wp + (W - 1);
   g.tiles_m = (int)(last / 128) + 1;
@@ -139,7 +143,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
           yp = rem / G.wp;
           xp = rem - yp * G.wp;
         }
-        const int hp = a.Hin + 2;
+        const int hp = a.Hin + 1;                             // strip rows per image: the zero row, then H pixel rows
 #pragma unroll
         for (int i = 0; i < TP_LD_MAX; ++i) {
           v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -245,7 +249,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
           const int b = resident ? tap : q % BS;
           if (!(resident && b_ready))
             if (!umma::mbar_wait(&bfull[b], resident ? 0u : (uint32_t)((q / BS) & 1))) s_fail = 1;
-          const uint64_t dAh = dAs + (uint64_t)((kh * G.wp + kw) * 8);   // + (kh*(W+2) + kw) rows of 128 B
+          const uint64_t dAh = dAs + (uint64_t)((kh * G.wp + kw) * 8);   // + (kh*(W+1) + kw) rows of 128 B
           const uint64_t dAl = dAh + A_LO;
           const uint64_t dBh = dB0 + (uint64_t)(b * B_SLOT);
           const uint64_t dBl = dBh + B_LO;

@@ -862,7 +862,9 @@ int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200OCL_CHECK_ARG(x && w_oihw && out && workspace, "null pointer");
   B200OCL_CHECK_ARG(N > 0 && H > 0 && W > 0 && cin % 20 == 0 && cout % 20 == 0 && cin > 0 && cout > 0, "bad shape");
-  B200OCL_CHECK_ARG(mode >= 0 && mode <= 2 && (mode != 2 || (stats_out && !dgrad)), "mode 2 (train) needs stats_out, forward only");
+  B200OCL_CHECK_ARG(mode >= 0 && mode <= 4 && (mode != 2 || (stats_out && !dgrad)), "mode 2 (train) needs stats_out, forward only");
+  B200OCL_CHECK_ARG(mode < 3 || (stats_out && !dgrad && (mode == 3 || cin == cout)),
+                    "modes 3 / 4 (eval) need stats_out, forward only; mode 4 needs cin == cout");
   B200OCL_CHECK_ARG((ks == 3 || ks == 1) && (stride == 1 || stride == 2) && (!dgrad || (ks == 3 && stride == 1)),
                     "3x3 or 1x1, stride 1 or 2; data gradient for 3x3 stride 1 only");
   B200OCL_CHECK_ARG(workspace_bytes >= b200ocl_conv_selftest_workspace_bytes(N, cin, cout, H, W, ks, stride), "workspace too small");
@@ -881,7 +883,7 @@ int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N
   int rc = launch_pack(p, w_oihw, packed, stream);
   if (rc) return rc;
   ConvArgs a = conv_layer_args(p.conv[0], N, x, packed, out, dgrad);
-  a.mode = mode == 2 ? CONV_TRAIN : (mode == 1 ? CONV_ACCUM : CONV_RAW);
+  a.mode = mode >= 3 ? CONV_EVAL : mode == 2 ? CONV_TRAIN : (mode == 1 ? CONV_ACCUM : CONV_RAW);
   a.force_path = path;
   a.eps = NET_BN_EPS;
   a.momentum = NET_BN_MOMENTUM;
@@ -894,6 +896,14 @@ int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N
     a.save_invstd = stats_out + cout;
     a.run_mean = stats_out + 2 * cout;
     a.run_var = stats_out + 3 * cout;
+  }
+  if (mode >= 3) {
+    a.rmean = stats_out;
+    a.rvar = stats_out + cout;
+    a.gamma = stats_out + 2 * cout;
+    a.beta = stats_out + 3 * cout;
+    a.residual = mode == 4 ? x : nullptr;
+    a.relu = mode == 4;
   }
   return launch_conv(a, stream);
 }

@@ -10,12 +10,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 out = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, 'gpurun_out', 'net_layers.csv')
 os.environ['B200OCL_PROF_DUMP'] = out
-from b200ocl import _native  # noqa: E402
+from b200ocl import _native, engine  # noqa: E402
 from b200ocl.engine import Engine  # noqa: E402
 
 
 def main():
     lib = _native.lib()
+    engine.set_graphs(False)      # the per-launch profiler records eager launches only
     torch.manual_seed(0)
     eng = Engine(32, 100)
     g = torch.Generator(device='cuda').manual_seed(1)
