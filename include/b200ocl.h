@@ -192,6 +192,27 @@ int b200ocl_net_features_eval(const b200ocl_net_desc* desc, const b200ocl_net_st
  * num_batches_tracked updated (momentum 0.1, unbiased variance); activations are kept in
  * `workspace` for b200ocl_net_backward.  out [N,out_dim]. */
 size_t b200ocl_net_train_workspace_bytes(const b200ocl_net_desc* desc, int N);
+
+/* Where a train workspace of N images keeps conv layer `layer`'s tensors (layers in BatchNorm2d module order) and the
+ * launches b200ocl_net_backward makes for it on the current device.  Byte offsets are from the workspace start:
+ * z / a the raw / activated output [N,hout,wout,cout] (a block's conv2 slot holds the block output), mean / invstd the
+ * saved BN statistics [cout], feat / hid / proj the head tensors [N,dim_in] / [N,dim_in] / [N,out_dim] (the same for every
+ * layer), wg_part the start of the weight-gradient partials and wg_layer this layer's wgrad_splits partials of
+ * [ks*ks*cin][cout] floats.  bn_fused: 1 fused BN backward, 0 reduce + apply, over bn_grid CTAs.  wgrad_kernel: 0 stem,
+ * 1 wgmma (wgrad_tc.cu), 2 fp32.  Host only, launches nothing; exists so that tests can read what the engine's forward
+ * left behind and check which launch geometries a batch size reaches.  B200OCL_EINVAL for N < 1 or a layer out of range. */
+typedef struct {
+  size_t bytes;
+  size_t z, a, mean, invstd;
+  size_t feat, hid, proj;
+  size_t wg_part, wg_layer;
+  int cin, cout, ks, stride, hout, wout;
+  int bn_fused, bn_grid;
+  int wgrad_kernel, wgrad_splits;
+  int sms;
+} b200ocl_net_ws_layout;
+int b200ocl_net_train_ws_layout(const b200ocl_net_desc* desc, int N, int layer, b200ocl_net_ws_layout* out);
+
 int b200ocl_net_forward_train(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const float* x, int N,
                               float* out, void* workspace, size_t workspace_bytes, void* stream);
 

@@ -39,6 +39,7 @@ SIGNATURES = {
     'b200ocl_net_eval_workspace_bytes': (c_size_t, [P, c_int]),
     'b200ocl_net_features_eval': (c_int, [P, P, P, c_int, P, P, c_size_t, P]),
     'b200ocl_net_train_workspace_bytes': (c_size_t, [P, c_int]),
+    'b200ocl_net_train_ws_layout': (c_int, [P, c_int, c_int, P]),
     'b200ocl_net_forward_train': (c_int, [P, P, P, c_int, P, P, c_size_t, P]),
     'b200ocl_net_forward_evalgrad': (c_int, [P, P, P, c_int, P, P, c_size_t, P]),
     'b200ocl_net_forward_train_deferred': (c_int, [P, P, P, c_int, P, P, c_size_t, P]),

@@ -1030,6 +1030,43 @@ size_t b200ocl_net_train_workspace_bytes(const b200ocl_net_desc* desc, int N) {
   return train_ws(p, N > 0 ? N : 1, nullptr, sm_count()).bytes;
 }
 
+int b200ocl_net_train_ws_layout(const b200ocl_net_desc* desc, int N, int layer, b200ocl_net_ws_layout* out) {
+  using namespace b200ocl;
+  B200OCL_CHECK_ARG(desc && out, "null pointer");
+  NetPlan p;
+  const int rc = build_plan(*desc, p);
+  if (rc) {
+    set_error("b200ocl_net_train_ws_layout: unsupported network description");
+    return rc;
+  }
+  B200OCL_CHECK_ARG(N >= 1, "need N >= 1");
+  B200OCL_CHECK_ARG(layer >= 0 && layer < p.n_conv, "layer out of range");
+  const int sms = sm_count();
+  const TrainWs w = train_ws(p, N, nullptr, sms);   // offsets from a null base
+  const ConvL& c = p.conv[layer];
+  auto off = [](const void* q) { return (size_t)reinterpret_cast<uintptr_t>(q); };
+  *out = b200ocl_net_ws_layout{};
+  out->bytes = w.bytes;
+  out->z = off(w.z + (size_t)N * c.act_off);
+  out->a = off(w.a + (size_t)N * c.act_off);
+  out->mean = off(w.save + p.bn[layer].save_off);
+  out->invstd = off(w.save + p.bn[layer].save_off + p.bn[layer].c);
+  out->feat = off(w.feat);
+  out->hid = off(w.hid);
+  out->proj = off(w.proj);
+  out->wg_part = off(w.wg_part);
+  out->wg_layer = off(w.wg_part + w.wg_off[layer]);
+  out->cin = c.cin; out->cout = c.cout; out->ks = c.ks; out->stride = c.stride; out->hout = c.hout; out->wout = c.wout;
+  const BnBwdGeom g = bn_bwd_geom(N * c.hout * c.wout, c.cout, sms, true);   // b200ocl_net_backward always has a ready flag
+  out->bn_fused = g.fused ? 1 : 0;
+  out->bn_grid = g.grid;
+  const WgradPlan wp = wgrad_plan(p, layer, N, sms);
+  out->wgrad_kernel = wp.kernel == WGRAD_STEM ? 0 : (wp.kernel == WGRAD_TC ? 1 : 2);
+  out->wgrad_splits = wp.splits;
+  out->sms = sms;
+  return B200OCL_OK;
+}
+
 static int net_forward_impl(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const float* x, int N, float* out,
                             void* workspace, size_t workspace_bytes, void* stream_, int ev) {
   using namespace b200ocl;

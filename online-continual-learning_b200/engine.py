@@ -32,8 +32,24 @@ class NetInfo(ctypes.Structure):
                 ('n_tensors', c_int), ('dim_in', c_int), ('out_dim', c_int)]
 
 
+class NetWsLayout(ctypes.Structure):
+    """b200ocl_net_ws_layout: byte offsets of one conv layer's tensors in a train workspace and its backward launches."""
+    _fields_ = [('bytes', c_size_t), ('z', c_size_t), ('a', c_size_t), ('mean', c_size_t), ('invstd', c_size_t),
+                ('feat', c_size_t), ('hid', c_size_t), ('proj', c_size_t), ('wg_part', c_size_t), ('wg_layer', c_size_t),
+                ('cin', c_int), ('cout', c_int), ('ks', c_int), ('stride', c_int), ('hout', c_int), ('wout', c_int),
+                ('bn_fused', c_int), ('bn_grid', c_int), ('wgrad_kernel', c_int), ('wgrad_splits', c_int), ('sms', c_int)]
+
+
 def _lib():
     return _native.lib()
+
+
+def train_ws_layout(desc, n, layer):
+    """Host-only test hook (b200ocl_net_train_ws_layout) for conv layer `layer` of a train workspace of n images."""
+    out = NetWsLayout()
+    _native.check(_lib().b200ocl_net_train_ws_layout(ctypes.byref(desc), int(n), int(layer), ctypes.byref(out)),
+                  'b200ocl_net_train_ws_layout')
+    return out
 
 
 def describe(in_hw, num_classes, head=None, feat_dim=128, nf=20):
