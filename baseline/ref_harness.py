@@ -125,6 +125,9 @@ def make_params(kind, **over):
     elif kind == 'gdumb':      # config/agent/gdumb/gdumb_5k.yml
         base.update(agent='GDUMB', retrieve='random', update='random', eps_mem_batch=10, mem_epoch=30, clip=10.0,
                     minlr=0.0005)
+    elif kind == 'ewc':        # general_main.py:110-115 defaults, config/agent/ewc/ewc.yml
+        base.update(agent='EWC', retrieve='random', update='random', eps_mem_batch=10, lambda_=100.0, alpha=0.9,
+                    fisher_update_after=50)
     else:
         raise ValueError(kind)
     base.update(over)

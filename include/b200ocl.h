@@ -262,6 +262,43 @@ int b200ocl_net_sgd_step_clipped(const b200ocl_net_desc* desc, const b200ocl_net
                                  float weight_decay, float max_norm, float* norm_out, void* workspace,
                                  size_t workspace_bytes, void* stream);
 
+/* EWC++ state (agents/ewc_pp.py): four fp32 device arenas in the parameter arena's layout (n_params floats each):
+ * running_fisher, tmp_fisher, normalized_fisher and prev_params. */
+typedef struct {
+  float* running;
+  float* tmp;
+  float* normalized;
+  float* prev;
+} b200ocl_ewc_state;
+
+#define B200OCL_EWC_PENALTY 1 /* the penalty lambda * sum F * (p - prev)^2 is in the loss (from the second call on) */
+#define B200OCL_EWC_EMA 2     /* update_running_fisher fires before this step */
+
+/* One EWC++ step after the backward pass (ewc_pp.py:40-62), one launch and one pass per element, then `packed` is
+ * refreshed as by b200ocl_net_sgd_step.  In order, each with torch's separate fp32 roundings (no fma):
+ *   EMA:      running = ema_keep * running + ema_add * tmp, then tmp = 0, with ema_keep = fp32(1 - alpha) and
+ *             ema_add = fp32(1/fua * alpha) formed in double by the caller;
+ *   PENALTY:  g += (up * normalized) * (2 * (p - prev)), written back to the gradient arena; `up` is the gradient
+ *             autograd delivers to the regulariser: fp32(lambda), times the kd_trick / kd_trick_star mixing weights
+ *             in fp32 from the outermost inward;
+ *   always:   tmp += g * g, then the SGD update of b200ocl_net_sgd_step with g.
+ * The tensors b200ocl_net_sgd_step skips are left untouched in every arena.  penalty_out (nullable, device): with
+ * PENALTY sum normalized * (p - prev)^2 over the pre-step weights, from per-CTA fp64 partials added in CTA order by
+ * the last CTA (no floating-point atomics: repeated launches are bit-identical); 0 without.  workspace:
+ * b200ocl_net_sgd_step_ewc_workspace_bytes(desc) bytes of device memory, no initial contents needed. */
+size_t b200ocl_net_sgd_step_ewc_workspace_bytes(const b200ocl_net_desc* desc);
+int b200ocl_net_sgd_step_ewc(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const b200ocl_ewc_state* ewc,
+                             float lr, float weight_decay, float up, int flags, float ema_keep, float ema_add,
+                             float* penalty_out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* The end of an EWC++ train_learner call (ewc_pp.py:71-78), two launches, nothing read back: prev = params, then
+ * normalized = (running - mn) / ((mx - mn) + 1e-32) with mn / mx the min / max of running over every tensor, in fp32
+ * with an IEEE division.  The tensors b200ocl_net_sgd_step skips are left out and untouched.  workspace:
+ * b200ocl_ewc_consolidate_workspace_bytes(desc) bytes, no initial contents needed. */
+size_t b200ocl_ewc_consolidate_workspace_bytes(const b200ocl_net_desc* desc);
+int b200ocl_ewc_consolidate(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const b200ocl_ewc_state* ewc,
+                            void* workspace, size_t workspace_bytes, void* stream);
+
 /* Mean cross-entropy (agents/base.py:95,113) over logits [N,C], labels [N]:
  * loss[1]; per_sample [N] (F.cross_entropy(reduction='none'), mir_retrieve.py:26-27);
  * dlogits [N,C] = d(mean CE)/dlogits; n_correct[1] = #(argmax == label).  Each output nullable. */

@@ -9,7 +9,7 @@ library fallback: every op raises if the CUDA library is missing.
 __version__ = '0.1.0'
 
 
-def install(reference_name_match=None):
-    """Patch the reference registries in place (see registry.install)."""
+def install(reference_name_match=None, extra=()):
+    """Patch the reference registries in place (see registry.install); `extra` names opt-in agents, e.g. ('EWC',)."""
     from . import registry
-    return registry.install(reference_name_match)
+    return registry.install(reference_name_match, extra=extra)

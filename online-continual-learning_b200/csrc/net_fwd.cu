@@ -222,6 +222,33 @@ __global__ void __launch_bounds__(256) net_sgd_kernel(const float* __restrict__ 
 // Per-CTA fp64 partial sums of squares in a fixed order; the last CTA to arrive adds them in CTA order.
 constexpr int NORM_MAX_GRID = 1024;
 
+// Workspace of the arena reductions (grad_norm_kernel, the EWC++ kernels): one 8-byte partial per CTA (up to
+// NORM_MAX_GRID), then, at the next 256-byte boundary, the arrival counter followed by the reduction's fp32 results.
+constexpr size_t REDUCE_TAIL_OFF = (NORM_MAX_GRID * sizeof(double) + 255) / 256 * 256;
+constexpr size_t REDUCE_WS_BYTES = REDUCE_TAIL_OFF + 256;
+inline unsigned int* reduce_counter(void* ws) {
+  return reinterpret_cast<unsigned int*>(static_cast<unsigned char*>(ws) + REDUCE_TAIL_OFF);
+}
+inline float* reduce_scalars(void* ws) { return reinterpret_cast<float*>(reduce_counter(ws) + 1); }
+
+// The tensors that never receive a gradient (the SupCon network's unused classifier): every pass that steps the
+// arenas leaves [lo, hi) out.
+inline void sgd_skip_range(const NetPlan& p, size_t& lo, size_t& hi) {
+  lo = hi = 0;
+  if (p.head != 0) {
+    lo = p.lin[0].w_off;
+    hi = p.lin[0].b_off + p.lin[0].out;
+  }
+}
+
+// Grid of a grid-stride pass of 256-thread CTAs over the parameter arena: at most per_sm CTAs per SM and `cap`.
+inline unsigned arena_grid(const NetPlan& p, int per_sm, size_t cap) {
+  size_t blocks = (p.n_params + 255) / 256;
+  const size_t sm_cap = (size_t)per_sm * sm_count();
+  if (blocks > sm_cap) blocks = sm_cap;
+  return (unsigned)(blocks < cap ? blocks : cap);
+}
+
 __global__ void __launch_bounds__(256) grad_norm_kernel(const float* __restrict__ g, size_t n, size_t skip_lo,
                                                         size_t skip_hi, float max_norm, double* __restrict__ part,
                                                         unsigned int* counter, float* coef, float* norm_out) {
@@ -258,6 +285,134 @@ __global__ void __launch_bounds__(256) grad_norm_kernel(const float* __restrict_
     *coef = q > 1.f ? 1.f : q;          // torch.clamp(max=1.0): a NaN norm stays NaN
 
     if (norm_out) *norm_out = norm;
+  }
+}
+
+// ----------------------------------------------------------------------------- EWC++ step and consolidation
+// One pass per element in the order of agents/ewc_pp.py: the EMA of update_running_fisher (EMA), the penalty's gradient
+// added to the network's (PEN), accum_fisher's tmp += g*g, then the SGD update of net_sgd_kernel.  Every torch op is
+// its own rounding, so the products and sums are spelled with __f*_rn: nvcc would contract them to fma.  The SGD
+// update is written as net_sgd_kernel writes it, so that it compiles to the same instructions.  With PEN and pen_out,
+// sum F*d^2 over the pre-step weights goes to pen_out: per-CTA fp64 partials, added in CTA order by the last CTA.
+template <bool EMA, bool PEN>
+__global__ void __launch_bounds__(256) net_sgd_ewc_kernel(float* __restrict__ p, float* __restrict__ g,
+                                                          float* __restrict__ running, float* __restrict__ tmp,
+                                                          const float* __restrict__ fisher,
+                                                          const float* __restrict__ prev, size_t n, size_t skip_lo,
+                                                          size_t skip_hi, float lr, float wd, float up, float ema_keep,
+                                                          float ema_add, double* __restrict__ part,
+                                                          unsigned int* counter, float* pen_out) {
+  double acc = 0.0;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if (i >= skip_lo && i < skip_hi) continue;   // tensors that never receive a gradient: untouched in every arena
+    const float w = p[i];
+    float gi = g[i];
+    float t = tmp[i];
+    if (EMA) {
+      // (1 - alpha) * running + (1/fua * alpha) * tmp, then tmp = 0 (ewc_pp.py:104-108)
+      running[i] = __fadd_rn(__fmul_rn(ema_keep, running[i]), __fmul_rn(ema_add, t));
+      t = 0.f;
+    }
+    if (PEN) {
+      // autograd of lambda * (F * (p - prev)**2).sum(): (up * F) * (2 * d), added once to the network's gradient
+      const float f = fisher[i];
+      const float d = __fsub_rn(w, prev[i]);
+      gi = __fadd_rn(gi, __fmul_rn(__fmul_rn(up, f), __fmul_rn(2.f, d)));
+      g[i] = gi;
+      const double dd = (double)d;
+      acc = fma((double)f * dd, dd, acc);
+    }
+    tmp[i] = __fadd_rn(t, __fmul_rn(gi, gi));   // accum_fisher: tmp += grad ** 2 (pow 2 is grad * grad)
+    if (wd != 0.f) gi = fmaf(wd, w, gi);
+    p[i] = w - lr * gi;
+  }
+  if (!PEN || !pen_out) return;
+  __shared__ double s_red[8];
+  __shared__ bool is_last;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(FULL_MASK, acc, o);
+  if (lane == 0) s_red[warp] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) s += s_red[k];
+    part[blockIdx.x] = s;
+    __threadfence();
+    is_last = (atomicAdd(counter, 1u) == gridDim.x - 1);
+  }
+  __syncthreads();
+  if (is_last && threadIdx.x == 0) {
+    __threadfence();
+    double s = 0.0;
+    for (unsigned int b = 0; b < gridDim.x; ++b) s += __ldcg(part + b);
+    *pen_out = (float)s;
+  }
+}
+
+// End of an EWC++ call, first half: prev = params, and the global min / max of running (per-CTA partials, combined by
+// the last CTA, which stores mn and the denominator (mx - mn) + 1e-32 with torch's fp32 roundings).
+__global__ void __launch_bounds__(256) ewc_minmax_kernel(const float* __restrict__ p, const float* __restrict__ running,
+                                                         float* __restrict__ prev, size_t n, size_t skip_lo,
+                                                         size_t skip_hi, float2* __restrict__ part,
+                                                         unsigned int* counter, float* range) {
+  __shared__ float s_mn[8], s_mx[8];
+  __shared__ bool is_last;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float mn = INFINITY, mx = -INFINITY;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if (i >= skip_lo && i < skip_hi) continue;
+    prev[i] = p[i];
+    const float v = running[i];
+    mn = fminf(mn, v);
+    mx = fmaxf(mx, v);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    mn = fminf(mn, __shfl_xor_sync(FULL_MASK, mn, o));
+    mx = fmaxf(mx, __shfl_xor_sync(FULL_MASK, mx, o));
+  }
+  if (lane == 0) {
+    s_mn[warp] = mn;
+    s_mx[warp] = mx;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int k = 1; k < 8; ++k) {
+      s_mn[0] = fminf(s_mn[0], s_mn[k]);
+      s_mx[0] = fmaxf(s_mx[0], s_mx[k]);
+    }
+    part[blockIdx.x] = make_float2(s_mn[0], s_mx[0]);
+    __threadfence();
+    is_last = (atomicAdd(counter, 1u) == gridDim.x - 1);
+  }
+  __syncthreads();
+  if (is_last && threadIdx.x == 0) {
+    __threadfence();
+    float a = INFINITY, b = -INFINITY;
+    for (unsigned int k = 0; k < gridDim.x; ++k) {
+      const float2 v = __ldcg(part + k);
+      a = fminf(a, v.x);
+      b = fmaxf(b, v.y);
+    }
+    range[0] = a;
+    range[1] = __fadd_rn(__fsub_rn(b, a), 1e-32f);
+  }
+}
+
+// Second half: normalized = (running - mn) / ((mx - mn) + 1e-32), an IEEE division.
+__global__ void __launch_bounds__(256) ewc_normalize_kernel(const float* __restrict__ running,
+                                                            float* __restrict__ normalized, size_t n, size_t skip_lo,
+                                                            size_t skip_hi, const float* __restrict__ range) {
+  const float mn = range[0], den = range[1];
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if (i >= skip_lo && i < skip_hi) continue;
+    normalized[i] = __fdiv_rn(__fsub_rn(running[i], mn), den);
   }
 }
 
@@ -919,26 +1074,26 @@ int b200ocl_net_sgd_step(const b200ocl_net_desc* desc, const b200ocl_net_state* 
   float* out_params = dst ? dst->params : st->params;
   float* out_packed = dst ? dst->packed : st->packed;
   B200OCL_CHECK_ARG(out_params && out_packed, "destination state incomplete");
-  size_t skip_lo = 0, skip_hi = 0;
-  if (p.head != 0) {
-    skip_lo = p.lin[0].w_off;
-    skip_hi = p.lin[0].b_off + p.lin[0].out;
-  }
-  size_t blocks = (p.n_params + 255) / 256;
-  const size_t cap = (size_t)8 * sm_count();
-  if (blocks > cap) blocks = cap;
+  size_t skip_lo, skip_hi;
+  sgd_skip_range(p, skip_lo, skip_hi);
+  const unsigned blocks = arena_grid(p, 8, (size_t)-1);
   B200OCL_PROF("sgd", 12.0 * p.n_params, stream);
-  net_sgd_kernel<false><<<(unsigned)blocks, 256, 0, stream>>>(st->params, st->grads, out_params, p.n_params, lr,
+  net_sgd_kernel<false><<<blocks, 256, 0, stream>>>(st->params, st->grads, out_params, p.n_params, lr,
                                                               weight_decay, skip_lo, skip_hi, nullptr, nullptr);
   B200OCL_LAUNCHED();
   return launch_pack(p, out_params, out_packed, stream);
 }
 
-size_t b200ocl_net_sgd_step_clipped_workspace_bytes(const b200ocl_net_desc* desc) {
+// The workspace of the entry points that reduce over the arenas (b200ocl::REDUCE_WS_BYTES); 0 for a bad description.
+static size_t reduce_workspace_bytes(const b200ocl_net_desc* desc) {
   using namespace b200ocl;
   NetPlan p;
   if (!desc || build_plan(*desc, p)) return 0;
-  return align_up((size_t)NORM_MAX_GRID * sizeof(double), 256) + 256;   // partials, then counter and coefficient
+  return REDUCE_WS_BYTES;
+}
+
+size_t b200ocl_net_sgd_step_clipped_workspace_bytes(const b200ocl_net_desc* desc) {
+  return reduce_workspace_bytes(desc);   // partials, then counter and coefficient
 }
 
 int b200ocl_net_sgd_step_clipped(const b200ocl_net_desc* desc, const b200ocl_net_state* st, float lr,
@@ -952,31 +1107,87 @@ int b200ocl_net_sgd_step_clipped(const b200ocl_net_desc* desc, const b200ocl_net
   B200OCL_CHECK_ARG(st->grads, "state has no gradient arena");
   if ((rc = check_workspace("b200ocl_net_sgd_step_clipped", workspace, workspace_bytes,
                             b200ocl_net_sgd_step_clipped_workspace_bytes(desc)))) return rc;
-  unsigned char* base = static_cast<unsigned char*>(workspace);
-  double* part = reinterpret_cast<double*>(base);
-  unsigned int* counter = reinterpret_cast<unsigned int*>(base + align_up((size_t)NORM_MAX_GRID * sizeof(double), 256));
-  float* coef = reinterpret_cast<float*>(counter + 1);
-  size_t skip_lo = 0, skip_hi = 0;
-  if (p.head != 0) {
-    skip_lo = p.lin[0].w_off;
-    skip_hi = p.lin[0].b_off + p.lin[0].out;
-  }
-  size_t blocks = (p.n_params + 255) / 256;
-  size_t cap = (size_t)2 * sm_count();
-  if (cap > NORM_MAX_GRID) cap = NORM_MAX_GRID;
-  const unsigned norm_grid = (unsigned)(blocks < cap ? blocks : cap);
+  double* part = static_cast<double*>(workspace);
+  unsigned int* counter = reduce_counter(workspace);
+  float* coef = reduce_scalars(workspace);
+  size_t skip_lo, skip_hi;
+  sgd_skip_range(p, skip_lo, skip_hi);
+  const unsigned norm_grid = arena_grid(p, 2, NORM_MAX_GRID);
   B200OCL_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), stream));
   B200OCL_PROF("grad_norm", 4.0 * p.n_params, stream);
   grad_norm_kernel<<<norm_grid, 256, 0, stream>>>(st->grads, p.n_params, skip_lo, skip_hi, max_norm, part, counter, coef,
                                                   norm_out);
   B200OCL_LAUNCHED();
-  cap = (size_t)8 * sm_count();
-  if (blocks > cap) blocks = cap;
   B200OCL_PROF("sgd", 16.0 * p.n_params, stream);
-  net_sgd_kernel<true><<<(unsigned)blocks, 256, 0, stream>>>(st->params, st->grads, st->params, p.n_params, lr,
+  net_sgd_kernel<true><<<arena_grid(p, 8, (size_t)-1), 256, 0, stream>>>(st->params, st->grads, st->params, p.n_params, lr,
                                                              weight_decay, skip_lo, skip_hi, coef, st->grads);
   B200OCL_LAUNCHED();
   return launch_pack(p, st->params, st->packed, stream);
+}
+
+static int ewc_setup(const char* entry, const b200ocl_net_desc* desc, const b200ocl_net_state* st,
+                     const b200ocl_ewc_state* ewc, void* workspace, size_t workspace_bytes, b200ocl::NetPlan& p) {
+  using namespace b200ocl;
+  int rc = check_state(desc, st, p);
+  if (rc) return rc;
+  B200OCL_CHECK_ARG(ewc && ewc->running && ewc->tmp && ewc->normalized && ewc->prev, "EWC state incomplete");
+  return check_workspace(entry, workspace, workspace_bytes, REDUCE_WS_BYTES);
+}
+
+size_t b200ocl_net_sgd_step_ewc_workspace_bytes(const b200ocl_net_desc* desc) { return reduce_workspace_bytes(desc); }
+
+int b200ocl_net_sgd_step_ewc(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const b200ocl_ewc_state* ewc,
+                             float lr, float weight_decay, float up, int flags, float ema_keep, float ema_add,
+                             float* penalty_out, void* workspace, size_t workspace_bytes, void* stream_) {
+  using namespace b200ocl;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  NetPlan p;
+  int rc = ewc_setup("b200ocl_net_sgd_step_ewc", desc, st, ewc, workspace, workspace_bytes, p);
+  if (rc) return rc;
+  size_t skip_lo, skip_hi;
+  sgd_skip_range(p, skip_lo, skip_hi);
+  const unsigned grid = arena_grid(p, 8, NORM_MAX_GRID);
+  unsigned int* counter = reduce_counter(workspace);
+  B200OCL_CHECK_ARG(st->grads, "state has no gradient arena");
+  B200OCL_CHECK_ARG((flags & ~(B200OCL_EWC_PENALTY | B200OCL_EWC_EMA)) == 0, "unknown EWC flags");
+  const bool pen = flags & B200OCL_EWC_PENALTY, ema = flags & B200OCL_EWC_EMA;
+  double* part = static_cast<double*>(workspace);
+  float* pen_out = pen ? penalty_out : nullptr;
+  if (pen_out) B200OCL_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), stream));
+  auto kernel = pen ? (ema ? net_sgd_ewc_kernel<true, true> : net_sgd_ewc_kernel<false, true>)
+                    : (ema ? net_sgd_ewc_kernel<true, false> : net_sgd_ewc_kernel<false, false>);
+  B200OCL_PROF("sgd_ewc", 4.0 * p.n_params * (5 + (pen ? 3 : 0) + (ema ? 2 : 0)), stream);
+  kernel<<<grid, 256, 0, stream>>>(st->params, st->grads, ewc->running, ewc->tmp, ewc->normalized, ewc->prev,
+                                   p.n_params, skip_lo, skip_hi, lr, weight_decay, up, ema_keep, ema_add, part, counter,
+                                   pen_out);
+  B200OCL_LAUNCHED();
+  if (penalty_out && !pen) B200OCL_CUDA(cudaMemsetAsync(penalty_out, 0, sizeof(float), stream));
+  return launch_pack(p, st->params, st->packed, stream);
+}
+
+size_t b200ocl_ewc_consolidate_workspace_bytes(const b200ocl_net_desc* desc) { return reduce_workspace_bytes(desc); }
+
+int b200ocl_ewc_consolidate(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const b200ocl_ewc_state* ewc,
+                            void* workspace, size_t workspace_bytes, void* stream_) {
+  using namespace b200ocl;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  NetPlan p;
+  int rc = ewc_setup("b200ocl_ewc_consolidate", desc, st, ewc, workspace, workspace_bytes, p);
+  if (rc) return rc;
+  size_t skip_lo, skip_hi;
+  sgd_skip_range(p, skip_lo, skip_hi);
+  const unsigned grid = arena_grid(p, 8, NORM_MAX_GRID);
+  unsigned int* counter = reduce_counter(workspace);
+  float* range = reduce_scalars(workspace);
+  B200OCL_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), stream));
+  B200OCL_PROF("ewc_consolidate", 12.0 * p.n_params, stream);
+  ewc_minmax_kernel<<<grid, 256, 0, stream>>>(st->params, ewc->running, ewc->prev, p.n_params, skip_lo, skip_hi,
+                                              static_cast<float2*>(workspace), counter, range);
+  B200OCL_LAUNCHED();
+  B200OCL_PROF("ewc_consolidate", 8.0 * p.n_params, stream);
+  ewc_normalize_kernel<<<grid, 256, 0, stream>>>(ewc->running, ewc->normalized, p.n_params, skip_lo, skip_hi, range);
+  B200OCL_LAUNCHED();
+  return B200OCL_OK;
 }
 
 size_t b200ocl_net_eval_workspace_bytes(const b200ocl_net_desc* desc, int N) {

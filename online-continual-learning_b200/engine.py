@@ -8,6 +8,7 @@ torch.optim.SGD (models/resnet.py, utils/setup_elements.py:46-82).
 """
 import ctypes
 from ctypes import c_int, c_int64, c_size_t, c_void_p
+from types import SimpleNamespace
 
 import torch
 
@@ -25,6 +26,10 @@ class NetDesc(ctypes.Structure):
 class NetState(ctypes.Structure):
     _fields_ = [('params', c_void_p), ('grads', c_void_p), ('packed', c_void_p), ('bn_stats', c_void_p),
                 ('bn_tracked', c_void_p)]
+
+
+class EwcState(ctypes.Structure):
+    _fields_ = [('running', c_void_p), ('tmp', c_void_p), ('normalized', c_void_p), ('prev', c_void_p)]
 
 
 class NetInfo(ctypes.Structure):
@@ -385,6 +390,44 @@ class Engine:
                                                  ws.numel(), _stream())
         _native.check(rc, 'b200ocl_net_sgd_step_clipped')
         return norm
+
+    # ------------------------------------------------------------------ EWC++ (agents/ewc_pp.py)
+    def ewc_state(self):
+        """The EWC++ arenas, allocated once per engine and zero at first (ewc_pp.py:16-18 init_fisher): an object with
+        running, tmp, normalized and prev, each an fp32 tensor in the parameter arena's layout."""
+        if getattr(self, '_ewc', None) is None:
+            n = self.info.n_params
+            st = SimpleNamespace(**{name: torch.zeros(n, dtype=torch.float32, device=self.device)
+                                    for name in ('running', 'tmp', 'normalized', 'prev')})
+            st.c = EwcState(st.running.data_ptr(), st.tmp.data_ptr(), st.normalized.data_ptr(), st.prev.data_ptr())
+            lib = _lib()
+            st.ws = _workspace(max(lib.b200ocl_net_sgd_step_ewc_workspace_bytes(ctypes.byref(self.desc)),
+                                   lib.b200ocl_ewc_consolidate_workspace_bytes(ctypes.byref(self.desc))), self.device)
+            st.penalty = torch.zeros(1, dtype=torch.float32, device=self.device)
+            self._ewc = st
+        return self._ewc
+
+    def sgd_step_ewc(self, lr, weight_decay, up, penalty, ema, ema_keep=0.0, ema_add=0.0, want_penalty=False):
+        """One EWC++ step after backward (b200ocl_net_sgd_step_ewc): with ema, update_running_fisher first
+        (running = ema_keep * running + ema_add * tmp, tmp = 0); with penalty, the gradient of up * sum F * (p - prev)^2
+        added to the gradient arena; tmp += g * g; then opt.step().  want_penalty: returns sum F * (p - prev)^2 over the
+        pre-step weights as a device tensor [1] (the next call overwrites it), else None.  Nothing is read back."""
+        st = self.ewc_state()
+        flags = (1 if penalty else 0) | (2 if ema else 0)
+        rc = _lib().b200ocl_net_sgd_step_ewc(ctypes.byref(self.desc), ctypes.byref(self.state.c), ctypes.byref(st.c),
+                                             float(lr), float(weight_decay), float(up), flags, float(ema_keep),
+                                             float(ema_add), st.penalty.data_ptr() if want_penalty else None,
+                                             st.ws.data_ptr(), st.ws.numel(), _stream())
+        _native.check(rc, 'b200ocl_net_sgd_step_ewc')
+        return st.penalty if want_penalty else None
+
+    def ewc_consolidate(self):
+        """The end of an EWC++ call (b200ocl_ewc_consolidate, ewc_pp.py:71-78): prev = params, normalized = running
+        min-max normalised over every tensor."""
+        st = self.ewc_state()
+        rc = _lib().b200ocl_ewc_consolidate(ctypes.byref(self.desc), ctypes.byref(self.state.c), ctypes.byref(st.c),
+                                            st.ws.data_ptr(), st.ws.numel(), _stream())
+        _native.check(rc, 'b200ocl_ewc_consolidate')
 
 
 def ce_loss(logits, labels, want_grad=True, want_per_sample=False, want_correct=False):

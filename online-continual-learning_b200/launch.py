@@ -3,7 +3,8 @@
     python -m b200ocl.launch /path/to/reference/general_main.py --agent ER --retrieve ASER --update ASER ...
 
 The reference tree is put first on sys.path, its registries are patched in place
-(b200ocl.registry.install) and general_main.py is executed with runpy, byte-identical."""
+(b200ocl.registry.install) and general_main.py is executed with runpy, byte-identical.
+B200OCL_EXTRA_AGENTS (comma-separated, e.g. EWC) also registers those opt-in agents (registry.extra_agents)."""
 import os
 import runpy
 import sys
@@ -16,7 +17,8 @@ def main(argv=None):
     script = os.path.abspath(argv[0])
     sys.path.insert(0, os.path.dirname(script))
     from b200ocl import registry
-    registry.install()
+    extra = [k.strip() for k in os.environ.get('B200OCL_EXTRA_AGENTS', '').split(',') if k.strip()]
+    registry.install(extra=extra)
     sys.argv = [script] + argv[1:]
     runpy.run_path(script, run_name='__main__')
 

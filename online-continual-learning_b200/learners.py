@@ -1,8 +1,9 @@
 """Agents of the replay path with the reference surface `cls(model, opt, params)`,
 `.train_learner(x_train, y_train)`, `.evaluate(test_loaders)`:
 ExperienceReplay (agents/exp_replay.py:10-104: ER / MIR / ASER), SupContrastReplay (agents/scr.py:11-69), AGEM
-(agents/agem.py), Lwf (agents/lwf.py), Icarl (agents/icarl.py) and Gdumb (agents/gdumb.py), over ContinualLearner (agents/base.py:14-113) with
-its training tricks (labels trick, separated softmax, kd_trick / kd_trick_star, review trick).
+(agents/agem.py), Lwf (agents/lwf.py), Icarl (agents/icarl.py), Gdumb (agents/gdumb.py) and EWC_pp (agents/ewc_pp.py, registered
+only on request: registry.extra_agents), over ContinualLearner (agents/base.py:14-113) with its training tricks (labels
+trick, separated softmax, kd_trick / kd_trick_star, review trick).
 
 The loop structure, the order of train-mode forwards (they move BN running statistics) and the
 order of buffer operations follow the reference step exactly; what changes is who does the
@@ -759,3 +760,99 @@ class Gdumb(ContinualLearner):
         self.train_mem()                                                                       # :49
         self._raise_label_errors()
         self.after_train()                                                                     # :50
+
+
+def ewc_ema_schedule(n_batches, epochs, fisher_update_after):
+    """Per step of one train_learner call, in order: whether update_running_fisher fires before it (ewc_pp.py:40-41;
+    the counter restarts with every call)."""
+    return [(ep * n_batches + i + 1) % fisher_update_after == 0 for ep in range(epochs) for i in range(n_batches)]
+
+
+def ewc_ema_coefficients(alpha, fisher_update_after):
+    """(keep, add) of running = (1 - alpha) * running + (1/fua * alpha) * tmp: each formed in double, as Python forms
+    it, then rounded to fp32 where torch multiplies with it (ewc_pp.py:104-106)."""
+    return float(np.float32(1. - alpha)), float(np.float32(1. / fisher_update_after * alpha))
+
+
+def ewc_penalty_up(lambda_, task_seen, kd_trick=False, kd_trick_star=False):
+    """The gradient autograd delivers to the regulariser sum F * (p - prev)^2: fp32(lambda) times the kd_trick /
+    kd_trick_star mixing weights (ewc_pp.py:46-51 scale the whole loss, penalty included), multiplied in fp32 from the
+    outermost weight inward, as the backward pass multiplies them (not kd_mix's double w_ce)."""
+    up = np.float32(1.0)
+    if kd_trick_star:
+        up = np.float32(up * np.float32(1 / ((task_seen + 1) ** 0.5)))
+    if kd_trick:
+        up = np.float32(up * np.float32(1 / (task_seen + 1)))
+    return float(np.float32(up * np.float32(lambda_)))
+
+
+class EWC_pp(ContinualLearner):
+    """EWC++ (agents/ewc_pp.py) on the engine.  Per batch: one train-mode forward, the criterion (the labels trick and
+    separated softmax apply, mixed with the distillation term under kd_trick / kd_trick_star), one backward pass, then
+    one fused launch (b200ocl_net_sgd_step_ewc) that runs, per element, the running-Fisher EMA when the host-side
+    schedule says it fires before this batch, the penalty's gradient from the second call on, tmp += g*g and the SGD
+    step.  At the end of each call b200ocl_ewc_consolidate sets prev = params and min-max normalises the running
+    Fisher.  running_fisher, tmp_fisher, normalized_fisher and prev_params are name -> view dicts over the EWC arenas,
+    as the reference's dicts are.  There is no memory; evaluation is the inherited arg-max path."""
+
+    def __init__(self, model, opt, params):
+        if (getattr(params, 'trick', None) or {}).get('ncm_trick'):
+            # the reference's nearest-class-mean evaluation reads self.buffer, which EWC++ does not have
+            raise NotImplementedError('ncm_trick reads a buffer EWC++ does not keep')
+        super().__init__(model, opt, params)
+        self.lambda_ = params.lambda_
+        self.alpha = params.alpha
+        self.fisher_update_after = params.fisher_update_after
+        self._penalty_live = False              # ewc_pp.py:88: prev_params is filled at the end of the first call
+        st = self.engine.ewc_state()
+        names = [n for n, _ in self.model.named_parameters()]
+        views = lambda arena: {n: arena[o:o + k].view(p.shape) for n, (o, k, _), p in
+                               zip(names, self.engine.table, self.model.parameters())}
+        self.running_fisher, self.tmp_fisher = views(st.running), views(st.tmp)
+        self.normalized_fisher, self._prev = views(st.normalized), views(st.prev)
+
+    @property
+    def prev_params(self):
+        """The reference's prev_params: empty until the end of the first call."""
+        return self._prev if self._penalty_live else {}
+
+    def replay_step(self, batch_x, batch_y, batch_y_host, ema=False, meters=None):
+        """One iteration of ewc_pp.py:40-62, with update_running_fisher (ema) folded into the step launch."""
+        if self.grad_sync is not None:
+            raise NotImplementedError('data-parallel EWC++: the Fisher accumulation would have to follow the all-reduce')
+        eng = self.engine
+        lr, wd = self._lr_wd()
+        logits, ws = eng.forward_train(batch_x, slot=0)                              # :43
+        out = self._kd_loss(logits, batch_y, batch_x, want_grad=True, want_correct=meters is not None)   # :44-51
+        eng.backward(batch_x, out['dlogits'], ws)                                    # :58-59
+        up = ewc_penalty_up(self.lambda_, self.task_seen, self._trick['kd_trick'], self._trick['kd_trick_star'])
+        keep, add = ewc_ema_coefficients(self.alpha, self.fisher_update_after)
+        pen = eng.sgd_step_ewc(lr, wd, up, self._penalty_live, ema, keep, add,
+                               want_penalty=meters is not None and self._penalty_live)   # :41, :62-63
+        self.last_loss = out['loss']
+        if meters is not None:
+            loss = out['loss'] if pen is None else out['loss'] + up * pen
+            meters['acc_batch'].update(out['n_correct'] / batch_y.size(0), batch_y.size(0))
+            meters['losses_batch'].update(loss, batch_y.size(0))
+        self._throttle()
+
+    def train_learner(self, x_train, y_train):
+        self.before_train(x_train, y_train)
+        self.engine.pack()
+        self.model = self.model.train()
+        meters = {k: AverageMeter() for k in ('losses_batch', 'acc_batch')}
+        schedule = None
+        for ep in range(self.epoch):
+            stream = StreamFeeder(x_train, y_train, self.batch, self.device)
+            if schedule is None:
+                schedule = ewc_ema_schedule(len(stream), self.epoch, self.fisher_update_after)
+            for i, (batch_x, batch_y, y_host) in enumerate(stream):
+                self.replay_step(batch_x, batch_y, y_host, schedule[ep * len(stream) + i],
+                                 meters if self.verbose else None)
+                if i % 100 == 1 and self.verbose:
+                    print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
+                          .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
+        self.engine.ewc_consolidate()                                                # :71-78
+        self._penalty_live = True
+        self._raise_label_errors()
+        self.after_train()                                                           # :79

@@ -7,10 +7,12 @@ already hold), so `general_main.py` runs unchanged:
 
     import b200ocl; b200ocl.install()          # before main(args); or:  python -m b200ocl.launch general_main.py ...
 
-The agents registered here are ER, SCR, AGEM, LWF, ICARL and GDUMB.  Every other agent / plugin of the reference
-(EWC, CNDPM, the match retrievals) stays registered and untouched.
+The agents registered here are ER, SCR, AGEM, LWF, ICARL and GDUMB.  `extra_agents` holds agents that are only
+registered on request, `install(extra=('EWC',))` (or `B200OCL_EXTRA_AGENTS=EWC` with b200ocl.launch): EWC (EWC++).
+Every other agent / plugin of the reference (EWC unless requested, CNDPM, the match retrievals) stays registered and
+untouched.
 """
-from .learners import AGEM, ExperienceReplay, Gdumb, Icarl, Lwf, SupContrastReplay
+from .learners import AGEM, EWC_pp, ExperienceReplay, Gdumb, Icarl, Lwf, SupContrastReplay
 from .retrieve import ASER_retrieve, MIR_retrieve, Random_retrieve
 from .update import ASER_update, GSSGreedyUpdate, Reservoir_update
 
@@ -21,6 +23,11 @@ agents = {
     'LWF': Lwf,
     'ICARL': Icarl,
     'GDUMB': Gdumb,
+}
+
+# opt-in: install(extra=...) replaces these entries only when named
+extra_agents = {
+    'EWC': EWC_pp,
 }
 
 retrieve_methods = {
@@ -38,15 +45,21 @@ update_methods = {
 _installed = {}
 
 
-def install(reference_name_match=None):
-    """Swap the replay-path entries of the reference registries for the CUDA-backed classes.
-    Returns the dict of what was replaced (also kept for uninstall())."""
+def install(reference_name_match=None, extra=()):
+    """Swap the replay-path entries of the reference registries for the CUDA-backed classes, and the agents of
+    extra_agents named in `extra`.  Returns the dict of what was replaced (also kept for uninstall())."""
     import importlib
+    extra = tuple(extra)
+    unknown = [k for k in extra if k not in extra_agents]
+    if unknown:
+        raise ValueError('unknown extra agent(s) %s; available: %s' % (', '.join(map(repr, unknown)),
+                                                                      ', '.join(sorted(extra_agents))))
     if reference_name_match is None:
         reference_name_match = importlib.import_module('utils.name_match')
     nm = reference_name_match
     replaced = {}
-    for table_name, mine in (('agents', agents), ('retrieve_methods', retrieve_methods),
+    chosen = dict(agents, **{k: extra_agents[k] for k in extra})
+    for table_name, mine in (('agents', chosen), ('retrieve_methods', retrieve_methods),
                              ('update_methods', update_methods)):
         table = getattr(nm, table_name)
         for key, cls in mine.items():
