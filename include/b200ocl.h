@@ -295,6 +295,53 @@ int b200ocl_net_sgd_step_ewc(const b200ocl_net_desc* desc, const b200ocl_net_sta
  * normalized = (running - mn) / ((mx - mn) + 1e-32) with mn / mx the min / max of running over every tensor, in fp32
  * with an IEEE division.  The tensors b200ocl_net_sgd_step skips are left out and untouched.  workspace:
  * b200ocl_ewc_consolidate_workspace_bytes(desc) bytes, no initial contents needed. */
+/* ---------------------------------------------------------------- Adam
+ * torch.optim.Adam (utils/setup_elements.py:76-78, --optimizer Adam) with amsgrad, maximize and decoupled weight
+ * decay off.  The scalars are what torch/optim/adam.py forms in double on the host for one step, each rounded to fp32
+ * as torch converts it to the kernels' op-math type:
+ *   step_size = -(lr / (1 - beta1**step)), bc2_sqrt = (1 - beta2**step)**0.5, bc2_sqrt_inv = 1 / bc2_sqrt (the
+ *   reciprocal formed in double), eps, beta1_c = 1 - beta1, beta2, beta2_c = 1 - beta2, weight_decay;
+ *   grad_scale: with B200OCL_ADAM_GRAD_SCALE the gradient is first replaced by g * grad_scale and written back: the
+ *   review trick's p.grad.clone() / 10. (agents/base.py:84-88), which torch computes as g * fp32(1 / 10.).
+ * Per element, each torch op with its own rounding (fma where torch's kernels contract):
+ *   g' = g + wd * p (when wd != 0; g is not written), exp_avg.lerp_(g', beta1_c),
+ *   exp_avg_sq = exp_avg_sq * beta2 + beta2_c * g' * g', denom = sqrt(exp_avg_sq) / bc2_sqrt + eps,
+ *   p += step_size * exp_avg / denom.
+ * B200OCL_ADAM_FOREACH: the division by bc2_sqrt is an IEEE division, as torch's default multi-tensor path
+ * (_foreach_div_ by a scalar list) rounds it; without, it is a multiplication by bc2_sqrt_inv, as foreach=False
+ * (CUDA Tensor / Python float) rounds it.  Either way the result is bit-identical to that path on the device. */
+typedef struct {
+  float step_size, bc2_sqrt, bc2_sqrt_inv, eps, beta1_c, beta2, beta2_c, weight_decay, grad_scale;
+} b200ocl_adam_scalars;
+
+#define B200OCL_ADAM_FOREACH 1
+#define B200OCL_ADAM_GRAD_SCALE 2
+
+/* One Adam step over flat fp32 buffers of n floats: p, exp_avg m and exp_avg_sq v updated in place, g read (written
+ * only with B200OCL_ADAM_GRAD_SCALE).  One launch. */
+int b200ocl_adam_step(float* p, float* g, float* m, float* v, size_t n, const b200ocl_adam_scalars* s, int flags,
+                      void* stream);
+
+/* Adam state of the network: exp_avg and exp_avg_sq in the parameter arena's layout (n_params floats each). */
+typedef struct {
+  float* exp_avg;
+  float* exp_avg_sq;
+} b200ocl_adam_state;
+
+/* opt.step() of torch.optim.Adam over every tensor that has a gradient, one launch, then `packed` is refreshed as by
+ * b200ocl_net_sgd_step.  The tensors b200ocl_net_sgd_step skips are left untouched in all four arenas (torch creates no
+ * state for a parameter whose .grad is None). */
+int b200ocl_net_adam_step(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const b200ocl_adam_state* adam,
+                          const b200ocl_adam_scalars* s, int flags, void* stream);
+
+/* The EWC++ step of b200ocl_net_sgd_step_ewc with the Adam update of b200ocl_net_adam_step in place of the SGD one, in
+ * the same single launch: EMA, penalty gradient (written back), tmp += g * g, then Adam with that g.  adam_flags:
+ * B200OCL_ADAM_FOREACH only.  workspace: b200ocl_net_sgd_step_ewc_workspace_bytes(desc) bytes. */
+int b200ocl_net_adam_step_ewc(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const b200ocl_ewc_state* ewc,
+                              const b200ocl_adam_state* adam, const b200ocl_adam_scalars* s, int adam_flags, float up,
+                              int flags, float ema_keep, float ema_add, float* penalty_out, void* workspace,
+                              size_t workspace_bytes, void* stream);
+
 size_t b200ocl_ewc_consolidate_workspace_bytes(const b200ocl_net_desc* desc);
 int b200ocl_ewc_consolidate(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const b200ocl_ewc_state* ewc,
                             void* workspace, size_t workspace_bytes, void* stream);

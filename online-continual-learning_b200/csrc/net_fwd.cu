@@ -416,6 +416,140 @@ __global__ void __launch_bounds__(256) ewc_normalize_kernel(const float* __restr
   }
 }
 
+// ----------------------------------------------------------------------------- Adam over the arena
+// torch.optim.Adam's update (amsgrad, maximize and decoupled weight decay off) as torch's CUDA kernels round it, one op
+// at a time, so that the step is bit-identical to the optimizer the caller built:
+//   g' = fma(wd, p, g)                   grad.add(param, alpha=wd), only when wd != 0 (a temporary: g is not written)
+//   m  = lerp(m, g', w1)                 exp_avg.lerp_(grad, 1 - beta1), ATen/native/Lerp.h as nvcc contracts it:
+//                                        fma(w1, g' - m, m) for |w1| < 0.5, else fma(-(g' - m), 1 - w1, g')
+//   v  = fma(c2, g' * g', v * b2)        exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value=1 - beta2)
+//                                        (DeviceAddCmulCdiv.cuh: fma(g', g', v * b2) when the value is 1)
+//   d  = sqrt(v) / bc2_sqrt + eps        FOREACH (torch's default on CUDA, _foreach_div_ by a scalar list): an IEEE
+//                                        division; otherwise CUDA Tensor / Python float, which multiplies by the fp32
+//                                        rounding of the double reciprocal: `bc2` holds that reciprocal
+//   p  = fma(step_size, m / d, p)        param.addcdiv_(exp_avg, denom, value=-(lr / bc1))
+// GDIV first replaces g by the review trick's p.grad.clone() / 10. (also Tensor / Python float: g * fp32(1 / 10.),
+// `gmul`) and writes it back, as p.grad.data.copy_ does.
+struct AdamCoef {
+  float wd, w1, w1c, b2, c2, bc2, eps, step, gmul;   // w1c = 1 - w1 in fp32, as Lerp.h forms it on the device
+};
+
+template <bool FOREACH>
+__device__ __forceinline__ void adam_update(float& w, float gi, float& m, float& v, const AdamCoef& c) {
+  if (c.wd != 0.f) gi = __fmaf_rn(c.wd, w, gi);
+  const float diff = __fsub_rn(gi, m);
+  m = fabsf(c.w1) < 0.5f ? __fmaf_rn(c.w1, diff, m) : __fmaf_rn(-diff, c.w1c, gi);
+  const float vb = __fmul_rn(v, c.b2);
+  v = c.c2 == 1.f ? __fmaf_rn(gi, gi, vb) : __fmaf_rn(c.c2, __fmul_rn(gi, gi), vb);
+  const float s = __fsqrt_rn(v);
+  const float d = __fadd_rn(FOREACH ? __fdiv_rn(s, c.bc2) : __fmul_rn(s, c.bc2), c.eps);
+  w = __fmaf_rn(c.step, __fdiv_rn(m, d), w);
+}
+
+template <bool FOREACH, bool GDIV>
+__global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
+                                                   float* __restrict__ v, size_t n, size_t skip_lo, size_t skip_hi,
+                                                   AdamCoef c) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if (i >= skip_lo && i < skip_hi) continue;   // tensors without a gradient: torch creates no state, steps nothing
+    float gi = g[i];
+    if (GDIV) {
+      gi = __fmul_rn(gi, c.gmul);
+      g[i] = gi;
+    }
+    float w = p[i], mi = m[i], vi = v[i];
+    adam_update<FOREACH>(w, gi, mi, vi, c);
+    p[i] = w;
+    m[i] = mi;
+    v[i] = vi;
+  }
+}
+
+// EWC++ under Adam: the per-element pass of net_sgd_ewc_kernel (EMA, penalty gradient, tmp += g*g) followed by the
+// Adam update in place of the SGD one, in one launch (ewc_pp.py:58-63).
+template <bool EMA, bool PEN, bool FOREACH>
+__global__ void __launch_bounds__(256) net_adam_ewc_kernel(float* __restrict__ p, float* __restrict__ g,
+                                                           float* __restrict__ m, float* __restrict__ v,
+                                                           float* __restrict__ running, float* __restrict__ tmp,
+                                                           const float* __restrict__ fisher,
+                                                           const float* __restrict__ prev, size_t n, size_t skip_lo,
+                                                           size_t skip_hi, AdamCoef c, float up, float ema_keep,
+                                                           float ema_add, double* __restrict__ part,
+                                                           unsigned int* counter, float* pen_out) {
+  double acc = 0.0;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    if (i >= skip_lo && i < skip_hi) continue;
+    float w = p[i];
+    float gi = g[i];
+    float t = tmp[i];
+    if (EMA) {
+      running[i] = __fadd_rn(__fmul_rn(ema_keep, running[i]), __fmul_rn(ema_add, t));
+      t = 0.f;
+    }
+    if (PEN) {
+      const float f = fisher[i];
+      const float d = __fsub_rn(w, prev[i]);
+      gi = __fadd_rn(gi, __fmul_rn(__fmul_rn(up, f), __fmul_rn(2.f, d)));
+      g[i] = gi;
+      const double dd = (double)d;
+      acc = fma((double)f * dd, dd, acc);
+    }
+    tmp[i] = __fadd_rn(t, __fmul_rn(gi, gi));
+    float mi = m[i], vi = v[i];
+    adam_update<FOREACH>(w, gi, mi, vi, c);
+    p[i] = w;
+    m[i] = mi;
+    v[i] = vi;
+  }
+  if (!PEN || !pen_out) return;
+  __shared__ double s_red[8];
+  __shared__ bool is_last;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(FULL_MASK, acc, o);
+  if (lane == 0) s_red[warp] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) s += s_red[k];
+    part[blockIdx.x] = s;
+    __threadfence();
+    is_last = (atomicAdd(counter, 1u) == gridDim.x - 1);
+  }
+  __syncthreads();
+  if (is_last && threadIdx.x == 0) {
+    __threadfence();
+    double s = 0.0;
+    for (unsigned int b = 0; b < gridDim.x; ++b) s += __ldcg(part + b);
+    *pen_out = (float)s;
+  }
+}
+
+// The kernel's coefficients from the caller's scalars; false for unknown flags.
+inline bool adam_coef(const b200ocl_adam_scalars& s, int flags, AdamCoef& c) {
+  if (flags & ~(B200OCL_ADAM_FOREACH | B200OCL_ADAM_GRAD_SCALE)) return false;
+  c.wd = s.weight_decay;
+  c.w1 = s.beta1_c;
+  c.w1c = 1.f - s.beta1_c;
+  c.b2 = s.beta2;
+  c.c2 = s.beta2_c;
+  c.bc2 = (flags & B200OCL_ADAM_FOREACH) ? s.bc2_sqrt : s.bc2_sqrt_inv;
+  c.eps = s.eps;
+  c.step = s.step_size;
+  c.gmul = (flags & B200OCL_ADAM_GRAD_SCALE) ? s.grad_scale : 1.f;
+  return true;
+}
+
+template <bool FOREACH>
+void launch_adam(unsigned grid, cudaStream_t stream, float* p, float* g, float* m, float* v, size_t n, size_t skip_lo,
+                 size_t skip_hi, const AdamCoef& c, bool gdiv) {
+  if (gdiv) adam_kernel<FOREACH, true><<<grid, 256, 0, stream>>>(p, g, m, v, n, skip_lo, skip_hi, c);
+  else adam_kernel<FOREACH, false><<<grid, 256, 0, stream>>>(p, g, m, v, n, skip_lo, skip_hi, c);
+}
+
 // ----------------------------------------------------------------------------- train-mode BN apply
 struct BnApplyArgs {
   const float* z;
@@ -1188,6 +1322,90 @@ int b200ocl_ewc_consolidate(const b200ocl_net_desc* desc, const b200ocl_net_stat
   ewc_normalize_kernel<<<grid, 256, 0, stream>>>(ewc->running, ewc->normalized, p.n_params, skip_lo, skip_hi, range);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
+}
+
+int b200ocl_adam_step(float* p, float* g, float* m, float* v, size_t n, const b200ocl_adam_scalars* s, int flags,
+                      void* stream_) {
+  using namespace b200ocl;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200OCL_CHECK_ARG(s && (n == 0 || (p && g && m && v)), "null pointer");
+  AdamCoef c;
+  B200OCL_CHECK_ARG(adam_coef(*s, flags, c), "unknown Adam flags");
+  if (n == 0) return B200OCL_OK;
+  size_t blocks = (n + 255) / 256;
+  const size_t cap = (size_t)8 * sm_count();
+  if (blocks > cap) blocks = cap;
+  B200OCL_PROF("adam", 28.0 * n, stream);
+  if (flags & B200OCL_ADAM_FOREACH) launch_adam<true>((unsigned)blocks, stream, p, g, m, v, n, 0, 0, c,
+                                                      flags & B200OCL_ADAM_GRAD_SCALE);
+  else launch_adam<false>((unsigned)blocks, stream, p, g, m, v, n, 0, 0, c, flags & B200OCL_ADAM_GRAD_SCALE);
+  B200OCL_LAUNCHED();
+  return B200OCL_OK;
+}
+
+int b200ocl_net_adam_step(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const b200ocl_adam_state* adam,
+                          const b200ocl_adam_scalars* s, int flags, void* stream_) {
+  using namespace b200ocl;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  NetPlan p;
+  int rc = check_state(desc, st, p);
+  if (rc) return rc;
+  B200OCL_CHECK_ARG(st->grads, "state has no gradient arena");
+  B200OCL_CHECK_ARG(adam && adam->exp_avg && adam->exp_avg_sq && s, "Adam state incomplete");
+  AdamCoef c;
+  B200OCL_CHECK_ARG(adam_coef(*s, flags, c), "unknown Adam flags");
+  size_t skip_lo, skip_hi;
+  sgd_skip_range(p, skip_lo, skip_hi);
+  const unsigned blocks = arena_grid(p, 8, (size_t)-1);
+  const bool gdiv = flags & B200OCL_ADAM_GRAD_SCALE;
+  B200OCL_PROF("adam", (gdiv ? 32.0 : 28.0) * p.n_params, stream);
+  if (flags & B200OCL_ADAM_FOREACH) launch_adam<true>(blocks, stream, st->params, st->grads, adam->exp_avg,
+                                                      adam->exp_avg_sq, p.n_params, skip_lo, skip_hi, c, gdiv);
+  else launch_adam<false>(blocks, stream, st->params, st->grads, adam->exp_avg, adam->exp_avg_sq, p.n_params, skip_lo,
+                          skip_hi, c, gdiv);
+  B200OCL_LAUNCHED();
+  return launch_pack(p, st->params, st->packed, stream);
+}
+
+int b200ocl_net_adam_step_ewc(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const b200ocl_ewc_state* ewc,
+                              const b200ocl_adam_state* adam, const b200ocl_adam_scalars* s, int adam_flags, float up,
+                              int flags, float ema_keep, float ema_add, float* penalty_out, void* workspace,
+                              size_t workspace_bytes, void* stream_) {
+  using namespace b200ocl;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  NetPlan p;
+  int rc = ewc_setup("b200ocl_net_adam_step_ewc", desc, st, ewc, workspace, workspace_bytes, p);
+  if (rc) return rc;
+  B200OCL_CHECK_ARG(st->grads, "state has no gradient arena");
+  B200OCL_CHECK_ARG(adam && adam->exp_avg && adam->exp_avg_sq && s, "Adam state incomplete");
+  B200OCL_CHECK_ARG((adam_flags & ~B200OCL_ADAM_FOREACH) == 0, "unknown Adam flags for the EWC++ step");
+  AdamCoef c;
+  B200OCL_CHECK_ARG(adam_coef(*s, adam_flags, c), "unknown Adam flags");
+  B200OCL_CHECK_ARG((flags & ~(B200OCL_EWC_PENALTY | B200OCL_EWC_EMA)) == 0, "unknown EWC flags");
+  size_t skip_lo, skip_hi;
+  sgd_skip_range(p, skip_lo, skip_hi);
+  const unsigned grid = arena_grid(p, 8, NORM_MAX_GRID);
+  unsigned int* counter = reduce_counter(workspace);
+  const bool pen = flags & B200OCL_EWC_PENALTY, ema = flags & B200OCL_EWC_EMA;
+  const bool fe = adam_flags & B200OCL_ADAM_FOREACH;
+  double* part = static_cast<double*>(workspace);
+  float* pen_out = pen ? penalty_out : nullptr;
+  if (pen_out) B200OCL_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), stream));
+  using K = void (*)(float*, float*, float*, float*, float*, float*, const float*, const float*, size_t, size_t, size_t,
+                     AdamCoef, float, float, float, double*, unsigned int*, float*);
+  static const K kernels[8] = {
+      net_adam_ewc_kernel<false, false, false>, net_adam_ewc_kernel<false, false, true>,
+      net_adam_ewc_kernel<false, true, false>,  net_adam_ewc_kernel<false, true, true>,
+      net_adam_ewc_kernel<true, false, false>,  net_adam_ewc_kernel<true, false, true>,
+      net_adam_ewc_kernel<true, true, false>,   net_adam_ewc_kernel<true, true, true>};
+  const K kernel = kernels[(ema ? 4 : 0) + (pen ? 2 : 0) + (fe ? 1 : 0)];
+  B200OCL_PROF("adam_ewc", 4.0 * p.n_params * (10 + (pen ? 3 : 0) + (ema ? 2 : 0)), stream);
+  kernel<<<grid, 256, 0, stream>>>(st->params, st->grads, adam->exp_avg, adam->exp_avg_sq, ewc->running, ewc->tmp,
+                                   ewc->normalized, ewc->prev, p.n_params, skip_lo, skip_hi, c, up, ema_keep, ema_add,
+                                   part, counter, pen_out);
+  B200OCL_LAUNCHED();
+  if (penalty_out && !pen) B200OCL_CUDA(cudaMemsetAsync(penalty_out, 0, sizeof(float), stream));
+  return launch_pack(p, st->params, st->packed, stream);
 }
 
 size_t b200ocl_net_eval_workspace_bytes(const b200ocl_net_desc* desc, int N) {

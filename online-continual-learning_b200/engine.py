@@ -12,7 +12,7 @@ from types import SimpleNamespace
 
 import torch
 
-from . import _native
+from . import _native, ops
 from .ops import _stream, _workspace, _need_cuda
 
 HEAD_CODES = {None: 0, 'classifier': 0, 'linear': 1, 'mlp': 2, 'None': 3}
@@ -30,6 +30,10 @@ class NetState(ctypes.Structure):
 
 class EwcState(ctypes.Structure):
     _fields_ = [('running', c_void_p), ('tmp', c_void_p), ('normalized', c_void_p), ('prev', c_void_p)]
+
+
+class AdamState(ctypes.Structure):
+    _fields_ = [('exp_avg', c_void_p), ('exp_avg_sq', c_void_p)]
 
 
 class NetInfo(ctypes.Structure):
@@ -428,6 +432,45 @@ class Engine:
         rc = _lib().b200ocl_ewc_consolidate(ctypes.byref(self.desc), ctypes.byref(self.state.c), ctypes.byref(st.c),
                                             st.ws.data_ptr(), st.ws.numel(), _stream())
         _native.check(rc, 'b200ocl_ewc_consolidate')
+
+    # ------------------------------------------------------------------ torch.optim.Adam
+    def adam_state(self):
+        """Adam's state, allocated once per engine: exp_avg and exp_avg_sq (fp32, the parameter arena's layout, zero at
+        first) and `step`, the host-side step count shared by every tensor that has a gradient."""
+        if getattr(self, '_adam', None) is None:
+            n = self.info.n_params
+            st = SimpleNamespace(exp_avg=torch.zeros(n, dtype=torch.float32, device=self.device),
+                                 exp_avg_sq=torch.zeros(n, dtype=torch.float32, device=self.device), step=0)
+            st.c = AdamState(st.exp_avg.data_ptr(), st.exp_avg_sq.data_ptr())
+            self._adam = st
+        return self._adam
+
+    def adam_step(self, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, foreach=True, grad_div=None):
+        """opt.step() of torch.optim.Adam (b200ocl_net_adam_step): the step count advances, the scalars are formed on
+        the host as torch forms them, one launch updates params / exp_avg / exp_avg_sq, then the packed weights are
+        refreshed.  grad_div: the gradient arena is divided by it first (the review trick's p.grad.clone() / 10.)."""
+        st = self.adam_state()
+        st.step += 1
+        s = ops.adam_scalars(lr, betas, eps, weight_decay, st.step, grad_div)
+        flags = (ops.ADAM_FOREACH if foreach else 0) | (ops.ADAM_GRAD_SCALE if grad_div is not None else 0)
+        rc = _lib().b200ocl_net_adam_step(ctypes.byref(self.desc), ctypes.byref(self.state.c), ctypes.byref(st.c),
+                                          ctypes.byref(s), flags, _stream())
+        _native.check(rc, 'b200ocl_net_adam_step')
+
+    def adam_step_ewc(self, lr, betas, eps, weight_decay, foreach, up, penalty, ema, ema_keep=0.0, ema_add=0.0,
+                      want_penalty=False):
+        """sgd_step_ewc with torch.optim.Adam's update in place of SGD's (b200ocl_net_adam_step_ewc), one launch."""
+        ewc, st = self.ewc_state(), self.adam_state()
+        st.step += 1
+        s = ops.adam_scalars(lr, betas, eps, weight_decay, st.step)
+        flags = (1 if penalty else 0) | (2 if ema else 0)
+        rc = _lib().b200ocl_net_adam_step_ewc(ctypes.byref(self.desc), ctypes.byref(self.state.c), ctypes.byref(ewc.c),
+                                              ctypes.byref(st.c), ctypes.byref(s), ops.ADAM_FOREACH if foreach else 0,
+                                              float(up), flags, float(ema_keep), float(ema_add),
+                                              ewc.penalty.data_ptr() if want_penalty else None, ewc.ws.data_ptr(),
+                                              ewc.ws.numel(), _stream())
+        _native.check(rc, 'b200ocl_net_adam_step_ewc')
+        return ewc.penalty if want_penalty else None
 
 
 def ce_loss(logits, labels, want_grad=True, want_per_sample=False, want_correct=False):

@@ -11,6 +11,8 @@ arithmetic (the CUDA engine, not autograd) and that dead work is not executed: i
 branch the reference computes and then discards two backward passes (exp_replay.py:55,77,81) --
 their forwards are kept for the BN side effect, their backwards are skipped.
 """
+import collections
+
 import numpy as np
 import torch
 
@@ -120,6 +122,15 @@ def kd_mix(task_seen, kd_trick=False, kd_trick_star=False, lwf=False):
     return w_ce, w_kd
 
 
+class OptimizerSpec(collections.namedtuple('OptimizerSpec', 'kind lr weight_decay betas eps foreach')):
+    """What one opt.step() runs: kind 'sgd' (lr, weight_decay) or 'adam' (also betas, eps and foreach: torch's
+    multi-tensor path, else its single-tensor one; the two round sqrt(v) / bc2_sqrt differently)."""
+    __slots__ = ()
+
+    def __new__(cls, kind, lr, weight_decay, betas=None, eps=None, foreach=None):
+        return super().__new__(cls, kind, lr, weight_decay, betas, eps, foreach)
+
+
 class ContinualLearner(torch.nn.Module):
     """Label bookkeeping and loss dispatch of agents/base.py:14-113 for the replay path."""
 
@@ -160,6 +171,8 @@ class ContinualLearner(torch.nn.Module):
         self.device = self.engine.device
         self.grad_sync = None      # data-parallel stream shards: callable(engine) summing gradients over ranks
         self.grad_world = 1
+        self._adam_started = False  # this learner has stepped Adam (its state is the engine's from then on)
+        self._adam_synced = False   # the engine's Adam state was matched with opt.state in this train_learner call
 
     def _fork(self):
         """(main, side) streams with side ordered after everything issued on main so far."""
@@ -182,28 +195,128 @@ class ContinualLearner(torch.nn.Module):
         if len(ring) > depth:
             ring.pop(0).synchronize()
 
-    def _lr_wd(self):
-        """Step size / weight decay from the optimizer the caller built (run.py:40).  Only plain
-        SGD is implemented (setup_elements.py:73-75, the reference default)."""
+    def _optimizer(self):
+        """The optimizer this step runs, read afresh at every step so that a caller who changes its param group is
+        followed (run.py:40 builds it with setup_opt, setup_elements.py:71-82):
+          * torch.optim.SGD without momentum: OptimizerSpec('sgd', lr, weight_decay);
+          * torch.optim.Adam with one param group and amsgrad, maximize, fused, capturable, differentiable and
+            decoupled_weight_decay off: OptimizerSpec('adam', lr, weight_decay, betas, eps, foreach), foreach being
+            the path torch takes for CUDA parameters (the multi-tensor one unless foreach=False);
+          * opt None: params.optimizer selects, with params.learning_rate / weight_decay and, for 'Adam', the defaults
+            setup_opt's torch.optim.Adam(lr, weight_decay) takes.
+        Anything else raises NotImplementedError (AdamW is an Adam with decoupled_weight_decay=True)."""
         opt = self.opt
         if opt is None:
-            return float(self.params.learning_rate), float(getattr(self.params, 'weight_decay', 0.0))
-        if not isinstance(opt, torch.optim.SGD):
-            raise NotImplementedError('the b200ocl engine implements torch.optim.SGD only')
+            name = getattr(self.params, 'optimizer', 'SGD')
+            lr, wd = float(self.params.learning_rate), float(getattr(self.params, 'weight_decay', 0.0))
+            if name == 'SGD':
+                return OptimizerSpec('sgd', lr, wd)
+            if name == 'Adam':
+                return OptimizerSpec('adam', lr, wd, (0.9, 0.999), 1e-8, True)
+            raise NotImplementedError('the b200ocl engine implements SGD and Adam, not %r' % name)
+        if isinstance(opt, torch.optim.SGD):
+            g = opt.param_groups[0]
+            if g.get('momentum', 0) or g.get('nesterov', False) or g.get('dampening', 0):
+                raise NotImplementedError('SGD momentum/nesterov are not used by the reference and not implemented')
+            return OptimizerSpec('sgd', float(g['lr']), float(g['weight_decay']))
+        if not isinstance(opt, torch.optim.Adam):
+            raise NotImplementedError('the b200ocl engine implements torch.optim.SGD and torch.optim.Adam, not %s'
+                                      % type(opt).__name__)
+        if len(opt.param_groups) != 1:
+            raise NotImplementedError('Adam with %d param groups: the engine steps one' % len(opt.param_groups))
         g = opt.param_groups[0]
-        if g.get('momentum', 0) or g.get('nesterov', False) or g.get('dampening', 0):
-            raise NotImplementedError('SGD momentum/nesterov are not used by the reference and not implemented')
-        return float(g['lr']), float(g['weight_decay'])
+        for k in ('amsgrad', 'maximize', 'fused', 'capturable', 'differentiable', 'decoupled_weight_decay'):
+            if g.get(k):
+                raise NotImplementedError('Adam with %s=True is not implemented (AdamW: decoupled_weight_decay)' % k)
+        return OptimizerSpec('adam', float(g['lr']), float(g['weight_decay']),
+                             (float(g['betas'][0]), float(g['betas'][1])), float(g['eps']), g.get('foreach') is not False)
 
-    def _optimizer_step(self, lr, wd):
-        """opt.step(); with data-parallel stream shards the summed gradient is averaged first
-        (one all-reduce of the flat gradient arena, folded into the step size)."""
+    def _optimizer_step(self, spec, review=False):
+        """opt.step() with the optimizer `spec` describes.  review: the review trick's step on p.grad.clone() / 10.
+        (agents/base.py:84-88); for SGD that is SGD(lr / 10, 10 * wd) on the gradient, for Adam the division is made
+        on the device and written back to the gradient arena.  With data-parallel stream shards the summed gradient is
+        averaged first (one all-reduce of the flat gradient arena, folded into SGD's step size)."""
+        if spec.kind == 'adam':
+            if self.grad_sync is not None:
+                raise NotImplementedError('data-parallel Adam: the gradient average cannot be folded into its step')
+            self._adam_begin()
+            self.engine.adam_step(spec.lr, spec.betas, spec.eps, spec.weight_decay, spec.foreach,
+                                  grad_div=10.0 if review else None)
+            return
+        lr, wd = (spec.lr / 10.0, spec.weight_decay * 10.0) if review else (spec.lr, spec.weight_decay)
         if self.grad_sync is not None:
             self.grad_sync(self.engine)
             if wd != 0.0:
                 raise NotImplementedError('weight decay with gradient averaging')
             lr = lr / self.grad_world
         self.engine.sgd_step(lr, wd)
+
+    def _begin_call(self):
+        """Start of a train_learner call that steps self.opt: an optimizer the engine cannot step is refused before
+        anything launches, and the Adam state is matched with opt.state again at the call's first step."""
+        if self._optimizer().kind == 'adam' and self.grad_sync is not None:
+            raise NotImplementedError('data-parallel Adam: the gradient average cannot be folded into its step')
+        self._adam_synced = False
+
+    def _end_call(self):
+        """End of a train_learner call, after after_train (and its review trick): opt.state shows the Adam state."""
+        self._adam_export()
+
+    # ------------------------------------------------------------------ Adam state (torch.optim.Adam.state)
+    def _stepped(self):
+        """[(parameter, arena offset, numel)] of the tensors the optimizer steps (the ones with a gradient)."""
+        return [(p, o, n) for p, (o, n, hg) in zip(self.model.parameters(), self.engine.table) if hg]
+
+    def _adam_begin(self):
+        """Before the first Adam step of a train_learner call: make the engine's Adam state the optimizer's.  When the
+        caller's opt.state already holds the arenas (a previous call of this learner exported them) nothing moves.
+        Otherwise its state for the stepped tensors (a resumed or load_state_dict-ed optimizer) is copied into the
+        arenas; every stepped tensor must then carry state with one common step.  A fresh optimizer (no state, or opt
+        None on this learner's first step) starts from zero moments and step 0."""
+        if self._adam_synced:
+            return
+        self._adam_synced = True
+        st = self.engine.adam_state()
+        if self.opt is None:
+            if not self._adam_started:
+                st.exp_avg.zero_(), st.exp_avg_sq.zero_()
+                st.step = 0
+            self._adam_started = True
+            return
+        self._adam_started = True
+        stepped = self._stepped()
+        states = [self.opt.state.get(p) or {} for p, _, _ in stepped]
+        if all(s.get('exp_avg') is not None and s['exp_avg'].data_ptr() == st.exp_avg[o:o + n].data_ptr()
+               and s.get('exp_avg_sq') is not None and s['exp_avg_sq'].data_ptr() == st.exp_avg_sq[o:o + n].data_ptr()
+               and float(s['step']) == st.step for s, (_, o, n) in zip(states, stepped)):
+            return
+        if not any(states):
+            st.exp_avg.zero_(), st.exp_avg_sq.zero_()
+            st.step = 0
+            return
+        steps = set()
+        for s, (p, o, n) in zip(states, stepped):
+            if not all(k in s for k in ('step', 'exp_avg', 'exp_avg_sq')):
+                raise ValueError('Adam state covers some of the stepped tensors only: the engine steps all of them '
+                                 'with one step count')
+            steps.add(float(s['step']))
+            st.exp_avg[o:o + n].copy_(s['exp_avg'].detach().reshape(-1))
+            st.exp_avg_sq[o:o + n].copy_(s['exp_avg_sq'].detach().reshape(-1))
+        if len(steps) != 1:
+            raise ValueError('Adam state with different step counts %s: the engine steps every tensor together'
+                             % sorted(steps))
+        st.step = int(steps.pop())
+
+    def _adam_export(self):
+        """After train_learner: opt.state[p] = {'step', 'exp_avg', 'exp_avg_sq'} with torch's keys and dtypes for every
+        stepped tensor, the moments as views of the arenas (so opt.state_dict() reflects the engine)."""
+        if self.opt is None or not self._adam_started:
+            return
+        st = self.engine.adam_state()
+        for p, o, n in self._stepped():
+            self.opt.state[p] = {'step': torch.tensor(float(st.step), dtype=torch.float32),
+                                 'exp_avg': st.exp_avg[o:o + n].view(p.shape),
+                                 'exp_avg_sq': st.exp_avg_sq[o:o + n].view(p.shape)}
 
     def before_train(self, x_train, y_train):
         new_labels = list(set(np.asarray(y_train).tolist()))
@@ -272,7 +385,7 @@ class ContinualLearner(torch.nn.Module):
         pass over the filled memory in shuffled batches of eps_mem_batch (drop_last), gradients divided by 10.
         g/10 followed by SGD(lr, wd) is p -= lr*(g/10 + wd*p) = SGD(lr/10, 10*wd) on g: folded into the step."""
         eng = self.engine
-        lr, wd = self._lr_wd()
+        spec = self._optimizer()
         n = self.buffer.current_index
         bs = self.params.eps_mem_batch
         if n == 0 or n < bs:
@@ -301,7 +414,7 @@ class ContinualLearner(torch.nn.Module):
             else:
                 ce = self.criterion(out, by)                                         # base.py:80 (tricks apply, no KD)
                 eng.backward(bx, ce['dlogits'], ws)
-            self._optimizer_step(lr / 10.0, wd * 10.0)                               # base.py:83-87
+            self._optimizer_step(spec, review=True)                                  # base.py:83-88
             self._throttle()
 
     def train_learner(self, x_train, y_train):
@@ -374,7 +487,7 @@ class ExperienceReplay(ContinualLearner):
     def replay_step(self, batch_x, batch_y, batch_y_host, meters=None):
         """One iteration of exp_replay.py:34-92."""
         eng = self.engine
-        lr, wd = self._lr_wd()
+        spec = self._optimizer()
         aser = self._aser_branch
         # in the ASER branch the stream and memory losses reach only the meters (and MIR's virtual step): their
         # distillation terms, and so the teacher forwards, are skipped when nothing reads them
@@ -425,7 +538,7 @@ class ExperienceReplay(ContinualLearner):
                 self.last_loss = ce_c['loss']
             else:
                 self.last_loss = ce['loss']
-            self._optimizer_step(lr, wd)                                            # :87 / :89
+            self._optimizer_step(spec)                                            # :87 / :89
         # (Not overlapped with the FOLLOWING iteration's first forward on a second stream: the update's eval-feature pass
         # runs persistent one-CTA-per-SM kernels the forward cannot share the SMs with, and the host then waits for the
         # update's decision at the next retrieval.)
@@ -433,6 +546,7 @@ class ExperienceReplay(ContinualLearner):
         self._throttle()
 
     def train_learner(self, x_train, y_train):
+        self._begin_call()
         self.before_train(x_train, y_train)
         self.engine.pack()          # the caller may have written the Parameters (load_state_dict, weight surgery)
         self.model = self.model.train()
@@ -448,6 +562,7 @@ class ExperienceReplay(ContinualLearner):
                           .format(i, meters['losses_mem'].avg(), meters['acc_mem'].avg()))
         self._raise_label_errors()
         self.after_train()
+        self._end_call()
 
 
 class SupContrastReplay(ContinualLearner):
@@ -463,7 +578,7 @@ class SupContrastReplay(ContinualLearner):
     def replay_step(self, batch_x, batch_y, batch_y_host, meters=None):
         """One iteration of scr.py:40-63."""
         eng = self.engine
-        lr, wd = self._lr_wd()
+        spec = self._optimizer()
         for _ in range(self.mem_iters):
             mem_x, mem_y = self.buffer.retrieve(x=batch_x, y=batch_y)               # :47
             if mem_x.size(0) > 0:                                                   # :49 (no training on an empty buffer)
@@ -495,7 +610,7 @@ class SupContrastReplay(ContinualLearner):
                     loss, dfeat = ops.supcon(feats, labels, self.params.temp)       # :56  (base.py:109-111)
                     eng.backward(combined, dfeat[:, 0].contiguous(), ws1)           # :58-59
                     eng.backward(combined_aug, dfeat[:, 1].contiguous(), ws2, accumulate=True)
-                self._optimizer_step(lr, wd)                                        # :60
+                self._optimizer_step(spec)                                        # :60
                 self.last_loss = loss
                 if meters is not None:
                     meters['losses'].update(loss, batch_y.size(0))
@@ -503,6 +618,7 @@ class SupContrastReplay(ContinualLearner):
         self._throttle()
 
     def train_learner(self, x_train, y_train):
+        self._begin_call()
         self.before_train(x_train, y_train)
         self.engine.pack()          # the caller may have written the Parameters (load_state_dict, weight surgery)
         self.model = self.model.train()
@@ -514,6 +630,7 @@ class SupContrastReplay(ContinualLearner):
                 if i % 100 == 1 and self.verbose:
                     print('==>>> it: {}, avg. loss: {:.6f}, '.format(i, meters['losses'].avg()))
         self.after_train()
+        self._end_call()
 
 
 class AGEM(ContinualLearner):
@@ -532,7 +649,7 @@ class AGEM(ContinualLearner):
     def replay_step(self, batch_x, batch_y, batch_y_host, meters=None):
         """One iteration of agem.py:36-84."""
         eng = self.engine
-        lr, wd = self._lr_wd()
+        spec = self._optimizer()
         for _ in range(self.mem_iters):
             logits, ws = eng.forward_train(batch_x, slot=0)                          # :39
             ce = self._kd_loss(logits, batch_y, batch_x, want_grad=True, want_correct=meters is not None)   # :40-46
@@ -549,11 +666,12 @@ class AGEM(ContinualLearner):
                     ce_m = self.criterion(mem_logits, mem_y)                         # :66 (no distillation term)
                     eng.backward(mem_x, ce_m['dlogits'], ws_m)                       # :67-68 -> grad_ref in the arena
                     ops.agem_project(self._g_cur, eng.state.grads, out=eng.state.grads)   # :73-80
-            self._optimizer_step(lr, wd)                                             # :81
+            self._optimizer_step(spec)                                             # :81
         self.buffer.update(batch_x, batch_y, y_host=batch_y_host)                    # :83
         self._throttle()
 
     def train_learner(self, x_train, y_train):
+        self._begin_call()
         self.before_train(x_train, y_train)
         self.engine.pack()
         self.model = self.model.train()
@@ -567,6 +685,7 @@ class AGEM(ContinualLearner):
                           .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
         self._raise_label_errors()
         self.after_train()
+        self._end_call()
 
 
 class Lwf(ContinualLearner):
@@ -577,18 +696,19 @@ class Lwf(ContinualLearner):
     def replay_step(self, batch_x, batch_y, batch_y_host, meters=None):
         """One iteration of lwf.py:30-46."""
         eng = self.engine
-        lr, wd = self._lr_wd()
+        spec = self._optimizer()
         logits, ws = eng.forward_train(batch_x, slot=0)                              # :35
         out = self._kd_loss(logits, batch_y, batch_x, want_grad=True, want_correct=meters is not None)   # :36-38
         if meters is not None:
             meters['acc_batch'].update(out['n_correct'] / batch_y.size(0), batch_y.size(0))
             meters['losses_batch'].update(out['loss'], batch_y.size(0))
         eng.backward(batch_x, out['dlogits'], ws)                                    # :45-46
-        self._optimizer_step(lr, wd)                                                 # :47
+        self._optimizer_step(spec)                                                 # :47
         self.last_loss = out['loss']
         self._throttle()
 
     def train_learner(self, x_train, y_train):
+        self._begin_call()
         self.before_train(x_train, y_train)
         self.engine.pack()
         self.model = self.model.train()
@@ -602,6 +722,7 @@ class Lwf(ContinualLearner):
                           .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
         self._raise_label_errors()
         self.after_train()
+        self._end_call()
 
 
 class Icarl(ContinualLearner):
@@ -638,7 +759,7 @@ class Icarl(ContinualLearner):
     def replay_step(self, batch_x, batch_y, batch_y_host, meters=None):
         """One iteration of icarl.py:37-65."""
         eng = self.engine
-        lr, wd = self._lr_wd()
+        spec = self._optimizer()
         pos, n_old, K = self._pos
         B = batch_x.size(0)
         if K > eng.out_dim:
@@ -673,13 +794,14 @@ class Icarl(ContinualLearner):
         out = icarl_loss(logits, batch_y, pos, K, n_old if teacher is not None else 0, teacher=teacher,
                          err=self._pos_err)                                          # :43-62
         eng.backward(x, out['dlogits'], ws)                                          # :63
-        self._optimizer_step(lr, wd)                                                 # :64
+        self._optimizer_step(spec)                                                 # :64
         self.last_loss = out['loss']
         slots = self.buffer.update(batch_x, batch_y, y_host=batch_y_host)            # :65
         self._updated[np.asarray(slots, dtype=np.int64)] = True
         self._throttle()
 
     def train_learner(self, x_train, y_train):
+        self._begin_call()
         self.before_train(x_train, y_train)
         self.engine.pack()
         self.model = self.model.train()
@@ -695,6 +817,7 @@ class Icarl(ContinualLearner):
         self._prev_live = True
         self._raise_label_errors()
         self.after_train()
+        self._end_call()
 
 
 class Gdumb(ContinualLearner):
@@ -821,14 +944,20 @@ class EWC_pp(ContinualLearner):
         if self.grad_sync is not None:
             raise NotImplementedError('data-parallel EWC++: the Fisher accumulation would have to follow the all-reduce')
         eng = self.engine
-        lr, wd = self._lr_wd()
+        spec = self._optimizer()
         logits, ws = eng.forward_train(batch_x, slot=0)                              # :43
         out = self._kd_loss(logits, batch_y, batch_x, want_grad=True, want_correct=meters is not None)   # :44-51
         eng.backward(batch_x, out['dlogits'], ws)                                    # :58-59
         up = ewc_penalty_up(self.lambda_, self.task_seen, self._trick['kd_trick'], self._trick['kd_trick_star'])
         keep, add = ewc_ema_coefficients(self.alpha, self.fisher_update_after)
-        pen = eng.sgd_step_ewc(lr, wd, up, self._penalty_live, ema, keep, add,
-                               want_penalty=meters is not None and self._penalty_live)   # :41, :62-63
+        want = meters is not None and self._penalty_live
+        if spec.kind == 'adam':                                                      # :41, :62-63
+            self._adam_begin()
+            pen = eng.adam_step_ewc(spec.lr, spec.betas, spec.eps, spec.weight_decay, spec.foreach, up,
+                                    self._penalty_live, ema, keep, add, want_penalty=want)
+        else:
+            pen = eng.sgd_step_ewc(spec.lr, spec.weight_decay, up, self._penalty_live, ema, keep, add,
+                                   want_penalty=want)
         self.last_loss = out['loss']
         if meters is not None:
             loss = out['loss'] if pen is None else out['loss'] + up * pen
@@ -837,6 +966,7 @@ class EWC_pp(ContinualLearner):
         self._throttle()
 
     def train_learner(self, x_train, y_train):
+        self._begin_call()
         self.before_train(x_train, y_train)
         self.engine.pack()
         self.model = self.model.train()
@@ -856,3 +986,4 @@ class EWC_pp(ContinualLearner):
         self._penalty_live = True
         self._raise_label_errors()
         self.after_train()                                                           # :79
+        self._end_call()

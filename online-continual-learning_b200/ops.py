@@ -4,6 +4,8 @@ Every function takes CUDA torch tensors, hands raw device pointers and the curre
 CUDA stream to libb200ocl.so and returns torch tensors.  torch is used for memory and
 streams only.  Non-CUDA inputs raise: there is no CPU path.
 """
+import ctypes
+
 import torch
 
 from . import _native
@@ -286,3 +288,46 @@ def sgd_step(param, grad, lr, weight_decay=0.0, out=None):
                                         float(weight_decay), _stream())
     _native.check(rc, 'b200ocl_sgd_step')
     return out
+
+
+class AdamScalars(ctypes.Structure):
+    """b200ocl_adam_scalars."""
+    _fields_ = [(n, ctypes.c_float) for n in ('step_size', 'bc2_sqrt', 'bc2_sqrt_inv', 'eps', 'beta1_c', 'beta2',
+                                              'beta2_c', 'weight_decay', 'grad_scale')]
+
+
+ADAM_FOREACH, ADAM_GRAD_SCALE = 1, 2
+
+
+def adam_scalars(lr, betas, eps, weight_decay, step, grad_div=None):
+    """The scalars of Adam step number `step` (1-based), formed in double exactly as torch/optim/adam.py forms them
+    for a float step counter (the foreach and single-tensor paths give the same doubles), then rounded to fp32 by
+    ctypes as torch converts them to the kernels' op-math type.  A CUDA tensor divided by a Python float is multiplied
+    by the reciprocal formed in double: bc2_sqrt_inv (foreach=False) and grad_scale = 1 / grad_div."""
+    beta1, beta2 = float(betas[0]), float(betas[1])
+    step = float(step)
+    bias_correction1 = 1 - beta1 ** step
+    bias_correction2 = 1 - beta2 ** step
+    step_size = (float(lr) / bias_correction1) * -1
+    bias_correction2_sqrt = bias_correction2 ** 0.5
+    return AdamScalars(step_size, bias_correction2_sqrt, 1 / bias_correction2_sqrt, float(eps), 1 - beta1, beta2,
+                       1 - beta2, float(weight_decay), 1 / float(grad_div) if grad_div is not None else 1.0)
+
+
+def adam_step(param, grad, exp_avg, exp_avg_sq, step, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0,
+              foreach=True, grad_div=None):
+    """One torch.optim.Adam step (step = the state's step count after it, 1 for the first) over flat fp32 buffers, all
+    updated in place; bit-identical to torch's multi-tensor path (foreach=True, its default on CUDA) or its
+    single-tensor path (foreach=False).  grad_div: grad /= grad_div first (written back), as the review trick does."""
+    _need_cuda(param, grad, exp_avg, exp_avg_sq)
+    for t in (param, grad, exp_avg, exp_avg_sq):
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise ValueError('adam_step needs contiguous fp32 tensors')
+        if t.numel() != param.numel():
+            raise ValueError('size mismatch')
+    s = adam_scalars(lr, betas, eps, weight_decay, step, grad_div)
+    flags = (ADAM_FOREACH if foreach else 0) | (ADAM_GRAD_SCALE if grad_div is not None else 0)
+    rc = _native.lib().b200ocl_adam_step(_ptr(param), _ptr(grad), _ptr(exp_avg), _ptr(exp_avg_sq), param.numel(),
+                                         ctypes.byref(s), flags, _stream())
+    _native.check(rc, 'b200ocl_adam_step')
+    return param
