@@ -213,6 +213,25 @@ typedef struct {
 } b200ocl_net_ws_layout;
 int b200ocl_net_train_ws_layout(const b200ocl_net_desc* desc, int N, int layer, b200ocl_net_ws_layout* out);
 
+/* The convolution kernel one launch runs, with its template parameters and grid.  kernel: 0 stem, 1 wgmma fed from a
+ * halo strip (conv_tcp.cu, template nt), 2 wgmma with im2col tiles (conv_tc.cu, nt), 3 patch (bn, pt), 4 tiled (bn, pt),
+ * 5 k-split (pt, kwarps), -1 none covers it.  th / tw / ti: the patch kernel's spatial tile.  stat_bytes: the batch-statistics
+ * partials a train-mode launch writes (grid_x * channels * 2 doubles; 0 for the other passes); stat_region: the bytes
+ * the workspace keeps for them.  sms: the SM count the plan is for. */
+typedef struct {
+  int kernel;
+  int nt, bn, pt, kwarps;
+  int grid_x, grid_y;
+  int th, tw, ti;
+  size_t stat_bytes, stat_region;
+  int sms;
+} b200ocl_conv_geom;
+/* The launch of conv layer `layer` (BatchNorm2d module order) over N images in pass 0 train-mode forward, 1 eval-mode
+ * forward or 2 data gradient (layers >= 1), on a GPU with sms SMs (0: the current device), and the statistics region of
+ * the train workspace of N images planned for that SM count.  Host only, launches nothing; exists so that tests can
+ * check which kernels a batch size reaches and that the workspace holds what they write on any SM count. */
+int b200ocl_net_conv_geom(const b200ocl_net_desc* desc, int N, int layer, int pass, int sms, b200ocl_conv_geom* out);
+
 int b200ocl_net_forward_train(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const float* x, int N,
                               float* out, void* workspace, size_t workspace_bytes, void* stream);
 
@@ -415,6 +434,10 @@ int b200ocl_selftest_umma_tf32(const float* A, const float* B, float* D, int N, 
  * B200OCL_EUNSUPPORTED when the path does not cover the shape.  Path 3 covers 3x3 stride-1 convolutions in every mode
  * but 2: train mode, stride 2 and 1x1 return B200OCL_EUNSUPPORTED. */
 size_t b200ocl_conv_selftest_workspace_bytes(int N, int cin, int cout, int H, int W, int ks, int stride);
+/* Host only: the launch b200ocl_conv_selftest makes for these arguments on a GPU with sms SMs (0: the current device),
+ * and in stat_region the statistics region its workspace keeps for that SM count. */
+int b200ocl_conv_selftest_geom(int N, int H, int W, int cin, int cout, int ks, int stride, int dgrad, int path, int mode,
+                               int sms, b200ocl_conv_geom* out);
 int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N, int H, int W, int cin, int cout,
                           int ks, int stride, int dgrad, int path, int mode, float* stats_out, void* workspace,
                           size_t workspace_bytes, void* stream);

@@ -40,6 +40,7 @@ SIGNATURES = {
     'b200ocl_net_features_eval': (c_int, [P, P, P, c_int, P, P, c_size_t, P]),
     'b200ocl_net_train_workspace_bytes': (c_size_t, [P, c_int]),
     'b200ocl_net_train_ws_layout': (c_int, [P, c_int, c_int, P]),
+    'b200ocl_net_conv_geom': (c_int, [P, c_int, c_int, c_int, c_int, P]),
     'b200ocl_net_forward_train': (c_int, [P, P, P, c_int, P, P, c_size_t, P]),
     'b200ocl_net_forward_evalgrad': (c_int, [P, P, P, c_int, P, P, c_size_t, P]),
     'b200ocl_net_forward_train_deferred': (c_int, [P, P, P, c_int, P, P, c_size_t, P]),
@@ -63,6 +64,8 @@ SIGNATURES = {
     'b200ocl_scr_augment': (c_int, [P, P, P, c_int, c_int, c_int, P]),
     'b200ocl_aser_replace': (c_int, [P, c_int, c_int, P, P, P, c_int, c_size_t, P, P, P, P]),
     'b200ocl_conv_selftest_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
+    'b200ocl_conv_selftest_geom': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                           P]),
     'b200ocl_conv_selftest': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P, P, c_size_t, P]),
     'b200ocl_selftest_umma_tf32': (c_int, [P, P, P, c_int, c_int, c_int, P, P]),
     'b200ocl_selftest_umma_window': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, P, P]),

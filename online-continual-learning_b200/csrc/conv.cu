@@ -545,12 +545,12 @@ __global__ void __launch_bounds__(32 * KS, (KS == 4 ? 4 : 1)) conv_ksplit_kernel
 }
 
 template <int PT, int KS>
-int launch_conv_ksplit(const ConvArgs& a, cudaStream_t stream) {
+int launch_conv_ksplit(const ConvArgs& a, const ConvPlan& pl, cudaStream_t stream) {
   constexpr int BM = 32 * PT;
   constexpr int NST = (PT == 1 && KS == 4) ? 4 : 3;
   constexpr size_t smem = (size_t)(NST * KS * (BM * 20 + 400)) * sizeof(float) + 4 * BM * sizeof(int);
   B200OCL_CUDA((raise_smem_limit<conv_ksplit_kernel<PT, KS>>(smem)));
-  dim3 grid((a.M + BM - 1) / BM, a.CN / 20);
+  dim3 grid(pl.grid_x, pl.grid_y);
   B200OCL_PROF(a.transposed ? "conv_dgrad" : (a.mode == CONV_EVAL ? "conv_eval" : "conv_train"),
                2.0 * a.M * (double)a.CN * a.CK * a.ks * a.ks, stream);
   conv_ksplit_kernel<PT, KS><<<grid, 32 * KS, smem, stream>>>(a);
@@ -685,51 +685,89 @@ inline PatchTile patch_tile(const ConvArgs& a, int bn, int pt) {
 }
 
 template <int BN, int PT>
-int launch_conv_patch(ConvArgs a, const PatchTile& t, cudaStream_t stream) {
-  a.th = t.th; a.tw = t.tw; a.ti = t.ti;
-  B200OCL_CUDA((raise_smem_limit<conv_patch_kernel<BN, PT>>(t.smem)));
-  dim3 grid((unsigned)(t.ctas / (a.CN / BN)), a.CN / BN);
+int launch_conv_patch(ConvArgs a, const ConvPlan& pl, cudaStream_t stream) {
+  a.th = pl.th; a.tw = pl.tw; a.ti = pl.ti;
+  B200OCL_CUDA((raise_smem_limit<conv_patch_kernel<BN, PT>>(pl.smem)));
+  dim3 grid(pl.grid_x, pl.grid_y);
   B200OCL_PROF(a.flip ? "conv_dgrad" : (a.mode == CONV_EVAL ? "conv_eval" : "conv_train"),
                2.0 * a.M * (double)a.CN * a.CK * a.ks * a.ks, stream);
-  conv_patch_kernel<BN, PT><<<grid, CONV_THREADS, t.smem, stream>>>(a);
+  conv_patch_kernel<BN, PT><<<grid, CONV_THREADS, pl.smem, stream>>>(a);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }
 
 template <int BN, int PT>
-int launch_conv_cfg(const ConvArgs& a, cudaStream_t stream) {
+int launch_conv_cfg(const ConvArgs& a, const ConvPlan& pl, cudaStream_t stream) {
   constexpr int WN = BN / 20, WM = 4 / WN, BM = WM * 32 * PT;
   constexpr size_t smem = (size_t)(3 * BM * 20 + 3 * 20 * BN) * sizeof(float) + 4 * BM * sizeof(int);
   B200OCL_CUDA((raise_smem_limit<conv_kernel<BN, PT>>(smem)));
-  dim3 grid((a.M + BM - 1) / BM, a.CN / BN);
+  dim3 grid(pl.grid_x, pl.grid_y);
   B200OCL_PROF(a.transposed ? "conv_dgrad" : (a.mode == CONV_EVAL ? "conv_eval" : "conv_train"), 2.0 * a.M * (double)a.CN * a.CK * a.ks * a.ks, stream);
   conv_kernel<BN, PT><<<grid, CONV_THREADS, smem, stream>>>(a);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }
 
+int launch_stem(const ConvArgs& a, const ConvPlan& pl, cudaStream_t stream) {
+  B200OCL_PROF(a.mode == CONV_EVAL ? "conv_eval" : "conv_train", 2.0 * a.M * 20.0 * 27.0, stream);
+  stem_kernel<<<pl.grid_x, CONV_THREADS, 0, stream>>>(a);
+  B200OCL_LAUNCHED();
+  return B200OCL_OK;
+}
+
+ConvPlan none(const char* why) {
+  ConvPlan pl{};
+  pl.kernel = CONV_K_NONE;
+  pl.why = why;
+  return pl;
+}
+
+ConvPlan tiled(const ConvArgs& a, int kernel, int bn, int pt, int bm) {
+  ConvPlan pl{};
+  pl.kernel = kernel;
+  pl.bn = bn;
+  pl.pt = pt;
+  pl.grid_x = (a.M + bm - 1) / bm;
+  pl.grid_y = a.CN / bn;
+  return pl;
+}
+
 }  // namespace
 
-int conv_max_grid_m(int M) { return (M + 31) / 32; }
-
-int launch_conv(const ConvArgs& a, cudaStream_t stream) {
-  if (a.CK % 20 != 0 || a.CN % 20 != 0 || a.M <= 0) {
-    set_error("launch_conv: channel counts must be multiples of 20 (CK=%d CN=%d M=%d)", a.CK, a.CN, a.M);
-    return B200OCL_EUNSUPPORTED;
+ConvPlan conv_plan(const ConvArgs& a, int sms) {
+  if (a.CK == 3) {
+    if (a.CN != 20 || a.ks != 3 || a.stride != 1 || a.Hin != a.Hout || a.Win != a.Wout || a.M <= 0 || a.transposed)
+      return none("only the 3->20 3x3 stride-1 stem is supported");
+    return tiled(a, CONV_K_STEM, 20, 1, CONV_THREADS);
   }
+  if (a.CK % 20 != 0 || a.CN % 20 != 0 || a.M <= 0) return none("channel counts must be multiples of 20");
+  ConvPlan pl{};
   // 3x3 stride-1 convolutions on 8/16/32-wide maps: tensor cores fed from a halo patch (conv_tcp.cu);
   // other 3x3 stride-1 shapes with enough 128-pixel tiles: tensor cores with an im2col tile (conv_tc.cu).
+  bool tcp = false, tc = false;
   if (a.force_path == 3) {
-    if (!conv_tcp_eligible(a)) { set_error("launch_conv: launch not covered by the halo-patch tensor-core kernel (3x3 stride 1, no train mode)"); return B200OCL_EUNSUPPORTED; }
-    return launch_conv_tcp(a, stream);
+    if (!conv_tcp_eligible(a)) return none("launch not covered by the halo-patch tensor-core kernel (3x3 stride 1, no train mode)");
+    tcp = true;
+  } else if (a.force_path == 2) {
+    if (!(a.w_tc && a.ks == 3 && a.stride == 1 && !a.transposed)) return none("shape not covered by conv_tc");
+    tc = true;
+  } else if (a.force_path == 0) {
+    tcp = conv_tcp_eligible(a);
+    tc = !tcp && conv_tc_eligible(a, sms);
   }
-  if (a.force_path == 2) {
-    if (!(a.w_tc && a.ks == 3 && a.stride == 1 && !a.transposed)) { set_error("launch_conv: shape not covered by conv_tc"); return B200OCL_EUNSUPPORTED; }
-    return launch_conv_tc(a, stream);
+  if (tcp) {
+    pl.kernel = CONV_K_TCP;
+    pl.nt = a.tp_bn <= 20 ? 32 : 48;   // tp_bn <= 40 (conv_tcp_eligible)
+    pl.grid_x = conv_tcp_grid_x(a, sms);
+    pl.grid_y = a.CN / a.tp_bn;
+    return pl;
   }
-  if (a.force_path == 0) {
-    if (conv_tcp_eligible(a)) return launch_conv_tcp(a, stream);
-    if (conv_tc_eligible(a)) return launch_conv_tc(a, stream);
+  if (tc) {
+    pl.kernel = CONV_K_TC;
+    pl.nt = a.tc_bn <= 20 ? 32 : (a.tc_bn <= 40 ? 48 : 80);
+    pl.grid_x = (a.M + 127) / 128;
+    pl.grid_y = a.CN / a.tc_bn;
+    return pl;
   }
   // Forward convolutions and stride-1 data gradients with enough pixels go to the patch kernel:
   // pick the widest channel tile and 2 pixels per thread that still give >= 3 CTAs per SM.
@@ -737,66 +775,83 @@ int launch_conv(const ConvArgs& a, cudaStream_t stream) {
     // The inner loop issues 5 broadcast LDS.128 (20 weights) per k for 20*PT FMAs and a warp-wide
     // LDS.128 occupies the shared-memory pipe for 4 cycles, so PT = 2 is shared-memory bound by ~2x
     // PT = 4 is close to balance.  Take PT = 4 whenever it still fills the SMs.
-    const long want3 = 5L * sm_count() / 2;
+    const long want3 = 5L * sms / 2;
     const int pbn[3] = {80, 40, 20};
     const int ppt[3] = {4, 2, 1};
     for (int pi = 0; pi < 3; ++pi)
       for (int bi = 0; bi < 3; ++bi) {
         if (a.CN % pbn[bi]) continue;
         const PatchTile t = patch_tile(a, pbn[bi], ppt[pi]);
-        const long need = (ppt[pi] == 4) ? 3L * sm_count() / 2 : want3;
+        const long need = (ppt[pi] == 4) ? 3L * sms / 2 : want3;
         if (t.ctas < need || t.smem > (ppt[pi] == 4 ? 100 : 72) * 1024) continue;
-#define B200OCL_PATCH_CASE(BN_, PT_) \
-        if (pbn[bi] == BN_ && ppt[pi] == PT_) return launch_conv_patch<BN_, PT_>(a, t, stream)
-        B200OCL_PATCH_CASE(80, 4); B200OCL_PATCH_CASE(40, 4); B200OCL_PATCH_CASE(20, 4);
-        B200OCL_PATCH_CASE(80, 2); B200OCL_PATCH_CASE(40, 2); B200OCL_PATCH_CASE(20, 2);
-        B200OCL_PATCH_CASE(80, 1); B200OCL_PATCH_CASE(40, 1); B200OCL_PATCH_CASE(20, 1);
-#undef B200OCL_PATCH_CASE
+        pl.kernel = CONV_K_PATCH;
+        pl.bn = pbn[bi];
+        pl.pt = ppt[pi];
+        pl.grid_y = a.CN / pl.bn;
+        pl.grid_x = (int)(t.ctas / pl.grid_y);
+        pl.th = t.th; pl.tw = t.tw; pl.ti = t.ti;
+        pl.smem = t.smem;
+        return pl;
       }
   }
   // Tiling: the kernels are latency-sensitive (4 warps per CTA, LDS -> FMA chains), so the first goal is
   // >= 4 resident CTAs per SM (16 warps); among tilings that reach it prefer wide channel tiles (the
   // gathered pixel rows are shared by BN/20 warps) and 2-4 pixels per thread (weight loads amortised).
   // When the pixel count cannot provide that many CTAs the K loop is split inside the CTA instead.
-  const long want = 4L * sm_count();
+  const long want = 4L * sms;
   const int bns[3] = {80, 40, 20};
   auto ctas_reg = [&](int bn, int pt) {
     const int bm = (80 / bn) * 32 * pt;
     return (long)((a.M + bm - 1) / bm) * (a.CN / bn);
   };
-  int best_bn = 0, best_pt = 0;
-  for (int bi = 0; bi < 3 && !best_bn; ++bi)
-    if (a.CN % bns[bi] == 0 && ctas_reg(bns[bi], 2) >= want) { best_bn = bns[bi]; best_pt = 2; }
-  if (!best_bn) {
-    if (a.ks * a.ks * (a.CK / 20) >= 4) {
-      const long ctas2 = (long)((a.M + 63) / 64) * (a.CN / 20);
-      if (ctas2 >= want) return launch_conv_ksplit<2, 4>(a, stream);
-      // fewer than two CTAs per SM and a long K: eight warps share the K loop
-      const long ctas1 = (long)((a.M + 31) / 32) * (a.CN / 20);
-      if (ctas1 < 2L * sm_count() && a.ks * a.ks * (a.CK / 20) >= 16) return launch_conv_ksplit<1, 8>(a, stream);
-      return launch_conv_ksplit<1, 4>(a, stream);
-    }
-    best_bn = 20;   // 1x1 convolutions with a short K: most CTAs
-    best_pt = 1;
+  for (int bi = 0; bi < 3; ++bi)
+    if (a.CN % bns[bi] == 0 && ctas_reg(bns[bi], 2) >= want) return tiled(a, CONV_K_TILED, bns[bi], 2, (80 / bns[bi]) * 64);
+  if (a.ks * a.ks * (a.CK / 20) >= 4) {
+    int pt = 1, kwarps = 4;
+    const long ctas2 = (long)((a.M + 63) / 64) * (a.CN / 20);
+    const long ctas1 = (long)((a.M + 31) / 32) * (a.CN / 20);
+    if (ctas2 >= want) pt = 2;
+    // fewer than two CTAs per SM and a long K: eight warps share the K loop
+    else if (ctas1 < 2L * sms && a.ks * a.ks * (a.CK / 20) >= 16) kwarps = 8;
+    pl = tiled(a, CONV_K_KSPLIT, 20, pt, 32 * pt);
+    pl.kwarps = kwarps;
+    return pl;
   }
-#define B200OCL_CONV_CASE(BN_, PT_) \
-  if (best_bn == BN_ && best_pt == PT_) return launch_conv_cfg<BN_, PT_>(a, stream)
-  B200OCL_CONV_CASE(80, 4); B200OCL_CONV_CASE(80, 2); B200OCL_CONV_CASE(80, 1);
-  B200OCL_CONV_CASE(40, 4); B200OCL_CONV_CASE(40, 2); B200OCL_CONV_CASE(40, 1);
-  B200OCL_CONV_CASE(20, 4); B200OCL_CONV_CASE(20, 2); B200OCL_CONV_CASE(20, 1);
-#undef B200OCL_CONV_CASE
-  return B200OCL_EUNSUPPORTED;
+  return tiled(a, CONV_K_TILED, 20, 1, 128);   // 1x1 convolutions with a short K: most CTAs
 }
 
-int launch_stem(const ConvArgs& a, cudaStream_t stream) {
-  if (a.CK != 3 || a.CN != 20 || a.ks != 3 || a.stride != 1 || a.Hin != a.Hout || a.Win != a.Wout) {
-    set_error("launch_stem: only the 3->20 3x3 stride-1 stem is supported");
-    return B200OCL_EUNSUPPORTED;
+int launch_conv(const ConvArgs& a, int sms, cudaStream_t stream) {
+  const ConvPlan pl = conv_plan(a, sms);
+  switch (pl.kernel) {
+    case CONV_K_STEM: return launch_stem(a, pl, stream);
+    case CONV_K_TCP: return launch_conv_tcp(a, pl, stream);
+    case CONV_K_TC: return launch_conv_tc(a, pl, stream);
+    case CONV_K_PATCH:
+#define B200OCL_PATCH_CASE(BN_, PT_) \
+      if (pl.bn == BN_ && pl.pt == PT_) return launch_conv_patch<BN_, PT_>(a, pl, stream)
+      B200OCL_PATCH_CASE(80, 4); B200OCL_PATCH_CASE(40, 4); B200OCL_PATCH_CASE(20, 4);
+      B200OCL_PATCH_CASE(80, 2); B200OCL_PATCH_CASE(40, 2); B200OCL_PATCH_CASE(20, 2);
+      B200OCL_PATCH_CASE(80, 1); B200OCL_PATCH_CASE(40, 1); B200OCL_PATCH_CASE(20, 1);
+#undef B200OCL_PATCH_CASE
+      break;
+    case CONV_K_TILED:
+#define B200OCL_CONV_CASE(BN_, PT_) \
+      if (pl.bn == BN_ && pl.pt == PT_) return launch_conv_cfg<BN_, PT_>(a, pl, stream)
+      B200OCL_CONV_CASE(80, 4); B200OCL_CONV_CASE(80, 2); B200OCL_CONV_CASE(80, 1);
+      B200OCL_CONV_CASE(40, 4); B200OCL_CONV_CASE(40, 2); B200OCL_CONV_CASE(40, 1);
+      B200OCL_CONV_CASE(20, 4); B200OCL_CONV_CASE(20, 2); B200OCL_CONV_CASE(20, 1);
+#undef B200OCL_CONV_CASE
+      break;
+    case CONV_K_KSPLIT:
+      if (pl.pt == 2) return launch_conv_ksplit<2, 4>(a, pl, stream);
+      if (pl.kwarps == 8) return launch_conv_ksplit<1, 8>(a, pl, stream);
+      return launch_conv_ksplit<1, 4>(a, pl, stream);
+    default:
+      set_error("launch_conv: %s (CK=%d CN=%d M=%d)", pl.why, a.CK, a.CN, a.M);
+      return B200OCL_EUNSUPPORTED;
   }
-  B200OCL_PROF(a.mode == CONV_EVAL ? "conv_eval" : "conv_train", 2.0 * a.M * 20.0 * 27.0, stream);
-  stem_kernel<<<(a.M + CONV_THREADS - 1) / CONV_THREADS, CONV_THREADS, 0, stream>>>(a);
-  B200OCL_LAUNCHED();
-  return B200OCL_OK;
+  set_error("launch_conv: no kernel instantiated for the planned tiling");
+  return B200OCL_EUNSUPPORTED;
 }
 
 }  // namespace b200ocl

@@ -76,13 +76,36 @@ __device__ __forceinline__ void bn_finalize(const ConvArgs& a, int c, double S, 
 constexpr int TP_LD_MAX = 13;
 inline bool tcp_strip_fits(int W) { return 128 + 2 * (W + 2) + 2 <= 16 * TP_LD_MAX; }
 
-// Upper bound of gridDim.x over every tiling launch_conv may choose (sizes stat_part).
-int conv_max_grid_m(int M);
-int launch_conv(const ConvArgs& a, cudaStream_t stream);   // CK, CN multiples of 20
-int launch_stem(const ConvArgs& a, cudaStream_t stream);   // CK == 3, CN == 20, ks == 3, NCHW input
-int launch_conv_tc(const ConvArgs& a, cudaStream_t stream);  // conv_tc.cu: wgmma 3xTF32 path
-bool conv_tc_eligible(const ConvArgs& a);
-int launch_conv_tcp(const ConvArgs& a, cudaStream_t stream);  // conv_tcp.cu: wgmma fed from a halo patch
+// The kernel launch_conv runs for one ConvArgs on a GPU with `sms` SMs.  The numbering is the one
+// b200ocl_conv_geom reports (include/b200ocl.h).
+enum ConvKernel {
+  CONV_K_NONE = -1,   // no kernel covers the launch (ConvPlan::why)
+  CONV_K_STEM = 0,    // stem_kernel: 3 -> 20 channels, NCHW input
+  CONV_K_TCP = 1,     // conv_tcp_kernel<nt>: wgmma fed from a halo strip (conv_tcp.cu)
+  CONV_K_TC = 2,      // conv_tc_kernel<nt>: wgmma with im2col tiles (conv_tc.cu)
+  CONV_K_PATCH = 3,   // conv_patch_kernel<bn, pt>
+  CONV_K_TILED = 4,   // conv_kernel<bn, pt>
+  CONV_K_KSPLIT = 5   // conv_ksplit_kernel<pt, kwarps>
+};
+struct ConvPlan {
+  int kernel;            // ConvKernel
+  int nt;                // CONV_K_TCP / CONV_K_TC: padded MMA N
+  int bn, pt;            // CONV_K_PATCH / CONV_K_TILED: channels and pixels per thread; CONV_K_KSPLIT: bn = 20, pt
+  int kwarps;            // CONV_K_KSPLIT: warps sharing the K loop
+  int grid_x, grid_y;    // the grid; a train-mode launch writes grid_x * CN (sum, sum of squares) partials
+  int th, tw, ti;        // CONV_K_PATCH: spatial tile (rows, columns, images)
+  size_t smem;           // CONV_K_PATCH: dynamic shared memory
+  const char* why;       // CONV_K_NONE: the reason
+};
+// Pure host function: every decision launch_conv takes, for a GPU with `sms` SMs.  CK == 3 is the stem.
+ConvPlan conv_plan(const ConvArgs& a, int sms);
+// Bytes of statistics partials (stat_part) a train-mode launch with plan `pl` writes.
+inline size_t conv_stat_bytes(const ConvPlan& pl, int CN) { return (size_t)pl.grid_x * CN * 2 * sizeof(double); }
+int launch_conv(const ConvArgs& a, int sms, cudaStream_t stream);   // runs conv_plan(a, sms)
+bool conv_tc_eligible(const ConvArgs& a, int sms);
+int launch_conv_tc(const ConvArgs& a, const ConvPlan& pl, cudaStream_t stream);   // conv_tc.cu: wgmma 3xTF32 path
 bool conv_tcp_eligible(const ConvArgs& a);
+int conv_tcp_grid_x(const ConvArgs& a, int sms);   // persistent CTAs per channel tile of conv_tcp_kernel
+int launch_conv_tcp(const ConvArgs& a, const ConvPlan& pl, cudaStream_t stream);  // conv_tcp.cu: wgmma fed from a halo patch
 
 }  // namespace b200ocl

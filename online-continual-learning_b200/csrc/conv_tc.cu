@@ -260,10 +260,10 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(ConvArgs a) {
 }
 
 template <int NT>
-int launch_tc(const ConvArgs& a, cudaStream_t stream) {
+int launch_tc(const ConvArgs& a, const ConvPlan& pl, cudaStream_t stream) {
   constexpr size_t smem = (size_t)2 * (2 * A_TILE + 2 * NT * 32) * sizeof(float) + 1024;
   B200OCL_CUDA(raise_smem_limit<conv_tc_kernel<NT>>(smem));
-  dim3 grid((a.M + 127) / 128, a.CN / a.tc_bn);
+  dim3 grid(pl.grid_x, pl.grid_y);
   B200OCL_PROF(a.flip ? "conv_tc_dgrad" : (a.mode == CONV_EVAL ? "conv_tc_eval" : "conv_tc_train"),
                2.0 * a.M * (double)a.CN * a.CK * 9.0, stream);
   conv_tc_kernel<NT><<<grid, TC_THREADS, smem, stream>>>(a);
@@ -273,23 +273,22 @@ int launch_tc(const ConvArgs& a, cudaStream_t stream) {
 
 }  // namespace
 
-bool conv_tc_eligible(const ConvArgs& a) {
+bool conv_tc_eligible(const ConvArgs& a, int sms) {
   if (!a.w_tc || a.ks != 3 || a.stride != 1 || a.transposed || a.CK % 20 != 0) return false;
   if (a.Hin != a.Hout || a.Win != a.Wout) return false;
   // enough 128-pixel tiles to occupy a good part of the machine; small problems stay on the fp32 kernels
   const long ctas = (long)((a.M + 127) / 128) * (a.CN / a.tc_bn);
-  if (ctas < sm_count() / 4) return false;
+  if (ctas < sms / 4) return false;
   // 20 -> 20 channels (layer 1): K = 180 leaves the tensor-core kernel dominated by its per-tile gather, so the
   // fp32 patch kernel takes the layer once there are more than two tiles per SM.
-  if (a.CK == 20 && a.CN == 20 && ctas > 2L * sm_count()) return false;
+  if (a.CK == 20 && a.CN == 20 && ctas > 2L * sms) return false;
   return true;
 }
 
-int launch_conv_tc(const ConvArgs& a, cudaStream_t stream) {
-  const int nt = a.tc_bn <= 20 ? 32 : (a.tc_bn <= 40 ? 48 : 80);
-  if (nt == 32) return launch_tc<32>(a, stream);
-  if (nt == 48) return launch_tc<48>(a, stream);
-  return launch_tc<80>(a, stream);
+int launch_conv_tc(const ConvArgs& a, const ConvPlan& pl, cudaStream_t stream) {
+  if (pl.nt == 32) return launch_tc<32>(a, pl, stream);
+  if (pl.nt == 48) return launch_tc<48>(a, pl, stream);
+  return launch_tc<80>(a, pl, stream);
 }
 
 }  // namespace b200ocl

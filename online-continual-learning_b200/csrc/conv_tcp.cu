@@ -342,7 +342,7 @@ size_t tcp_smem_bytes(const TileGeom& G, int slices, int ps, int bs) {
 }
 
 template <int NT>
-int launch_tcp(ConvArgs a, cudaStream_t stream) {
+int launch_tcp(ConvArgs a, const ConvPlan& pl, cudaStream_t stream) {
   const TileGeom G = tile_geom(a.N, a.Hin, a.Win);
   // Deepest pipeline that fits: 3 patch stages + 6 weight slots, 3 + 4, else 2 + 6.  The fit still sets aside the
   // [128][bn + 1] float scratch of the batch-statistics epilogue this kernel used to have (the smem it allocates does
@@ -356,22 +356,25 @@ int launch_tcp(ConvArgs a, cudaStream_t stream) {
   const size_t smem = tcp_smem_bytes<NT>(G, a.tp_slices, a.tp_ps, a.tp_bs);
   B200OCL_CUDA(raise_smem_limit<conv_tcp_kernel<NT>>(smem));
   a.tp_tiles = G.tiles_m;
-  const int n_tiles = a.CN / a.tp_bn;
-  int gx = sm_count() / n_tiles;
-  if (gx < 1) gx = 1;
-  if (gx > G.tiles_m) gx = G.tiles_m;
-  // even out the tiles per CTA (e.g. 880 tiles on 132 CTAs = 7 rounds -> 126 CTAs of 7, one of 2)
-  const int rounds = (G.tiles_m + gx - 1) / gx;
-  gx = (G.tiles_m + rounds - 1) / rounds;
   // one kernel, two epilogues (eval / data gradient): profiled as one class
   B200OCL_PROF("conv_tcp",
                2.0 * a.M * (double)a.CN * a.CK * 9.0, stream);
-  conv_tcp_kernel<NT><<<dim3(gx, n_tiles), TP_THREADS, smem, stream>>>(a);
+  conv_tcp_kernel<NT><<<dim3(pl.grid_x, pl.grid_y), TP_THREADS, smem, stream>>>(a);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }
 
 }  // namespace
+
+int conv_tcp_grid_x(const ConvArgs& a, int sms) {
+  const TileGeom G = tile_geom(a.N, a.Hin, a.Win);
+  int gx = sms / (a.CN / a.tp_bn);
+  if (gx < 1) gx = 1;
+  if (gx > G.tiles_m) gx = G.tiles_m;
+  // even out the tiles per CTA (e.g. 880 tiles on 132 CTAs = 7 rounds -> 126 CTAs of 7, one of 2)
+  const int rounds = (G.tiles_m + gx - 1) / gx;
+  return (G.tiles_m + rounds - 1) / rounds;
+}
 
 bool conv_tcp_eligible(const ConvArgs& a) {
   // Precision policy: no train-mode forwards.  The truncating tensor-core accumulate leaves a small sign-dependent
@@ -385,10 +388,9 @@ bool conv_tcp_eligible(const ConvArgs& a) {
   return true;
 }
 
-int launch_conv_tcp(const ConvArgs& a, cudaStream_t stream) {
-  // tp_bn <= 40 (conv_tcp_eligible)
-  if (a.tp_bn <= 20) return launch_tcp<32>(a, stream);
-  return launch_tcp<48>(a, stream);
+int launch_conv_tcp(const ConvArgs& a, const ConvPlan& pl, cudaStream_t stream) {
+  if (pl.nt == 32) return launch_tcp<32>(a, pl, stream);
+  return launch_tcp<48>(a, pl, stream);
 }
 
 }  // namespace b200ocl

@@ -889,7 +889,7 @@ extern "C" int b200ocl_net_backward(const b200ocl_net_desc* desc, const b200ocl_
   auto dgrad = [&](int ci, const float* dz, float* dx, int accum) -> int {
     ConvArgs a = conv_layer_args(p.conv[ci], N, dz, st->packed, dx, true);
     a.mode = accum ? CONV_ACCUM : CONV_RAW;
-    return launch_conv(a, stream);
+    return launch_conv(a, sms, stream);
   };
 
   // dz double buffer + fork / join (see bwd_async above)

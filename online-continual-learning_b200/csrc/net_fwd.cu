@@ -936,7 +936,7 @@ int conv_eval(const NetPlan& p, const b200ocl_net_state& st, int ci, int N, cons
   a.rvar = st.bn_stats + b.stat_off + b.c;
   a.residual = residual;
   a.relu = relu;
-  return ci == 0 ? launch_stem(a, stream) : launch_conv(a, stream);
+  return launch_conv(a, sm_count(), stream);
 }
 
 
@@ -981,7 +981,7 @@ int conv_train(const NetPlan& p, const b200ocl_net_state& st, const TrainWs& w, 
     a.run_var = w.run_defer + b.stat_off + b.c;
     a.momentum = 1.0f;
   }
-  const int rc = ci == 0 ? launch_stem(a, stream) : launch_conv(a, stream);
+  const int rc = launch_conv(a, w.sms, stream);   // the geometry train_ws sized stat_part for
   if (rc == 0 && eval_stats) {
     bn_save_running_kernel<<<(b.c + 127) / 128, 128, 0, stream>>>(st.bn_stats + b.stat_off, st.bn_stats + b.stat_off + b.c, a.eps,
                                                                    b.c, a.save_mean, a.save_invstd);
@@ -1135,13 +1135,71 @@ static void selftest_layer(b200ocl::ConvL& c, int cin, int cout, int H, int W, i
   b200ocl::conv_pack_layout(c, pk);
 }
 
-size_t b200ocl_conv_selftest_workspace_bytes(int N, int cin, int cout, int H, int W, int ks, int stride) {
+// The self-test's launch: geometry, weight images addressed from `packed`, mode and forced path as b200ocl_conv_selftest
+// sets them (the BatchNorm pointers are the caller's).
+static b200ocl::ConvArgs selftest_args(const b200ocl::ConvL& c, int N, const float* x, const float* packed, float* out,
+                                       int dgrad, int path, int mode) {
+  using namespace b200ocl;
+  ConvArgs a = conv_layer_args(c, N, x, packed, out, dgrad);
+  a.mode = mode >= 3 ? CONV_EVAL : mode == 2 ? CONV_TRAIN : (mode == 1 ? CONV_ACCUM : CONV_RAW);
+  a.force_path = path;
+  return a;
+}
+
+// Statistics partials region of the self-test workspace: the largest a train-mode launch (forward, paths 0-2) writes.
+static size_t selftest_stat_bytes(const b200ocl::ConvL& c, int N, int sms) {
+  using namespace b200ocl;
+  size_t stat = 0;
+  for (int path = 0; path <= 2; ++path) {
+    const ConvPlan pl = conv_plan(selftest_args(c, N, nullptr, nullptr, nullptr, 0, path, 2), sms);
+    if (pl.kernel != CONV_K_NONE && conv_stat_bytes(pl, c.cout) > stat) stat = conv_stat_bytes(pl, c.cout);
+  }
+  return stat;
+}
+
+static size_t selftest_workspace_bytes(int N, int cin, int cout, int H, int W, int ks, int stride, int sms) {
   b200ocl::ConvL c;
   size_t pk = 0;
   selftest_layer(c, cin, cout, H, W, ks, stride, pk);
-  const size_t M = (size_t)N * H * W;   // upper bound (stride 1)
-  const size_t stat = (size_t)b200ocl::conv_max_grid_m((int)M) * (cin > cout ? cin : cout) * 2 * sizeof(double);
+  const size_t stat = selftest_stat_bytes(c, N, sms);
   return b200ocl::align_up(pk * sizeof(float), 256) + b200ocl::align_up(stat, 256) + 256 /* counters */ + 256;
+}
+
+size_t b200ocl_conv_selftest_workspace_bytes(int N, int cin, int cout, int H, int W, int ks, int stride) {
+  return selftest_workspace_bytes(N, cin, cout, H, W, ks, stride, b200ocl::sm_count());
+}
+
+static void report_geom(const b200ocl::ConvPlan& pl, size_t stat_bytes, size_t stat_region, int sms,
+                        b200ocl_conv_geom* out) {
+  *out = b200ocl_conv_geom{};
+  out->kernel = pl.kernel;
+  out->nt = pl.nt;
+  out->bn = pl.bn;
+  out->pt = pl.pt;
+  out->kwarps = pl.kwarps;
+  out->grid_x = pl.grid_x;
+  out->grid_y = pl.grid_y;
+  out->th = pl.th; out->tw = pl.tw; out->ti = pl.ti;
+  out->stat_bytes = stat_bytes;
+  out->stat_region = stat_region;
+  out->sms = sms;
+}
+
+int b200ocl_conv_selftest_geom(int N, int H, int W, int cin, int cout, int ks, int stride, int dgrad, int path, int mode,
+                               int sms, b200ocl_conv_geom* out) {
+  using namespace b200ocl;
+  B200OCL_CHECK_ARG(out, "null pointer");
+  B200OCL_CHECK_ARG(N > 0 && H > 0 && W > 0 && cin % 20 == 0 && cout % 20 == 0 && cin > 0 && cout > 0, "bad shape");
+  B200OCL_CHECK_ARG((ks == 3 || ks == 1) && (stride == 1 || stride == 2) && mode >= 0 && mode <= 4 && sms >= 0,
+                    "3x3 or 1x1, stride 1 or 2, mode 0..4, sms >= 0");
+  if (sms == 0) sms = sm_count();
+  ConvL c;
+  size_t pk = 0;
+  selftest_layer(c, cin, cout, H, W, ks, stride, pk);
+  const ConvPlan pl = conv_plan(selftest_args(c, N, nullptr, nullptr, nullptr, dgrad, path, mode), sms);
+  const bool train = mode == 2 && pl.kernel != CONV_K_NONE;
+  report_geom(pl, train ? conv_stat_bytes(pl, cout) : 0, selftest_stat_bytes(c, N, sms), sms, out);
+  return B200OCL_OK;
 }
 
 int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N, int H, int W, int cin, int cout,
@@ -1166,14 +1224,12 @@ int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N
   unsigned char* base = static_cast<unsigned char*>(workspace);
   float* packed = reinterpret_cast<float*>(base);
   double* stat_part = reinterpret_cast<double*>(base + align_up(pk * sizeof(float), 256));
-  const size_t M = (size_t)N * H * W;
-  const size_t stat = (size_t)conv_max_grid_m((int)M) * (cin > cout ? cin : cout) * 2 * sizeof(double);
+  const int sms = sm_count();
+  const size_t stat = selftest_stat_bytes(p.conv[0], N, sms);
   unsigned int* counters = reinterpret_cast<unsigned int*>(reinterpret_cast<unsigned char*>(stat_part) + align_up(stat, 256));
   int rc = launch_pack(p, w_oihw, packed, stream);
   if (rc) return rc;
-  ConvArgs a = conv_layer_args(p.conv[0], N, x, packed, out, dgrad);
-  a.mode = mode >= 3 ? CONV_EVAL : mode == 2 ? CONV_TRAIN : (mode == 1 ? CONV_ACCUM : CONV_RAW);
-  a.force_path = path;
+  ConvArgs a = selftest_args(p.conv[0], N, x, packed, out, dgrad, path, mode);
   a.eps = NET_BN_EPS;
   a.momentum = NET_BN_MOMENTUM;
   if (mode == 2) {
@@ -1194,7 +1250,7 @@ int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N
     a.residual = mode == 4 ? x : nullptr;
     a.relu = mode == 4;
   }
-  return launch_conv(a, stream);
+  return launch_conv(a, sms, stream);
 }
 
 int b200ocl_net_sgd_step(const b200ocl_net_desc* desc, const b200ocl_net_state* st, float lr, float weight_decay,
@@ -1493,6 +1549,28 @@ int b200ocl_net_train_ws_layout(const b200ocl_net_desc* desc, int N, int layer, 
   out->wgrad_kernel = wp.kernel == WGRAD_STEM ? 0 : (wp.kernel == WGRAD_TC ? 1 : 2);
   out->wgrad_splits = wp.splits;
   out->sms = sms;
+  return B200OCL_OK;
+}
+
+int b200ocl_net_conv_geom(const b200ocl_net_desc* desc, int N, int layer, int pass, int sms, b200ocl_conv_geom* out) {
+  using namespace b200ocl;
+  B200OCL_CHECK_ARG(desc && out, "null pointer");
+  NetPlan p;
+  const int rc = build_plan(*desc, p);
+  if (rc) {
+    set_error("b200ocl_net_conv_geom: unsupported network description");
+    return rc;
+  }
+  B200OCL_CHECK_ARG(N >= 1, "need N >= 1");
+  B200OCL_CHECK_ARG(layer >= 0 && layer < p.n_conv, "layer out of range");
+  B200OCL_CHECK_ARG(pass == PASS_TRAIN || pass == PASS_EVAL || pass == PASS_DGRAD, "pass must be 0, 1 or 2");
+  B200OCL_CHECK_ARG(pass != PASS_DGRAD || layer > 0, "the stem has no data-gradient launch");
+  B200OCL_CHECK_ARG(sms >= 0, "sms must be 0 (this device) or an SM count");
+  if (sms == 0) sms = sm_count();
+  const ConvL& c = p.conv[layer];
+  const ConvPlan pl = layer_conv_plan(c, N, pass, sms);
+  const size_t stat = pass == PASS_TRAIN ? conv_stat_bytes(pl, c.cout) : 0;
+  report_geom(pl, stat, train_ws(p, N, nullptr, sms).stat_bytes, sms, out);
   return B200OCL_OK;
 }
 

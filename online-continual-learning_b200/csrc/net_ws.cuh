@@ -134,6 +134,17 @@ inline BnBwdGeom bn_bwd_geom(int M, int C, int sms, bool fused_ok) {
 }
 constexpr int NET_COEF_DOUBLES = 512;  // 3 x 160 floats of BN-backward coefficients fit in front of the partials
 
+// The convolution launches of a layer: train-mode forward (batch statistics), eval-mode forward, data gradient.
+enum ConvPass { PASS_TRAIN = 0, PASS_EVAL = 1, PASS_DGRAD = 2 };
+
+// conv_plan of layer c's launch in pass `pass` over N images.  Only the presence of the weight images matters to the
+// plan, so they are addressed from a null packed arena (their offsets are never 0: the packed weights come first).
+inline ConvPlan layer_conv_plan(const ConvL& c, int N, int pass, int sms) {
+  ConvArgs a = conv_layer_args(c, N, nullptr, nullptr, nullptr, pass == PASS_DGRAD);
+  a.mode = pass == PASS_TRAIN ? CONV_TRAIN : (pass == PASS_EVAL ? CONV_EVAL : CONV_RAW);
+  return conv_plan(a, sms);
+}
+
 struct TrainWs {
   unsigned int* counters;  // NET_COUNTERS x u32 (8 per conv), zeroed at the start of forward / backward
   double* stat_part;
@@ -155,6 +166,8 @@ struct TrainWs {
   float* dproj;
   float* wg_part;  // weight-gradient partials, conv i at wg_off[i]
   size_t wg_off[NET_MAX_CONV];
+  size_t stat_bytes;   // size of the stat_part region
+  int sms;             // SM count the launch geometries (and so the partial regions) were planned for
   size_t bytes;
 };
 
@@ -168,16 +181,20 @@ inline TrainWs train_ws(const NetPlan& p, int N, void* base, int sms) {
     return r;
   };
   w.counters = reinterpret_cast<unsigned int*>(take(NET_COUNTERS * sizeof(unsigned int)));
+  // stat_part holds the batch-statistics partials of the train-mode convolution that runs (one per CTA along the
+  // pixels of its grid) and, in the backward, the BN-backward coefficients and partials
   size_t stat_max = 0;
   for (int i = 0; i < p.n_conv; ++i) {
     const size_t M = (size_t)N * p.conv[i].hout * p.conv[i].wout;
-    const size_t s = (size_t)conv_max_grid_m((int)M) * p.conv[i].cout * 2 * sizeof(double);
+    const size_t s = conv_stat_bytes(layer_conv_plan(p.conv[i], N, PASS_TRAIN, sms), p.conv[i].cout);
     if (s > stat_max) stat_max = s;
     const int grid = bn_bwd_geom((int)M, p.conv[i].cout, sms, false).grid;
     const size_t sb = ((size_t)grid * p.conv[i].cout * 2 + NET_COEF_DOUBLES) * sizeof(double);
     if (sb > stat_max) stat_max = sb;
   }
   w.stat_part = reinterpret_cast<double*>(take(stat_max));
+  w.stat_bytes = stat_max;
+  w.sms = sms;
   w.save = reinterpret_cast<float*>(take(2 * p.n_bn_channels * sizeof(float)));
   w.run_scratch = reinterpret_cast<float*>(take(2 * 1024 * sizeof(float)));
   w.run_defer = reinterpret_cast<float*>(take(p.n_stats * sizeof(float)));

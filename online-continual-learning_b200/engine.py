@@ -49,6 +49,30 @@ class NetWsLayout(ctypes.Structure):
                 ('bn_fused', c_int), ('bn_grid', c_int), ('wgrad_kernel', c_int), ('wgrad_splits', c_int), ('sms', c_int)]
 
 
+class ConvGeom(ctypes.Structure):
+    """b200ocl_conv_geom: the convolution kernel one launch runs, its template parameters and grid, and the statistics
+    partials it writes against the workspace region kept for them."""
+    _fields_ = [('kernel', c_int), ('nt', c_int), ('bn', c_int), ('pt', c_int), ('kwarps', c_int), ('grid_x', c_int),
+                ('grid_y', c_int), ('th', c_int), ('tw', c_int), ('ti', c_int), ('stat_bytes', c_size_t),
+                ('stat_region', c_size_t), ('sms', c_int)]
+
+    KERNELS = ('stem', 'tcp', 'tc', 'patch', 'tiled', 'ksplit')
+
+    @property
+    def name(self):
+        return self.KERNELS[self.kernel] if self.kernel >= 0 else 'none'
+
+    @property
+    def template(self):
+        """(kernel name, template parameters) of the instantiation that runs."""
+        return {'stem': ('stem',), 'tcp': ('tcp', self.nt), 'tc': ('tc', self.nt), 'patch': ('patch', self.bn, self.pt),
+                'tiled': ('tiled', self.bn, self.pt), 'ksplit': ('ksplit', self.pt, self.kwarps),
+                'none': ('none',)}[self.name]
+
+
+CONV_PASSES = {'train': 0, 'eval': 1, 'dgrad': 2}
+
+
 def _lib():
     return _native.lib()
 
@@ -58,6 +82,24 @@ def train_ws_layout(desc, n, layer):
     out = NetWsLayout()
     _native.check(_lib().b200ocl_net_train_ws_layout(ctypes.byref(desc), int(n), int(layer), ctypes.byref(out)),
                   'b200ocl_net_train_ws_layout')
+    return out
+
+
+def conv_geom(desc, n, layer, pass_, sms=0):
+    """Host-only test hook (b200ocl_net_conv_geom): the convolution launch of conv layer `layer` over n images in pass
+    'train', 'eval' or 'dgrad' on a GPU with sms SMs (0: the current device)."""
+    out = ConvGeom()
+    _native.check(_lib().b200ocl_net_conv_geom(ctypes.byref(desc), int(n), int(layer), CONV_PASSES[pass_], int(sms),
+                                               ctypes.byref(out)), 'b200ocl_net_conv_geom')
+    return out
+
+
+def conv_selftest_geom(n, h, w, cin, cout, ks, stride, dgrad, path, mode, sms=0):
+    """Host-only test hook (b200ocl_conv_selftest_geom): the launch b200ocl_conv_selftest makes for these arguments."""
+    out = ConvGeom()
+    _native.check(_lib().b200ocl_conv_selftest_geom(int(n), int(h), int(w), int(cin), int(cout), int(ks), int(stride),
+                                                    int(dgrad), int(path), int(mode), int(sms), ctypes.byref(out)),
+                  'b200ocl_conv_selftest_geom')
     return out
 
 

@@ -15,7 +15,7 @@ pytestmark = pytest.mark.gpu
 
 # batch sizes that cross the planner's thresholds (the coverage test below checks what they reach on this card)
 CASES = ([(32, None, n) for n in (1, 2, 10, 20, 37, 110, 160, 210)] + [(32, 'mlp', n) for n in (2, 20, 110, 220)] +
-         [(32, 'linear', 20), (32, 'None', 20)] + [(84, None, n) for n in (2, 20, 22, 110, 160)] + [(84, 'mlp', 110)])
+         [(32, 'linear', 20), (32, 'None', 20)] + [(84, None, n) for n in (2, 6, 10, 20, 22, 110, 160)] + [(84, 'mlp', 110)])
 EVAL_CASES = [(32, None, n) for n in (1, 10, 110)]
 
 # max |got - ref| / max |ref| per parameter tensor, by kind, about 3x the largest value measured over all cases on an
