@@ -97,13 +97,20 @@ int b200ocl_scatter_rows(const void* src, const int64_t* idx, int n_rows, size_t
  * of the normalised features of the samples with that label (base.py:121-141); counts[k] == 0 leaves means[k]
  * untouched (the reference draws a random vector there).  classify: pred[b] = class_ids[arg-min_k ||f_b/||f_b|| -
  * means[k]||^2] (first minimum), *n_correct += #(pred == truth) (truth / pred / n_correct nullable).
- * linear_argmax: pred[b] = arg-max_c (feats[b] . weight[c] + bias[c]) -- the classifier branch (base.py:172-175). */
+ * linear_argmax: pred[b] = arg-max_c (feats[b] . weight[c] + bias[c]) -- the classifier branch (base.py:172-175).
+ * class_means takes d <= B200OCL_NET_MAX_DIM; classify and linear_argmax take any d. */
 int b200ocl_ncm_class_means(const float* feats, const int64_t* labels, int n, int d, const int64_t* class_ids, int K,
                             float* means, int* counts, void* stream);
 int b200ocl_ncm_classify(const float* feats, int B, int d, const float* means, int K, const int64_t* class_ids,
                          const int64_t* truth, int64_t* pred, uint64_t* n_correct, void* stream);
 int b200ocl_linear_argmax(const float* feats, int B, int d, const float* weight, const float* bias, int C,
                           const int64_t* truth, int64_t* pred, uint64_t* n_correct, void* stream);
+
+/* The network's linear layer on its own: y [N,out] = x [N,in] . W[out,in]^T + b (relu != 0: then ReLU), the kernel the
+ * classifier and projection heads run.  Each output sums its lane-strided products in a fixed order (no atomics).
+ * 1 <= in <= B200OCL_NET_MAX_DIM. */
+int b200ocl_linear_fwd(const float* x, const float* W, const float* b, float* y, int N, int in, int out, int relu,
+                       void* stream);
 
 /* A-GEM gradient projection (agents/agem.py:60-80) on flat gradient arenas: out = g - (g.g_ref / g_ref.g_ref) g_ref if
  * g.g_ref < 0, else out = g (out may alias g_ref or g).  dots_out (nullable, [2] f32) receives g.g_ref and g_ref.g_ref.
@@ -154,8 +161,10 @@ int b200ocl_sgd_step(const float* p, const float* g, float* out, size_t n, float
  *   bn_tracked      num_batches_tracked per BatchNorm2d.
  * Images are fp32 NCHW [N,3,H,W] exactly as the reference feeds them (no normalisation,
  * setup_elements.py:29-43); activations are NHWC inside the engine. */
+#define B200OCL_NET_MAX_DIM 4096 /* largest flattened feature size (dim_in) and output size (out_dim) of a network */
+
 typedef struct {
-  int in_h, in_w;      /* 32x32 CIFAR, 84x84 Mini-ImageNet (setup_elements.py:11-17) */
+  int in_h, in_w;      /* 32x32 CIFAR, 84x84 Mini-ImageNet, 128x128 CORe50 (setup_elements.py:11-17) */
   int nf;              /* 20 (Reduced_ResNet18, resnet.py:112-116) */
   int num_classes;     /* classifier width when head == 0 */
   int head;            /* 0 classifier | 1 linear | 2 mlp | 3 none */
@@ -170,7 +179,8 @@ typedef struct {
   int64_t* bn_tracked;
 } b200ocl_net_state;
 
-/* Sizes (in elements) of the arenas and basic shape facts. */
+/* Sizes (in elements) of the arenas and basic shape facts.  A description whose dim_in or out_dim exceeds
+ * B200OCL_NET_MAX_DIM (160 dim_in at 32x32, 640 at 84x84, 2560 at 128x128) is refused with B200OCL_EUNSUPPORTED. */
 typedef struct {
   size_t n_params, n_packed, n_bn_stats;
   int n_bn, n_tensors, dim_in, out_dim;
@@ -182,6 +192,10 @@ int b200ocl_net_tensor(const b200ocl_net_desc* desc, int i, size_t* offset, size
 
 /* packed <- params (call after loading weights). */
 int b200ocl_net_pack(const b200ocl_net_desc* desc, const b200ocl_net_state* st, void* stream);
+
+/* Batch limit of every pass below (features_eval, the forwards, backward): N times the largest activation of one image
+ * must stay within INT_MAX elements, the range the kernels' 32-bit pixel and element indices cover (N <= 104857 at
+ * 32x32, 15217 at 84x84, 6553 at 128x128).  A larger N is refused with B200OCL_EUNSUPPORTED before anything launches. */
 
 /* model.eval(); model.features(x) under no_grad (utils/utils.py:45-90): feat [N,dim_in]. */
 size_t b200ocl_net_eval_workspace_bytes(const b200ocl_net_desc* desc, int N);

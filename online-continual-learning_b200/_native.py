@@ -27,6 +27,7 @@ SIGNATURES = {
     'b200ocl_ncm_class_means': (c_int, [P, P, c_int, c_int, P, c_int, P, P, P]),
     'b200ocl_ncm_classify': (c_int, [P, c_int, c_int, P, c_int, P, P, P, P, P]),
     'b200ocl_linear_argmax': (c_int, [P, c_int, c_int, P, P, c_int, P, P, P, P]),
+    'b200ocl_linear_fwd': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, P]),
     'b200ocl_agem_project_workspace_bytes': (c_size_t, []),
     'b200ocl_agem_project': (c_int, [P, P, P, c_size_t, P, P, c_size_t, P]),
     'b200ocl_grad_cosine_workspace_bytes': (c_size_t, [c_int]),

@@ -5,7 +5,7 @@
 // every test batch builds a [B, d, C] broadcast, takes squared distances and the arg-min (base.py:155-170).
 // Here the buffer features come from the batched eval-feature pass of the engine and three small kernels do the
 // rest:
-//   ncm_class_means   one CTA per class: samples of that class in slot order, thread per feature dimension,
+//   ncm_class_means   one CTA per class: samples of that class in slot order, 4 or 16 feature dimensions per thread,
 //                     x / ||x|| accumulated in fp32, mean, normalised mean; deterministic (no atomics)
 //   ncm_classify      one warp per test sample: normalise, squared distance to every class mean with the
 //                     reference's (f - mu)^2 form, first arg-min, label lookup, correct count (integer atomic)
@@ -17,6 +17,12 @@
 namespace b200ocl {
 namespace {
 
+// DPT dimensions per thread: d <= 256 * DPT.  DPT = 4 serves d <= 1024 (32x32 and 84x84 networks), NCM_WIDE_DPT the
+// wider features up to NET_MAX_DIM (2560 at 128x128); the per-thread sums run in the same order for every DPT.
+constexpr int NCM_MAX_DIM = B200OCL_NET_MAX_DIM;
+constexpr int NCM_WIDE_DPT = NCM_MAX_DIM / 256;
+
+template <int DPT>
 __global__ void __launch_bounds__(256) ncm_class_means_kernel(const float* __restrict__ feats,
                                                               const long long* __restrict__ labels, int n, int d,
                                                               const long long* __restrict__ class_ids, float* __restrict__ means,
@@ -25,8 +31,7 @@ __global__ void __launch_bounds__(256) ncm_class_means_kernel(const float* __res
   __shared__ float s_inv;
   const long long cls = class_ids[blockIdx.x];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  constexpr int DPT = 4;                                  // dimensions per thread: d <= 1024
-  float acc[DPT] = {0.f, 0.f, 0.f, 0.f};
+  float acc[DPT] = {};
   int count = 0;
   for (int i = 0; i < n; ++i) {
     if (labels[i] != cls) continue;                       // uniform across the CTA
@@ -132,12 +137,16 @@ int b200ocl_ncm_class_means(const float* feats, const int64_t* labels, int n, in
                             float* means, int* counts, void* stream_) {
   using namespace b200ocl;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  B200OCL_CHECK_ARG(n >= 0 && d >= 1 && d <= 1024 && K >= 0, "need n >= 0, 1 <= d <= 1024, K >= 0");
+  B200OCL_CHECK_ARG(n >= 0 && d >= 1 && d <= NCM_MAX_DIM && K >= 0, "need n >= 0, 1 <= d <= 4096, K >= 0");
   if (K == 0) return B200OCL_OK;
   B200OCL_CHECK_ARG(class_ids && means && counts && (n == 0 || (feats && labels)), "null pointer");
   B200OCL_PROF("ncm", 4.0 * n * (double)d + 8.0 * n * (double)K, stream);
-  ncm_class_means_kernel<<<K, 256, 0, stream>>>(feats, reinterpret_cast<const long long*>(labels), n, d,
-                                                reinterpret_cast<const long long*>(class_ids), means, counts);
+  const long long* lab = reinterpret_cast<const long long*>(labels);
+  const long long* ids = reinterpret_cast<const long long*>(class_ids);
+  if (d <= 256 * 4)
+    ncm_class_means_kernel<4><<<K, 256, 0, stream>>>(feats, lab, n, d, ids, means, counts);
+  else
+    ncm_class_means_kernel<NCM_WIDE_DPT><<<K, 256, 0, stream>>>(feats, lab, n, d, ids, means, counts);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }

@@ -784,6 +784,7 @@ extern "C" int b200ocl_net_backward(const b200ocl_net_desc* desc, const b200ocl_
     return rc;
   }
   B200OCL_CHECK_ARG(N >= 1 && dout && x, "need N >= 1, x and dout");
+  if ((rc = check_batch("b200ocl_net_backward", p, N))) return rc;
   if ((rc = check_workspace("b200ocl_net_backward", workspace, workspace_bytes,
                             b200ocl_net_train_workspace_bytes(desc, N)))) return rc;
   const int eval_stats = (accumulate >> 1) & 1;   // bit 1 of `accumulate`: backward of b200ocl_net_forward_evalgrad

@@ -632,16 +632,20 @@ __global__ void __launch_bounds__(256) pool_kernel(const float* __restrict__ in,
 
 // ----------------------------------------------------------------------------- linear forward
 // y[n][o] = b[o] + sum_i x[n][i] * W[o][i]  (+ReLU).  One warp per output feature keeps its weight
-// row in registers and walks the batch; in <= 1024.
+// row in registers (CH chunks of 32: in <= 32 * CH) and walks the batch.  Lane l sums its strided elements
+// l, l + 32, ... in order, then the warp reduces: the same summation order for every CH.  CH = 32 serves in <= 1024
+// (32x32 and 84x84 networks), LINEAR_WIDE_CH the wider rows up to NET_MAX_DIM (2560 at 128x128).
+constexpr int LINEAR_WIDE_CH = NET_MAX_DIM / 32;
+template <int CH>
 __global__ void __launch_bounds__(256) linear_fwd_kernel(const float* __restrict__ x, const float* __restrict__ W,
                                                          const float* __restrict__ b, float* __restrict__ y, int N,
                                                          int in, int out, int relu) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int o = blockIdx.x * 8 + warp;
   if (o >= out) return;
-  float w[32];
+  float w[CH];
 #pragma unroll
-  for (int j = 0; j < 32; ++j) {
+  for (int j = 0; j < CH; ++j) {
     const int i = lane + 32 * j;
     w[j] = (i < in) ? W[(size_t)o * in + i] : 0.f;
   }
@@ -650,7 +654,7 @@ __global__ void __launch_bounds__(256) linear_fwd_kernel(const float* __restrict
     const float* xr = x + (size_t)n * in;
     float s = 0.f;
 #pragma unroll
-    for (int j = 0; j < 32; ++j) {
+    for (int j = 0; j < CH; ++j) {
       const int i = lane + 32 * j;
       if (i < in) s = fmaf(xr[i], w[j], s);
     }
@@ -666,7 +670,15 @@ int launch_linear_fwd(const float* x, const float* W, const float* b, float* y, 
                       cudaStream_t stream) {
   int gy = N < 32 ? N : 32;
   B200OCL_PROF("head", 4.0 * ((double)N * in + (double)in * out + (double)N * out), stream);
-  linear_fwd_kernel<<<dim3((out + 7) / 8, gy), 256, 0, stream>>>(x, W, b, y, N, in, out, relu);
+  const dim3 grid((out + 7) / 8, gy);
+  if (in <= 32 * 32) {
+    linear_fwd_kernel<32><<<grid, 256, 0, stream>>>(x, W, b, y, N, in, out, relu);
+  } else if (in <= 32 * LINEAR_WIDE_CH) {
+    linear_fwd_kernel<LINEAR_WIDE_CH><<<grid, 256, 0, stream>>>(x, W, b, y, N, in, out, relu);
+  } else {
+    set_error("linear forward: in=%d exceeds the kernel's limit of %d", in, 32 * LINEAR_WIDE_CH);
+    return B200OCL_EUNSUPPORTED;
+  }
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }
@@ -1062,7 +1074,7 @@ int check_state(const b200ocl_net_desc* desc, const b200ocl_net_state* st, NetPl
     return B200OCL_EINVAL;
   }
   const int rc = build_plan(*desc, p);
-  if (rc) set_error("net: unsupported network description (nf must be 20, head in 0..3, dims <= 1024)");
+  if (rc) set_error("net: unsupported network description (nf must be 20, head in 0..3, dims <= %d)", NET_MAX_DIM);
   return rc;
 }
 
@@ -1088,6 +1100,15 @@ int b200ocl_net_query(const b200ocl_net_desc* desc, b200ocl_net_info* info) {
   info->dim_in = p.dim_in;
   info->out_dim = p.out_dim;
   return B200OCL_OK;
+}
+
+int b200ocl_linear_fwd(const float* x, const float* W, const float* b, float* y, int N, int in, int out, int relu,
+                       void* stream) {
+  using namespace b200ocl;
+  B200OCL_CHECK_ARG(N >= 0 && in >= 1 && out >= 1, "need N >= 0, in >= 1, out >= 1");
+  if (N == 0) return B200OCL_OK;
+  B200OCL_CHECK_ARG(x && W && b && y, "null pointer");
+  return launch_linear_fwd(x, W, b, y, N, in, out, relu, static_cast<cudaStream_t>(stream));
 }
 
 int b200ocl_net_tensor(const b200ocl_net_desc* desc, int i, size_t* offset, size_t* numel, int* has_grad) {
@@ -1481,6 +1502,7 @@ int b200ocl_net_features_eval(const b200ocl_net_desc* desc, const b200ocl_net_st
   B200OCL_CHECK_ARG(N >= 0, "negative batch");
   if (N == 0) return B200OCL_OK;
   B200OCL_CHECK_ARG(x && feat, "null pointer");
+  if ((rc = check_batch("b200ocl_net_features_eval", p, N))) return rc;
   if ((rc = check_workspace("b200ocl_net_features_eval", workspace, workspace_bytes,
                             b200ocl_net_eval_workspace_bytes(desc, N)))) return rc;
   EvalWs w = eval_ws(p, N, workspace);
@@ -1582,6 +1604,7 @@ static int net_forward_impl(const b200ocl_net_desc* desc, const b200ocl_net_stat
   int rc = check_state(desc, st, p);
   if (rc) return rc;
   B200OCL_CHECK_ARG(N >= 1 && x && out, "need N >= 1 and non-null x/out");
+  if ((rc = check_batch("b200ocl_net_forward_train", p, N))) return rc;
   if ((rc = check_workspace("b200ocl_net_forward_train", workspace, workspace_bytes,
                             b200ocl_net_train_workspace_bytes(desc, N)))) return rc;
   TrainWs w = train_ws(p, N, workspace, sm_count());

@@ -18,6 +18,7 @@ namespace b200ocl {
 
 constexpr int NET_MAX_CONV = 20;
 constexpr int NET_MAX_LIN = 3;
+constexpr int NET_MAX_DIM = B200OCL_NET_MAX_DIM;   // largest dim_in / out_dim
 constexpr float NET_BN_EPS = 1e-5f;       // nn.BatchNorm2d defaults (models/resnet.py:20)
 constexpr float NET_BN_MOMENTUM = 0.1f;
 
@@ -76,6 +77,16 @@ struct NetPlan {
 };
 
 inline int conv_out(int x, int ks, int stride, int pad) { return (x + 2 * pad - ks) / stride + 1; }
+
+// The kernels index pixels and elements of one activation tensor with 32-bit ints: N images fit when N times the
+// largest activation of one image stays within INT_MAX elements.
+inline bool net_batch_fits(const NetPlan& p, int N) { return (size_t)N * p.max_act_per_image <= 2147483647u; }
+inline int net_max_batch(const NetPlan& p) { return (int)(2147483647u / p.max_act_per_image); }
+inline int check_batch(const char* what, const NetPlan& p, int N) {
+  if (net_batch_fits(p, N)) return B200OCL_OK;
+  set_error("%s: N=%d images exceed the batch limit of %d for %dx%d inputs", what, N, net_max_batch(p), p.in_h, p.in_w);
+  return B200OCL_EUNSUPPORTED;
+}
 
 // Packed-arena layout of one convolution (kernel-side weight copies); c.cin/cout/ks/stride/hin/win set.
 inline void conv_pack_layout(ConvL& c, size_t& pk) {
@@ -206,7 +217,9 @@ inline int build_plan(const b200ocl_net_desc& d, NetPlan& p) {
       p.out_dim = p.dim_in;
     }
   }
-  if (p.dim_in > 1024 || p.out_dim > 1024) return B200OCL_EUNSUPPORTED;
+  // the linear forward keeps a row of at most NET_MAX_DIM weights in registers, the NCM class means a feature of as many
+  // dimensions (dim_in 2560 at 128x128)
+  if (p.dim_in > NET_MAX_DIM || p.out_dim > NET_MAX_DIM) return B200OCL_EUNSUPPORTED;
   p.n_params = off;
   p.n_packed = pk;
   p.n_stats = st;

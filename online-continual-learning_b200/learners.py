@@ -567,6 +567,7 @@ class ExperienceReplay(ContinualLearner):
 
 class SupContrastReplay(ContinualLearner):
     def __init__(self, model, opt, params):
+        nets.check_supcon(input_size_match[params.data][1], getattr(params, 'head', 'mlp'))   # before adopt() allocates
         super().__init__(model, opt, params)
         self.buffer = Buffer(model, params)
         self.mem_size = params.mem_size

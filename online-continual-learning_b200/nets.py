@@ -10,7 +10,7 @@ import weakref
 import torch
 import torch.nn as nn
 
-from .engine import Engine
+from .engine import Engine, describe
 from .memory import input_size_match, n_classes
 
 _ENGINES = weakref.WeakKeyDictionary()
@@ -128,10 +128,29 @@ def Reduced_ResNet18(nclasses, nf=20, bias=True, in_hw=32):
 
 def SupConResNet(dim_in=160, head='mlp', feat_dim=128, in_hw=None):
     """models/resnet.py:140-157.  dim_in selects the dataset like the reference does
-    (160: 32x32 inputs, 640: 84x84 inputs; setup_elements.py:49-51)."""
+    (160: 32x32 inputs, 640: 84x84 inputs; setup_elements.py:49-51).  The reference builds no SupConResNet for
+    128x128 inputs: SCR on CORe50 is refused by check_supcon."""
     if in_hw is None:
         in_hw = {160: 32, 640: 84}[dim_in]
     return EngineModel(in_hw, 100, head=head, feat_dim=feat_dim)
+
+
+SUPCON_MAX_DIM = 1024     # b200ocl_supcon's feature limit
+
+
+def check_supcon(in_hw, head, head_in=None):
+    """SCR's network on in_hw x in_hw inputs, refused before anything is allocated where it cannot run:
+      * head 'mlp' / 'linear' built for head_in features while the encoder gives reduced_resnet_dim_in(in_hw) (the
+        reference's SupConResNet(dim_in=160) on 128x128 inputs): ValueError -- the reference fails at its first forward;
+      * head 'None' on features wider than b200ocl_supcon takes (2560 at 128x128): NotImplementedError."""
+    dim_in = reduced_resnet_dim_in(in_hw)
+    if head in ('mlp', 'linear'):
+        if head_in is not None and head_in != dim_in:
+            raise ValueError('SupConResNet with a %r head over %d features: the encoder gives %d features for %dx%d '
+                             'inputs (the reference fails at its first forward)' % (head, head_in, dim_in, in_hw, in_hw))
+    elif dim_in > SUPCON_MAX_DIM:
+        raise NotImplementedError('SCR without a head takes the SupCon loss over the %d encoder features of %dx%d inputs; '
+                                  'the engine\'s SupCon kernel takes at most %d' % (dim_in, in_hw, in_hw, SUPCON_MAX_DIM))
 
 
 def setup_architecture(params):
@@ -139,8 +158,10 @@ def setup_architecture(params):
     nclass = n_classes[params.data]
     in_hw = input_size_match[params.data][1]
     if params.agent in ['SCR', 'SCP']:
-        return SupConResNet(640 if params.data == 'mini_imagenet' else 160, head=params.head)
-    if params.data in ('cifar100', 'cifar10', 'mini_imagenet'):
+        dim_in = 640 if params.data == 'mini_imagenet' else 160
+        check_supcon(in_hw, params.head, dim_in)
+        return SupConResNet(dim_in, head=params.head)
+    if params.data in ('cifar100', 'cifar10', 'mini_imagenet', 'core50'):
         return Reduced_ResNet18(nclass, in_hw=in_hw)
     raise NotImplementedError('dataset %s is outside the replay-path scope (SURVEY section 8)' % params.data)
 
@@ -159,8 +180,8 @@ def reference_init(data, num_classes, in_hw):
     agents/gdumb.py:61 calls it), in parameters() order, drawn in module construction order from torch's default CPU
     generator by the torch.nn.init calls the layers' reset_parameters() make: kaiming_uniform_(a=sqrt(5)) for every
     convolution and linear weight, uniform_(+-1/sqrt(fan_in)) for the linear bias; BatchNorm weights 1 and biases 0
-    take no draws.  For mini_imagenet the 160-input classifier Reduced_ResNet18 builds is drawn and then replaced by a
-    640-input one (setup_elements.py:63-66), so both are drawn and the first is discarded."""
+    take no draws.  For mini_imagenet and core50 the 160-input classifier Reduced_ResNet18 builds is drawn and then
+    replaced by a 640- / 2560-input one (setup_elements.py:59-66), so both are drawn and the first is discarded."""
     dim_in = reduced_resnet_dim_in(in_hw)
 
     def linear(fan_in):
@@ -184,7 +205,7 @@ def reference_init(data, num_classes, in_hw):
             nn.init.zeros_(t)
         out.append(t)
     w, b = linear(20 * 8)
-    if data == 'mini_imagenet':
+    if data in ('mini_imagenet', 'core50'):
         w, b = linear(dim_in)
     elif dim_in != 20 * 8:
         raise NotImplementedError('reference_init: %dx%d inputs of %s are outside the replay path' % (in_hw, in_hw, data))
@@ -216,6 +237,16 @@ def adopt(module, in_hw):
         feat_dim = module.head.out_features
     elif head == 'mlp':
         feat_dim = module.head[2].out_features
+    # the classifier (or SupCon head) must take the features the plan's encoder gives at in_hw
+    head_in = enc.linear.in_features if head is None else None
+    if head == 'linear':
+        head_in = module.head.in_features
+    elif head == 'mlp':
+        head_in = module.head[0].in_features
+    _, info, _ = describe(in_hw, num_classes, head=head, feat_dim=feat_dim)
+    if head_in is not None and head_in != info.dim_in:
+        raise ValueError('adopt(): the module\'s %s takes %d features, the encoder gives %d for %dx%d inputs'
+                         % ('classifier' if head is None else 'head', head_in, info.dim_in, in_hw, in_hw))
     params = list(module.parameters())
     dev = params[0].device
     if dev.type != 'cuda':

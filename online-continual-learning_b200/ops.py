@@ -194,6 +194,18 @@ def linear_argmax(feats, weight, bias, truth=None, n_correct=None):
     return pred
 
 
+def linear_fwd(x, weight, bias, relu=False):
+    """x @ weight.T + bias (then ReLU when relu) with the network heads' kernel: y [N, out] for x [N, in], in <= 4096."""
+    _need_cuda(x, weight, bias)
+    x, weight, bias = _f32(x), _f32(weight), _f32(bias)
+    N, d = x.shape
+    y = torch.empty((N, weight.shape[0]), dtype=torch.float32, device=x.device)
+    rc = _native.lib().b200ocl_linear_fwd(_ptr(x), _ptr(weight), _ptr(bias), _ptr(y), N, d, weight.shape[0],
+                                          1 if relu else 0, _stream())
+    _native.check(rc, 'b200ocl_linear_fwd')
+    return y
+
+
 def agem_project(g, g_ref, out=None, want_dots=False):
     """A-GEM projection of the flat gradient g against g_ref (agents/agem.py:60-80); out may alias either input."""
     _need_cuda(g, g_ref, out)
