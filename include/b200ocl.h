@@ -79,10 +79,35 @@ int b200ocl_rank_desc(const float* a, float sa, const float* b, float sb, int n,
 /* ---------------------------------------------------------------- SupCon loss
  * Replaces SupConLoss.forward (+ its autograd backward), all-views-anchor mode
  * (utils/loss.py:19-96): features [B,V,d] f32, labels [B] i64 -> loss[1] and, when
- * dfeats != NULL, dL/dfeatures [B,V,d].  d <= 1024. */
+ * dfeats != NULL, dL/dfeatures [B,V,d].  d <= 1024.
+ * An anchor without positives (V = 1, a class with one sample) makes the loss NaN, as in the reference (loss.py:90);
+ * the gradient stays finite: that anchor's positive term is taken as 0, so it contributes the gradient of lse_i / A
+ * (its log-sum-exp over the other anchors) and nothing else.  Autograd on the reference gives NaN everywhere. */
 size_t b200ocl_supcon_workspace_bytes(int B, int V, int d);
 int b200ocl_supcon(const float* feats, const int64_t* labels, int B, int V, int d, float temperature,
                    float* loss, float* dfeats, void* workspace, size_t workspace_bytes, void* stream);
+
+/* The launch b200ocl_supcon makes for B x V anchors of width d on a GPU with sms SMs (0: the current device), with
+ * aligned != 0 when feats (and dfeats, if given) are 16-byte aligned.  family: the fused kernel with the whole
+ * contrast set resident in shared memory (rm x rn = 1 x 4), with a two-slot ring of 16-anchor units (1 x 2) or of
+ * 64-anchor units (4 x 4), all with nc = ceil(d / 64) float4 columns per thread; or the stats kernel + grad kernel
+ * with dch = 4/8/16/32 columns per lane.  grid: CTAs of the launch (each of the fallback's two); n_units: anchor blocks
+ * (the entries of the workspace's loss partials it writes); units_per_cta: the most units one CTA takes; smem_bytes:
+ * dynamic shared memory of the largest launch, smem_limit: the limit the launcher raises the kernel to; tx_bytes: the
+ * largest single mbarrier transaction a fused launch expects (0 for the fallback).  Host only, launches nothing; exists
+ * so that tests can check which kernels a shape reaches and that every plan fits on any SM count. */
+#define B200OCL_SUPCON_RESIDENT 0
+#define B200OCL_SUPCON_RING16 1
+#define B200OCL_SUPCON_RING64 2
+#define B200OCL_SUPCON_FALLBACK 3
+typedef struct {
+  int family;
+  int rm, rn, nc, dch;
+  int grid, n_units, units_per_cta;
+  size_t smem_bytes, smem_limit, tx_bytes;
+  int sms;
+} b200ocl_supcon_launch;
+int b200ocl_supcon_plan(int B, int V, int d, int aligned, int sms, b200ocl_supcon_launch* out);
 
 /* ---------------------------------------------------------------- buffer rows
  * dst[i,:] = src[idx[i],:]  /  dst[idx[i],:] = src[i,:]   rows of row_bytes bytes

@@ -21,6 +21,7 @@ SIGNATURES = {
     'b200ocl_rank_desc': (c_int, [P, c_float, P, c_float, c_int, P, c_int, P, P]),
     'b200ocl_supcon_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'b200ocl_supcon': (c_int, [P, P, c_int, c_int, c_int, c_float, P, P, P, c_size_t, P]),
+    'b200ocl_supcon_plan': (c_int, [c_int, c_int, c_int, c_int, c_int, P]),
     'b200ocl_gather_rows': (c_int, [P, P, c_int, c_size_t, P, P]),
     'b200ocl_scatter_rows': (c_int, [P, P, c_int, c_size_t, P, P]),
     'b200ocl_stream_prepare': (c_int, [P, P, c_int, c_int, c_int, P, P]),

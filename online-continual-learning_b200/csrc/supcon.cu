@@ -22,7 +22,17 @@
 //                 dc_i = (1/T) sum_j (G_ij + G_ji) c_j,  G_ij = (exp(l_ij - lse_i) - 1[j in P(i)]/|P(i)|)/A,
 //                 using l_ji = l_ij (anchor set == contrast set in 'all' mode, loss.py:60-62).
 // Anchors are in view-major order a = v*B + b (loss.py:56); features/grad are [B,V,d].
+//
+// supcon_plan() below is the one place that picks the launch: the resident fused kernel <1,4,NC,true>, the ring
+// kernels <1,2,NC,false> (16-anchor units) and <4,4,NC,false> (64-anchor units), or the two-kernel fallback with
+// grad kernel <DCH>.  b200ocl_supcon_plan reports it without launching anything.
+//
+// An anchor without positives (V = 1 and a class with one sample): its loss term is 0/0, so the loss is NaN, as in
+// the reference (loss.py:90).  The gradient stays finite on every launch: G_ij's positive term 1[j in P(i)] / |P(i)|
+// is taken as 0 for every j when P(i) is empty, so that anchor contributes its softmax term (the gradient of
+// lse_i / A) and nothing else.  Autograd on the reference would make every entry NaN.
 #include <float.h>
+#include <limits.h>
 #include <math.h>
 
 #include "common.cuh"
@@ -179,9 +189,10 @@ __global__ void __launch_bounds__(SC_THREADS) supcon_grad_kernel(SupconParams p)
     float w = 0.f;
     if (valid && j < p.A && j != i) {
       const float l = __fdiv_rn(tile_dot(sa + warp * p.d, sct + lane * p.pitch, p.d), p.T);
-      const float pos = (p.labels[j % p.B] == yi) ? 1.f : 0.f;
-      const float g_ij = expf(l - lse_i) - pos / np_i;
-      const float g_ji = expf(l - p.lse[j]) - pos / p.npos[j];
+      // the positive terms only where j in P(i) (then i in P(j)): an anchor without positives has none (see the top)
+      const bool pos = p.labels[j % p.B] == yi;
+      const float g_ij = expf(l - lse_i) - (pos ? 1.f / np_i : 0.f);
+      const float g_ji = expf(l - p.lse[j]) - (pos ? 1.f / p.npos[j] : 0.f);
       w = (g_ij + g_ji) * invA / p.T;
     }
     wbuf[warp * 32 + lane] = w;
@@ -515,34 +526,79 @@ size_t fused_smem_bytes(int A, int d) {
   return 128 + (size_t)(TM + b_rows) * P * 4 + (size_t)TN * WP * 4 + (size_t)b_rows * 16 + (size_t)TM * 4;
 }
 
+constexpr size_t SCF_SMEM_LIMIT = 227 * 1024;     // the fused kernels' dynamic shared-memory limit
+constexpr size_t SCF_RES_MAX_SMEM = 200 * 1024;   // the resident family is taken up to this much
+constexpr size_t SC_SMEM_LIMIT = 200 * 1024;      // the two-kernel fallback's limit (d = 1024 needs 165 KB)
+
+// The one place that decides which SupCon kernels a call launches (b200ocl_supcon launches what this returns;
+// b200ocl_supcon_plan reports it).  Host only.
+b200ocl_supcon_launch supcon_plan(int B, int V, int d, bool aligned, int sms) {
+  b200ocl_supcon_launch L{};
+  const int A = B * V;
+  L.sms = sms;
+  if (d % 4 == 0 && d <= SCF_MAX_D && aligned) {
+    L.nc = (d + 63) / 64;
+    if (A <= 16 * sms && fused_smem_bytes<1, 4, 4, true>(A, d) <= SCF_RES_MAX_SMEM) {
+      L.family = B200OCL_SUPCON_RESIDENT;
+      L.rm = 1; L.rn = 4;
+    } else if (A <= 16 * sms) {
+      L.family = B200OCL_SUPCON_RING16;
+      L.rm = 1; L.rn = 2;
+    } else {
+      // large anchor sets: 64-anchor blocks, one CTA per SM.  Shared memory, not occupancy, bounds the inner loop, so
+      // the 4 x 4 register tile with the least shared-memory traffic per FMA is used.
+      L.family = B200OCL_SUPCON_RING64;
+      L.rm = 4; L.rn = 4;
+    }
+    const int TM = 16 * L.rm, TN = 16 * L.rn;
+    const bool res = L.family == B200OCL_SUPCON_RESIDENT;
+    // fused_smem_bytes does not depend on NC
+    L.smem_bytes = res ? fused_smem_bytes<1, 4, 4, true>(A, d)
+                       : (L.rm == 1 ? fused_smem_bytes<1, 2, 4, false>(A, d) : fused_smem_bytes<4, 4, 4, false>(A, d));
+    L.smem_limit = SCF_SMEM_LIMIT;
+    L.n_units = (A + TM - 1) / TM;
+    L.grid = L.n_units < sms ? L.n_units : sms;          // the grid-wide wait needs every CTA resident: one per SM
+    L.units_per_cta = (L.n_units + L.grid - 1) / L.grid;
+    const int staged = res ? A : (TM > TN ? TM : TN);    // rows behind one mbarrier expect_tx
+    L.tx_bytes = (size_t)staged * (size_t)d * 4;
+  } else {
+    L.family = B200OCL_SUPCON_FALLBACK;
+    L.dch = d <= 128 ? 4 : d <= 256 ? 8 : d <= 512 ? 16 : 32;
+    L.n_units = (A + SC_WARPS - 1) / SC_WARPS;
+    L.grid = L.n_units;
+    L.units_per_cta = 1;
+    const int pitch = (d % 2 == 0) ? d + 1 : d;
+    L.smem_bytes = (size_t)(SC_WARPS * d + 32 * pitch) * sizeof(float) + SC_WARPS * 32 * sizeof(float);   // grad kernel
+    L.smem_limit = SC_SMEM_LIMIT;
+  }
+  return L;
+}
+
 template <int RM, int RN, int NC, bool RES>
-int launch_fused(SupconParams p, cudaStream_t stream) {
-  constexpr int TM = 16 * RM;
-  const size_t smem = fused_smem_bytes<RM, RN, NC, RES>(p.A, p.d);
-  B200OCL_CUDA((raise_smem_limit<supcon_fused_kernel<RM, RN, NC, RES>>(227 * 1024)));
-  p.n_units = (p.A + TM - 1) / TM;
+int launch_fused(SupconParams p, const b200ocl_supcon_launch& L, cudaStream_t stream) {
+  B200OCL_CUDA((raise_smem_limit<supcon_fused_kernel<RM, RN, NC, RES>>(SCF_SMEM_LIMIT)));
+  p.n_units = L.n_units;
   // the grid-wide wait needs every CTA resident: one CTA per SM
   int per_sm = 0;
-  B200OCL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, supcon_fused_kernel<RM, RN, NC, RES>, SC_THREADS, smem));
+  B200OCL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, supcon_fused_kernel<RM, RN, NC, RES>, SC_THREADS,
+                                                             L.smem_bytes));
   if (per_sm < 1) {
-    set_error("b200ocl_supcon: fused kernel does not fit on an SM (%zu bytes of shared memory)", smem);
+    set_error("b200ocl_supcon: fused kernel does not fit on an SM (%zu bytes of shared memory)", L.smem_bytes);
     return B200OCL_EUNSUPPORTED;
   }
-  const int coresident = sm_count();
-  const int grid = p.n_units < coresident ? p.n_units : coresident;
   B200OCL_PROF("supcon", 2.0 * 4.0 * p.A * p.d + 8.0 * p.B, stream);
-  supcon_fused_kernel<RM, RN, NC, RES><<<grid, SC_THREADS, smem, stream>>>(p);
+  supcon_fused_kernel<RM, RN, NC, RES><<<L.grid, SC_THREADS, L.smem_bytes, stream>>>(p);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }
 
 template <int RM, int RN, bool RES>
-int launch_fused_nc(const SupconParams& p, cudaStream_t stream) {
-  switch ((p.d + 63) / 64) {
-    case 1: return launch_fused<RM, RN, 1, RES>(p, stream);
-    case 2: return launch_fused<RM, RN, 2, RES>(p, stream);
-    case 3: return launch_fused<RM, RN, 3, RES>(p, stream);
-    default: return launch_fused<RM, RN, 4, RES>(p, stream);
+int launch_fused_nc(const SupconParams& p, const b200ocl_supcon_launch& L, cudaStream_t stream) {
+  switch (L.nc) {
+    case 1: return launch_fused<RM, RN, 1, RES>(p, L, stream);
+    case 2: return launch_fused<RM, RN, 2, RES>(p, L, stream);
+    case 3: return launch_fused<RM, RN, 3, RES>(p, L, stream);
+    default: return launch_fused<RM, RN, 4, RES>(p, L, stream);
   }
 }
 
@@ -584,35 +640,49 @@ int b200ocl_supcon(const float* feats, const int64_t* labels, int B, int V, int 
   p.part = ws + 2 * (size_t)p.A;
   p.loss = loss;
   p.dfeats = dfeats;
-  const int grid = (p.A + SC_WARPS - 1) / SC_WARPS;
-  const size_t smem_stats = (size_t)(SC_WARPS * d + 32 * p.pitch) * sizeof(float);
-  const size_t smem_grad = smem_stats + SC_WARPS * 32 * sizeof(float);
+  const bool aligned = (reinterpret_cast<uintptr_t>(feats) & 15) == 0 &&
+                       (!dfeats || (reinterpret_cast<uintptr_t>(dfeats) & 15) == 0);
+  const b200ocl_supcon_launch L = supcon_plan(B, V, d, aligned, sm_count());
 
   B200OCL_CUDA(cudaMemsetAsync(p.counter, 0, sizeof(unsigned int), stream));
-  if (d % 4 == 0 && d <= SCF_MAX_D && (reinterpret_cast<uintptr_t>(feats) & 15) == 0 &&
-      (!dfeats || (reinterpret_cast<uintptr_t>(dfeats) & 15) == 0)) {
-    const int sms = sm_count();
-    if (p.A <= 16 * sms && fused_smem_bytes<1, 4, 4, true>(p.A, d) <= 200 * 1024) return launch_fused_nc<1, 4, true>(p, stream);
-    if (p.A <= 16 * sms) return launch_fused_nc<1, 2, false>(p, stream);
-    // large anchor sets: 64-anchor blocks, one CTA per SM.  Shared memory, not occupancy, bounds the inner loop, so
-    // the 4 x 4 register tile with the least shared-memory traffic per FMA is used.
-    return launch_fused_nc<4, 4, false>(p, stream);
+  switch (L.family) {
+    case B200OCL_SUPCON_RESIDENT: return launch_fused_nc<1, 4, true>(p, L, stream);
+    case B200OCL_SUPCON_RING16: return launch_fused_nc<1, 2, false>(p, L, stream);
+    case B200OCL_SUPCON_RING64: return launch_fused_nc<4, 4, false>(p, L, stream);
+    default: break;
   }
-  // d = 1024 needs 165 KB; static smem takes a little of the 227 KB
+  // static smem takes a little of the 227 KB
+  const size_t smem_stats = L.smem_bytes - SC_WARPS * 32 * sizeof(float);
   B200OCL_CUDA((raise_smem_limit<supcon_stats_kernel, supcon_grad_kernel<4>, supcon_grad_kernel<8>, supcon_grad_kernel<16>,
-                                 supcon_grad_kernel<32>>(200 * 1024)));
+                                 supcon_grad_kernel<32>>(L.smem_limit)));
   B200OCL_PROF("supcon", 4.0 * p.A * d + 8.0 * B + 8.0 * p.A, stream);
-  supcon_stats_kernel<<<grid, SC_THREADS, smem_stats, stream>>>(p);
+  supcon_stats_kernel<<<L.grid, SC_THREADS, smem_stats, stream>>>(p);
   B200OCL_LAUNCHED();
   if (!dfeats) return B200OCL_OK;
-#define B200OCL_SC_GRAD(DCH) supcon_grad_kernel<DCH><<<grid, SC_THREADS, smem_grad, stream>>>(p)
+#define B200OCL_SC_GRAD(DCH) supcon_grad_kernel<DCH><<<L.grid, SC_THREADS, L.smem_bytes, stream>>>(p)
   B200OCL_PROF("supcon", 8.0 * p.A * d, stream);
-  if (d <= 128) B200OCL_SC_GRAD(4);
-  else if (d <= 256) B200OCL_SC_GRAD(8);
-  else if (d <= 512) B200OCL_SC_GRAD(16);
-  else B200OCL_SC_GRAD(32);
+  switch (L.dch) {
+    case 4: B200OCL_SC_GRAD(4); break;
+    case 8: B200OCL_SC_GRAD(8); break;
+    case 16: B200OCL_SC_GRAD(16); break;
+    default: B200OCL_SC_GRAD(32); break;
+  }
 #undef B200OCL_SC_GRAD
   B200OCL_LAUNCHED();
+  return B200OCL_OK;
+}
+
+int b200ocl_supcon_plan(int B, int V, int d, int aligned, int sms, b200ocl_supcon_launch* out) {
+  using namespace b200ocl;
+  B200OCL_CHECK_ARG(out, "null pointer");
+  B200OCL_CHECK_ARG(B >= 1 && V >= 1 && d >= 1, "need B,V,d >= 1");
+  B200OCL_CHECK_ARG((long long)B * V <= INT_MAX / 2, "B*V out of range");
+  B200OCL_CHECK_ARG(sms >= 0, "sms must be 0 (this device) or an SM count");
+  if (d > 1024) {
+    set_error("b200ocl_supcon_plan: d=%d exceeds the kernel's limit of 1024", d);
+    return B200OCL_EUNSUPPORTED;
+  }
+  *out = supcon_plan(B, V, d, aligned != 0, sms ? sms : sm_count());
   return B200OCL_OK;
 }
 

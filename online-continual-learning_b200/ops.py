@@ -119,6 +119,34 @@ def supcon(features, labels, temperature, need_grad=True):
     return loss, grad
 
 
+class SupconLaunch(ctypes.Structure):
+    """b200ocl_supcon_launch: the kernels one b200ocl_supcon call runs."""
+    _fields_ = [('family', ctypes.c_int), ('rm', ctypes.c_int), ('rn', ctypes.c_int), ('nc', ctypes.c_int),
+                ('dch', ctypes.c_int), ('grid', ctypes.c_int), ('n_units', ctypes.c_int),
+                ('units_per_cta', ctypes.c_int), ('smem_bytes', ctypes.c_size_t), ('smem_limit', ctypes.c_size_t),
+                ('tx_bytes', ctypes.c_size_t), ('sms', ctypes.c_int)]
+
+    FAMILIES = ('resident', 'ring16', 'ring64', 'fallback')
+
+    @property
+    def name(self):
+        return self.FAMILIES[self.family]
+
+    @property
+    def kernel(self):
+        """(family, NC) of a fused launch, ('fallback', DCH) of the two-kernel one."""
+        return (self.name, self.dch if self.name == 'fallback' else self.nc)
+
+
+def supcon_plan(B, V, d, aligned=True, sms=0):
+    """Host-only test hook (b200ocl_supcon_plan): the launch supcon() makes for features [B,V,d] on a GPU with sms
+    SMs (0: the current device); aligned: the feature and gradient pointers are 16-byte aligned."""
+    out = SupconLaunch()
+    _native.check(_native.lib().b200ocl_supcon_plan(int(B), int(V), int(d), 1 if aligned else 0, int(sms),
+                                                    ctypes.byref(out)), 'b200ocl_supcon_plan')
+    return out
+
+
 def gather_rows(src, idx, out=None):
     """out[i] = src[idx[i]] over the first dimension (buffer_img[indices])."""
     _need_cuda(src, idx, out)
@@ -167,14 +195,27 @@ def ncm_class_means(feats, labels, class_ids):
     return means, counts
 
 
+def _check_truth(truth, B):
+    if truth is None:
+        return None
+    truth = _i64(truth).reshape(-1)
+    if truth.numel() != B:
+        raise ValueError('truth must hold one label per feature row')
+    return truth
+
+
 def ncm_classify(feats, means, class_ids, truth=None, n_correct=None):
     """Nearest normalised class mean (agents/base.py:155-170).  Returns pred [B]; adds the number of hits to
     n_correct (uint64 tensor [1], as int64 storage) when truth is given."""
     _need_cuda(feats, means, class_ids, truth, n_correct)
     feats, means, class_ids = _f32(feats), _f32(means), _i64(class_ids).reshape(-1)
     B, d = feats.shape
+    if means.dim() != 2 or means.shape[1] != d:
+        raise ValueError('means [K,d] must have the features\' width d=%d' % d)
+    if class_ids.numel() != means.shape[0]:
+        raise ValueError('class_ids must hold one label per class mean')
+    truth = _check_truth(truth, B)
     pred = torch.empty(B, dtype=torch.int64, device=feats.device)
-    truth = None if truth is None else _i64(truth).reshape(-1)
     rc = _native.lib().b200ocl_ncm_classify(_ptr(feats), B, d, _ptr(means), means.shape[0], _ptr(class_ids), _ptr(truth),
                                             _ptr(pred), _ptr(n_correct), _stream())
     _native.check(rc, 'b200ocl_ncm_classify')
@@ -184,10 +225,14 @@ def ncm_classify(feats, means, class_ids, truth=None, n_correct=None):
 def linear_argmax(feats, weight, bias, truth=None, n_correct=None):
     """arg-max of feats @ weight.T + bias (agents/base.py:172-175)."""
     _need_cuda(feats, weight, bias, truth, n_correct)
-    feats, weight, bias = _f32(feats), _f32(weight), _f32(bias)
+    feats, weight, bias = _f32(feats), _f32(weight), _f32(bias).reshape(-1)
     B, d = feats.shape
+    if weight.dim() != 2 or weight.shape[1] != d:
+        raise ValueError('weight [C,d] must have the features\' width d=%d' % d)
+    if bias.numel() != weight.shape[0]:
+        raise ValueError('bias must hold one entry per weight row')
+    truth = _check_truth(truth, B)
     pred = torch.empty(B, dtype=torch.int64, device=feats.device)
-    truth = None if truth is None else _i64(truth).reshape(-1)
     rc = _native.lib().b200ocl_linear_argmax(_ptr(feats), B, d, _ptr(weight), _ptr(bias), weight.shape[0], _ptr(truth),
                                              _ptr(pred), _ptr(n_correct), _stream())
     _native.check(rc, 'b200ocl_linear_argmax')
