@@ -256,7 +256,8 @@ int b200ocl_net_train_ws_layout(const b200ocl_net_desc* desc, int N, int layer, 
  * halo strip (conv_tcp.cu, template nt), 2 wgmma with im2col tiles (conv_tc.cu, nt), 3 patch (bn, pt), 4 tiled (bn, pt),
  * 5 k-split (pt, kwarps), -1 none covers it.  th / tw / ti: the patch kernel's spatial tile.  stat_bytes: the batch-statistics
  * partials a train-mode launch writes (grid_x * channels * 2 doubles; 0 for the other passes); stat_region: the bytes
- * the workspace keeps for them.  sms: the SM count the plan is for. */
+ * the workspace keeps for them.  sms: the SM count the plan is for.  tp_ps / tp_bs: the halo-strip kernel's patch
+ * stages and weight ring depth (0 for the other kernels). */
 typedef struct {
   int kernel;
   int nt, bn, pt, kwarps;
@@ -264,6 +265,7 @@ typedef struct {
   int th, tw, ti;
   size_t stat_bytes, stat_region;
   int sms;
+  int tp_ps, tp_bs;
 } b200ocl_conv_geom;
 /* The launch of conv layer `layer` (BatchNorm2d module order) over N images in pass 0 train-mode forward, 1 eval-mode
  * forward or 2 data gradient (layers >= 1), on a GPU with sms SMs (0: the current device), and the statistics region of

@@ -760,6 +760,7 @@ ConvPlan conv_plan(const ConvArgs& a, int sms) {
     pl.nt = a.tp_bn <= 20 ? 32 : 48;   // tp_bn <= 40 (conv_tcp_eligible)
     pl.grid_x = conv_tcp_grid_x(a, sms);
     pl.grid_y = a.CN / a.tp_bn;
+    conv_tcp_pipeline(a, pl.nt, &pl.tp_ps, &pl.tp_bs);
     return pl;
   }
   if (tc) {

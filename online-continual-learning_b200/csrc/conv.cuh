@@ -70,9 +70,10 @@ __device__ __forceinline__ void bn_finalize(const ConvArgs& a, int c, double S, 
   a.run_var[c] = bn_running_update(a.run_var[c], (float)unbiased, a.momentum);
 }
 
-// conv_tcp.cu stages 128 + 2 * (W + 1) + 2 strip rows per tile, TP_LD_MAX per patch-loader thread (16 rows per pass).
-// The bound still counts the 128 + 2 * (W + 2) + 2 rows of the earlier two-position halo, so the eligible maps stay
-// those up to W = 37 wide.  The network plan builds halo-strip weight images exactly for the maps that fit.
+// conv_tcp.cu stages 128 + 2 * (W + 1) + 2 strip rows per tile; 16 * TP_LD_MAX is the bound on those rows (its patch
+// loaders size their per-thread loads from it).  The bound still counts the 128 + 2 * (W + 2) + 2 rows of the earlier
+// two-position halo, so the eligible maps stay those up to W = 37 wide.  The network plan builds halo-strip weight
+// images exactly for the maps that fit.
 constexpr int TP_LD_MAX = 13;
 inline bool tcp_strip_fits(int W) { return 128 + 2 * (W + 2) + 2 <= 16 * TP_LD_MAX; }
 
@@ -95,6 +96,7 @@ struct ConvPlan {
   int grid_x, grid_y;    // the grid; a train-mode launch writes grid_x * CN (sum, sum of squares) partials
   int th, tw, ti;        // CONV_K_PATCH: spatial tile (rows, columns, images)
   size_t smem;           // CONV_K_PATCH: dynamic shared memory
+  int tp_ps, tp_bs;      // CONV_K_TCP: patch stages and weight ring depth (conv_tcp_pipeline)
   const char* why;       // CONV_K_NONE: the reason
 };
 // Pure host function: every decision launch_conv takes, for a GPU with `sms` SMs.  CK == 3 is the stem.
@@ -106,6 +108,8 @@ bool conv_tc_eligible(const ConvArgs& a, int sms);
 int launch_conv_tc(const ConvArgs& a, const ConvPlan& pl, cudaStream_t stream);   // conv_tc.cu: wgmma 3xTF32 path
 bool conv_tcp_eligible(const ConvArgs& a);
 int conv_tcp_grid_x(const ConvArgs& a, int sms);   // persistent CTAs per channel tile of conv_tcp_kernel
+// Pure host function: the patch stages and weight ring depth conv_tcp_kernel<nt> runs with (its shared-memory fit).
+void conv_tcp_pipeline(const ConvArgs& a, int nt, int* ps, int* bs);
 int launch_conv_tcp(const ConvArgs& a, const ConvPlan& pl, cudaStream_t stream);  // conv_tcp.cu: wgmma fed from a halo patch
 
 }  // namespace b200ocl

@@ -26,13 +26,17 @@
 //
 // Per tile and slice the tensor core runs 9 taps x ceil(channels/8) K steps x 3 MMAs (3xTF32:
 // hi*hi + hi*lo + lo*hi); each tap accumulates into a fresh register fragment that is added into the fp32
-// sum in tap order (a long tensor-core accumulation truncates, see conv_tc.cu).  Roles:
-//   warps 0-7  two consumer warpgroups: warpgroup g issues the MMAs of tile rows 64g .. 64g+63 and promotes
-//              them; the fragments of a finished tile go through shared memory to warps 0-3, which run the
-//              epilogue with one pixel row per thread: folded eval BN (+ residual, ReLU) / raw / accumulate
-//   warp  8    weight loader (one elected lane): cp.async.bulk of pre-split, pre-swizzled [NT x 32] tiles,
-//              resident for the whole kernel when all 9 taps fit (cin <= 32), a ring otherwise
-//   warps 9-12 patch loaders: coalesced LDG.128 of NHWC pixels, cvt.rna.tf32 split, swizzled stores
+// sum in tap order (a long tensor-core accumulation truncates, see conv_tc.cu).  Two taps are in flight per
+// warpgroup: tap t+1 is issued into the other of two fragments before the wait that completes tap t, so the
+// tensor core works on t+1 while tap t is added into the sum.  Roles (four warpgroups, registers reallocated
+// with setmaxnreg: TP_REG_* below):
+//   warps 0-7   two consumer warpgroups: warpgroup g issues the MMAs of tile rows 64g .. 64g+63 and promotes
+//               them; a finished tile goes to one of two shared-memory tiles s_acc[2][128][NT + 1]
+//   warps 8-11  epilogue, one pixel row per thread: folded eval BN (+ residual, ReLU) / raw / accumulate,
+//               streamed in float4 chunks while the consumers run the next tile
+//   warp  12    weight loader (one elected lane): cp.async.bulk of pre-split, pre-swizzled [NT x 32] tiles,
+//               resident for the whole kernel when all 9 taps fit (cin <= 32), a ring otherwise
+//   warps 13-15 patch loaders: coalesced LDG.128 of NHWC pixels, cvt.rna.tf32 split, swizzled stores
 // CTAs are persistent over pixel tiles (one CTA per SM).  The kernel serves eval-mode forwards and
 // stride-1 data gradients; train-mode forwards, which need batch statistics, run on conv.cu or conv_tc.cu
 // (conv_tcp_eligible says why).
@@ -42,11 +46,22 @@
 namespace b200ocl {
 namespace {
 
-constexpr int TP_THREADS = 32 * 13;
-constexpr int TP_LOADER_WARP = 9;                   // first patch-loader warp; warp 8 loads the weights
+constexpr int TP_THREADS = 32 * 16;
+constexpr int TP_EPI_WARP = 8;                      // first epilogue warp
+constexpr int TP_WLOAD_WARP = 12;                   // weight loader
+constexpr int TP_LOADER_WARP = 13;                  // first patch-loader warp
+constexpr int TP_LOADERS = 96;                      // patch-loader threads: 8 chunks x 12 rows per pass
+constexpr int TP_LD = (16 * TP_LD_MAX + 11) / 12;   // loads per patch-loader thread: the rows tcp_strip_fits allows
 constexpr int TP_PS_MAX = 3;                        // patch stages: 3 when shared memory allows, else 2
 constexpr int TP_BS_MAX = 6;                        // weight ring depth (streaming mode): 6 or 4
 constexpr int TP_CONSUMER_WARPS = 8;                // arrivals that release a patch stage or a weight slot
+// Registers per thread after setmaxnreg: loaders, consumers (the fp32 sum and two fragments), epilogue.
+// 128 * P + 256 * C + 128 * E = 65536, the 128 per thread of the 512-thread launch.  The patch loaders hold 18 float4
+// loads across the stage wait and need all 128 (at 120 ptxas spills), so the loader warpgroup keeps its launch count;
+// the epilogue, which streams its row, hands 32 to the consumers.
+constexpr int TP_REG_LOAD = 128, TP_REG_MMA = 144, TP_REG_EPI = 96;
+static_assert(TP_REG_LOAD == 128, "the loader warpgroup runs no setmaxnreg");
+static_assert(128 * TP_REG_LOAD + 256 * TP_REG_MMA + 128 * TP_REG_EPI <= 65536, "register file");
 
 using umma::mbar_expect_tx;
 using umma::bulk_g2s;
@@ -69,7 +84,10 @@ __host__ __device__ inline TileGeom tile_geom(int N, int H, int W) {
   return g;
 }
 
-// One tap of one 32-channel slice into a fresh fragment: KS K steps (8 channels each) x 3 MMAs, then wait.
+// One tap of one 32-channel slice into a fresh fragment: KS K steps (8 channels each) x 3 MMAs, committed as one
+// group; the caller waits for it.  The commit stays inside each KS variant: committed after the caller's switch
+// joins, ptxas closes every variant's chain there itself and adds an empty group at the join, so a tap would be two
+// groups and wait_group 1 would leave only the empty one outstanding.
 template <int NT, int KS>
 __device__ __forceinline__ void issue_tap(float (&d)[NT / 2], uint64_t dAh, uint64_t dAl, uint64_t dBh, uint64_t dBl) {
   umma::fence();
@@ -81,8 +99,6 @@ __device__ __forceinline__ void issue_tap(float (&d)[NT / 2], uint64_t dAh, uint
     umma::mma_tf32_ss<NT>(d, dAl + adv, dBh + adv, 1u);
   }
   umma::commit();
-  umma::wait<0>();
-  umma::fence_regs(d);
 }
 
 template <int NT>
@@ -92,6 +108,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* patch0 = smem_raw;                                          // [PS][hi | lo][PROWS][128 B]
   __shared__ __align__(8) uint64_t pfull[TP_PS_MAX], pempty[TP_PS_MAX], bfull[9], bempty[TP_BS_MAX];
+  __shared__ __align__(8) uint64_t afull[2], aempty[2];   // s_acc buffer written by the consumers / read by the epilogue
   __shared__ int s_fail;
   __shared__ float s_coef[3 * 80];   // eval BN: mean, scale, shift per channel of the tile
 
@@ -101,20 +118,24 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
   const int slices = a.tp_slices;
   const TileGeom G = tile_geom(a.N, a.Hin, a.Win);
   const int PS = a.tp_ps, BS = a.tp_bs;            // patch stages, weight ring depth (launcher fits them to smem)
-  // the tile loops run to a.tp_tiles (= G.tiles_m): a kernel parameter is not a register live across them, which
-  // keeps conv_tcp_kernel<48> within 128 registers without spills
+  // the tile loops run to a.tp_tiles (= G.tiles_m): a kernel parameter is not a register live across them
   float* sB = reinterpret_cast<float*>(smem_raw + (size_t)PS * 2 * G.pbytes);   // weight blocks
   const bool resident = (slices == 1 && NT == 32);   // all 9 weight blocks stay in shared memory
   const int b_slots = resident ? 9 : BS;
-  float* s_acc = sB + (size_t)b_slots * B_BLOCK;   // [128][NT + 1] finished tile, one pixel row per epilogue thread
+  constexpr int ACC_TILE = 128 * (NT + 1);
+  float* s_acc = sB + (size_t)b_slots * B_BLOCK;   // [2][128][NT + 1] finished tiles, one pixel row per epilogue thread
 
   if (tid == 0) {
     for (int i = 0; i < TP_PS_MAX; ++i) {
-      umma::mbar_init(&pfull[i], 128);
+      umma::mbar_init(&pfull[i], TP_LOADERS);
       umma::mbar_init(&pempty[i], TP_CONSUMER_WARPS);
     }
     for (int i = 0; i < 9; ++i) umma::mbar_init(&bfull[i], 1);
     for (int i = 0; i < TP_BS_MAX; ++i) umma::mbar_init(&bempty[i], TP_CONSUMER_WARPS);
+    for (int i = 0; i < 2; ++i) {
+      umma::mbar_init(&afull[i], 256);    // every consumer thread, after its stores
+      umma::mbar_init(&aempty[i], 128);   // every epilogue thread, after its reads
+    }
     umma::fence_mbar_init();
     s_fail = 0;
   }
@@ -122,19 +143,19 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
   const float* wimg = a.w_tp + (size_t)blockIdx.y * slices * 9 * B_BLOCK;
 
   if (warp >= TP_LOADER_WARP) {
-    // =========================================================== patch loaders (128 threads)
+    // =========================================================== patch loaders (96 threads)
     const int lt = tid - 32 * TP_LOADER_WARP;
     int pc = 0;
     for (int tile = blockIdx.x; tile < a.tp_tiles; tile += gridDim.x) {
       for (int sl = 0; sl < slices; ++sl, ++pc) {
         const int ch_valid = min(32, a.CK - sl * 32);       // real channels in this slice (multiple of 4)
         const int nch = 2 * ((ch_valid + 7) / 8);            // 16-byte chunks the MMAs will read per row
-        // thread -> (patch row lt/8 + 16*i, chunk lt%8): lanes with chunk >= nch idle
+        // thread -> (patch row lt/8 + 12*i, chunk lt%8): lanes with chunk >= nch idle
         const int ch = lt & 7, r0 = lt >> 3;
         const int nrow = G.prow;
         const bool ch_live = ch < nch, ch_real = ch * 4 < ch_valid;
-        float4 v[TP_LD_MAX];
-        // strip position of this thread's first row, then 16 rows further per pass (no divisions in the loop)
+        float4 v[TP_LD];
+        // strip position of this thread's first row, then 12 rows further per pass (no divisions in the loop)
         int img, yp, xp;
         {
           const int sp = tile * 128 + r0;
@@ -145,15 +166,15 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
         }
         const int hp = a.Hin + 1;                             // strip rows per image: the zero row, then H pixel rows
 #pragma unroll
-        for (int i = 0; i < TP_LD_MAX; ++i) {
+        for (int i = 0; i < TP_LD; ++i) {
           v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-          const int ri = r0 + 16 * i;
+          const int ri = r0 + 12 * i;
           if (ch_real && ri < nrow) {
             const int y = yp - 1, x = xp - 1;
             if (img < a.N && (unsigned)y < (unsigned)a.Hin && (unsigned)x < (unsigned)a.Win)
               v[i] = __ldg(reinterpret_cast<const float4*>(a.in + ((size_t)(img * a.Hin + y) * a.Win + x) * a.CK + sl * 32) + ch);
           }
-          xp += 16;
+          xp += 12;
           while (xp >= G.wp) {
             xp -= G.wp;
             if (++yp == hp) {
@@ -168,8 +189,8 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
         float* pl = ph + G.pbytes / 4;
         if (ch_live) {
 #pragma unroll
-          for (int i = 0; i < TP_LD_MAX; ++i) {
-            const int ri = r0 + 16 * i;
+          for (int i = 0; i < TP_LD; ++i) {
+            const int ri = r0 + 12 * i;
             if (ri < nrow) {
               float4 h, l;
               umma::split_tf32(v[i].x, h.x, l.x); umma::split_tf32(v[i].y, h.y, l.y);
@@ -184,7 +205,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
         umma::mbar_arrive(&pfull[ps]);
       }
     }
-  } else if (warp == TP_LOADER_WARP - 1) {
+  } else if (warp == TP_WLOAD_WARP) {
     // =========================================================== weight loader (one elected lane)
     const uint32_t bytes = (uint32_t)(B_BLOCK * sizeof(float));
     if (resident) {
@@ -208,14 +229,73 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
             __syncwarp();
           }
     }
+  } else if (warp >= TP_EPI_WARP) {
+    // =========================================================== epilogue (warps 8-11)
+    umma::reg_dealloc<TP_REG_EPI>();
+    const int et = tid - 32 * TP_EPI_WARP;               // pixel row of the tile
+    if (a.mode == CONV_EVAL) {
+      for (int c = et; c < bn; c += 128) {
+        const float inv = 1.0f / sqrtf(a.rvar[n0 + c] + a.eps);
+        s_coef[c] = a.rmean[n0 + c];
+        s_coef[80 + c] = inv * a.gamma[n0 + c];
+        s_coef[160 + c] = a.beta[n0 + c];
+      }
+      asm volatile("bar.sync 1, 128;\n" ::);
+    }
+    int k = 0;                                           // tiles this CTA has finished
+    for (int tile = blockIdx.x; tile < a.tp_tiles; tile += gridDim.x, ++k) {
+      const int buf = k & 1;
+      const int sp = tile * 128 + et;                    // strip position of this MMA row
+      const int img = sp / G.pp, rem = sp - img * G.pp;
+      const int y = rem / G.wp, x = rem - y * G.wp;
+      const bool valid = img < a.N && y < a.Hin && x < a.Win;   // halo positions are by-products
+      const size_t m = ((size_t)img * a.Hin + y) * a.Win + x;   // stride 1: output pixel = input pixel
+      // src = the residual (eval) or the gradient being accumulated into (data gradient); pre is 0 without one
+      const float* src = nullptr;
+      if (valid && a.mode == CONV_EVAL && a.residual) src = a.residual + m * a.CN + n0;
+      if (valid && a.mode == CONV_ACCUM) src = a.out + m * a.CN + n0;
+      // All of the row's loads are issued before the wait, so their latency hides behind the consumers' tile: src
+      // may be the output itself (accumulate) or alias it, so a load after a store could not be moved ahead of it.
+      float pre[NT];
+#pragma unroll
+      for (int c = 0; c < NT; ++c) pre[c] = 0.f;
+      if (src) {
+#pragma unroll
+        for (int c0 = 0; c0 < NT; c0 += 4) {
+          if (c0 >= bn) break;
+          const float4 v = *reinterpret_cast<const float4*>(src + c0);
+          pre[c0] = v.x; pre[c0 + 1] = v.y; pre[c0 + 2] = v.z; pre[c0 + 3] = v.w;
+        }
+      }
+      if (!umma::mbar_wait(&afull[buf], (uint32_t)((k >> 1) & 1))) s_fail = 1;
+      const float* row = s_acc + (size_t)buf * ACC_TILE + et * (NT + 1);
+      if (valid) {
+        float* o = a.out + m * a.CN + n0;
+#pragma unroll
+        for (int c0 = 0; c0 < NT; c0 += 4) {   // the tile's row streams from s_acc a float4 at a time
+          if (c0 >= bn) break;
+          float rr[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float acc = row[c0 + j];
+            if (a.mode == CONV_EVAL) {
+              rr[j] = (acc - s_coef[c0 + j]) * s_coef[80 + c0 + j] + s_coef[160 + c0 + j];
+              rr[j] += pre[c0 + j];                       // residual (0 when there is none)
+              if (a.relu) rr[j] = fmaxf(rr[j], 0.f);
+            } else {
+              rr[j] = acc + pre[c0 + j];                  // raw: pre == 0; accumulate: pre = previous contents
+            }
+          }
+          *reinterpret_cast<float4*>(o + c0) = make_float4(rr[0], rr[1], rr[2], rr[3]);
+        }
+      }
+      umma::mbar_arrive(&aempty[buf]);
+    }
   } else {
-    // =========================================================== consumers (warps 0-7) + epilogue (warps 0-3)
+    // =========================================================== consumers (warps 0-7)
+    umma::reg_alloc<TP_REG_MMA>();
     const int g = warp >> 2, wt = tid & 127;            // warpgroup, thread inside it
-    const int et = tid;                                  // epilogue threads 0..127 = pixel row of the tile
-    const bool epi = tid < 128;
     const bool lane0 = (tid & 31) == 0;
-    auto esync = []() { asm volatile("bar.sync 1, 128;\n" ::); };
-    auto csync = []() { asm volatile("bar.sync 2, 256;\n" ::); };
     // descriptor templates: only the 14-bit start-address field (16-byte units) changes per stage / tap / K step
     const uint64_t dA0 = umma::make_smem_desc_sw128(umma::smem_u32(patch0) + (uint32_t)(g * 64 * 128));
     const uint64_t dB0 = umma::make_smem_desc_sw128(umma::smem_u32(sB));
@@ -223,110 +303,96 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
     const uint32_t A_STAGE = (uint32_t)(2 * G.pbytes) >> 4;
     constexpr uint32_t B_LO = (NT * 128) >> 4;
     constexpr uint32_t B_SLOT = (B_BLOCK * 4) >> 4;
-    if (epi && a.mode == CONV_EVAL) {
-      for (int c = et; c < bn; c += 128) {
-        const float inv = 1.0f / sqrtf(a.rvar[n0 + c] + a.eps);
-        s_coef[c] = a.rmean[n0 + c];
-        s_coef[80 + c] = inv * a.gamma[n0 + c];
-        s_coef[160 + c] = a.beta[n0 + c];
-      }
-      esync();
-    }
-    int pc = 0, q = 0;                       // (tile, slice) pairs; position in the weight stream
+    const int T = 9 * slices;                // taps per tile
+    // Issue side: patch stage and its phase, weight slot and its phase.  Retire side: the stage and slot to release.
+    // All run on over the CTA's tiles; counters wrap instead of dividing.
+    int ips = 0, ib = 0, rps = 0, rb = 0;
+    uint32_t ipph = 0, ibph = 0;
     bool b_ready = false;
-    for (int tile = blockIdx.x; tile < a.tp_tiles; tile += gridDim.x) {
+    int k = 0;                               // tiles this CTA has finished
+    for (int tile = blockIdx.x; tile < a.tp_tiles; tile += gridDim.x, ++k) {
       float accf[R];
 #pragma unroll
       for (int i = 0; i < R; ++i) accf[i] = 0.f;
-      for (int sl = 0; sl < slices; ++sl, ++pc) {
-        const int ps = pc % PS;
-        const int ksteps = (min(32, a.CK - sl * 32) + 7) / 8;
-        if (!umma::mbar_wait(&pfull[ps], (uint32_t)((pc / PS) & 1))) s_fail = 1;
-        const uint64_t dAs = dA0 + (uint64_t)(ps * A_STAGE);
+      // The tile's T taps as one stream (slice by slice, tap order within a slice).  Issue position (is, it) runs
+      // one tap ahead of the retire position rt; a weight slot or patch stage is released once the wait that
+      // completes the last MMA reading it has returned.
+      int is = 0, it = 0, rt = 0;
+      auto issue = [&](float (&d)[R]) {
+        if (it == 0)
+          if (!umma::mbar_wait(&pfull[ips], ipph)) s_fail = 1;
+        const int b = resident ? it : ib;
+        if (!(resident && b_ready))
+          if (!umma::mbar_wait(&bfull[b], resident ? 0u : ibph)) s_fail = 1;
+        const int kh = it / 3, kw = it - 3 * kh;
+        const uint64_t dAh = dA0 + (uint64_t)(ips * A_STAGE) + (uint64_t)((kh * G.wp + kw) * 8);   // + (kh*(W+1) + kw) rows
+        const uint64_t dAl = dAh + A_LO;
+        const uint64_t dBh = dB0 + (uint64_t)(b * B_SLOT);
+        const uint64_t dBl = dBh + B_LO;
+        switch ((min(32, a.CK - is * 32) + 7) / 8) {   // straight-line issue sequences: a run-time trip count
+          case 1: issue_tap<NT, 1>(d, dAh, dAl, dBh, dBl); break;   // would serialise the MMAs
+          case 2: issue_tap<NT, 2>(d, dAh, dAl, dBh, dBl); break;
+          case 3: issue_tap<NT, 3>(d, dAh, dAl, dBh, dBl); break;
+          default: issue_tap<NT, 4>(d, dAh, dAl, dBh, dBl); break;
+        }
+        if (!resident && ++ib == BS) {
+          ib = 0;
+          ibph ^= 1u;
+        }
+        if (++it == 9) {
+          it = 0;
+          ++is;
+          b_ready = true;
+          if (++ips == PS) {
+            ips = 0;
+            ipph ^= 1u;
+          }
+        }
+      };
+      auto retire = [&](float (&d)[R]) {
+        umma::fence_regs(d);
+#pragma unroll
+        for (int i = 0; i < R; ++i) accf[i] += d[i];
+        if (!resident) {
+          if (lane0) umma::mbar_arrive(&bempty[rb]);
+          if (++rb == BS) rb = 0;
+        }
+        if (rt == 8) {
+          if (lane0) umma::mbar_arrive(&pempty[rps]);
+          if (++rps == PS) rps = 0;
+        }
+        if (++rt == 9) rt = 0;
+      };
+      // Every exit drains with wait<0> in the block that leaves the loop, so that the compiler sees no fragment
+      // in flight past it.
+      float fa[R], fb[R];
+      issue(fa);
 #pragma unroll 1
-        for (int tap = 0; tap < 9; ++tap, ++q) {
-          const int kh = tap / 3, kw = tap - 3 * kh;
-          const int b = resident ? tap : q % BS;
-          if (!(resident && b_ready))
-            if (!umma::mbar_wait(&bfull[b], resident ? 0u : (uint32_t)((q / BS) & 1))) s_fail = 1;
-          const uint64_t dAh = dAs + (uint64_t)((kh * G.wp + kw) * 8);   // + (kh*(W+1) + kw) rows of 128 B
-          const uint64_t dAl = dAh + A_LO;
-          const uint64_t dBh = dB0 + (uint64_t)(b * B_SLOT);
-          const uint64_t dBl = dBh + B_LO;
-          float tmp[R];
-          switch (ksteps) {   // straight-line issue sequences: a run-time trip count would serialise the MMAs
-            case 1: issue_tap<NT, 1>(tmp, dAh, dAl, dBh, dBl); break;
-            case 2: issue_tap<NT, 2>(tmp, dAh, dAl, dBh, dBl); break;
-            case 3: issue_tap<NT, 3>(tmp, dAh, dAl, dBh, dBl); break;
-            default: issue_tap<NT, 4>(tmp, dAh, dAl, dBh, dBl); break;
-          }
-#pragma unroll
-          for (int i = 0; i < R; ++i) accf[i] += tmp[i];
-          if (!resident && lane0) umma::mbar_arrive(&bempty[b]);
+      for (int j = 0;; j += 2) {   // fa holds tap j, fb tap j + 1
+        if (j + 1 >= T) {
+          umma::wait<0>();
+          retire(fa);
+          break;
         }
-        b_ready = true;
-        if (lane0) umma::mbar_arrive(&pempty[ps]);
-      }
-      // ---- fragments -> pixel rows: the previous tile's epilogue has finished reading s_acc at the first barrier
-      csync();
-#pragma unroll
-      for (int i = 0; i < R; ++i) s_acc[(64 * g + umma::frag_row(wt, i)) * (NT + 1) + umma::frag_col(wt, i)] = accf[i];
-      csync();
-      if (!epi) continue;
-      const int sp = tile * 128 + et;                    // strip position of this MMA row
-      const int img = sp / G.pp, rem = sp - img * G.pp;
-      const int y = rem / G.wp, x = rem - y * G.wp;
-      const bool valid = img < a.N && y < a.Hin && x < a.Win;   // halo positions are by-products
-      const size_t m = ((size_t)img * a.Hin + y) * a.Win + x;   // stride 1: output pixel = input pixel
-      // pre[] = the residual (eval) or the gradient being accumulated into (data gradient), 0 otherwise; the
-      // loads are issued before the tile's row is read back from s_acc.
-      float acc[NT], pre[NT];
-#pragma unroll
-      for (int c = 0; c < NT; ++c) {
-        acc[c] = 0.f;
-        pre[c] = 0.f;
-      }
-      {
-        const float* src = nullptr;
-        if (valid && a.mode == CONV_EVAL && a.residual) src = a.residual + m * a.CN + n0;
-        if (valid && a.mode == CONV_ACCUM) src = a.out + m * a.CN + n0;
-        if (src) {
-#pragma unroll
-          for (int c0 = 0; c0 < NT; c0 += 4) {
-            if (c0 >= bn) break;
-            const float4 v = *reinterpret_cast<const float4*>(src + c0);
-            pre[c0] = v.x; pre[c0 + 1] = v.y; pre[c0 + 2] = v.z; pre[c0 + 3] = v.w;
-          }
+        issue(fb);
+        umma::wait<1>();
+        retire(fa);
+        if (j + 2 >= T) {
+          umma::wait<0>();
+          retire(fb);
+          break;
         }
+        issue(fa);
+        umma::wait<1>();
+        retire(fb);
       }
+      // ---- fragments -> pixel rows of s_acc[k % 2], once the epilogue has read that buffer's previous tile
+      const int buf = k & 1;
+      if (!umma::mbar_wait(&aempty[buf], (uint32_t)(((k >> 1) & 1) ^ 1))) s_fail = 1;
+      float* acc_out = s_acc + (size_t)buf * ACC_TILE;
 #pragma unroll
-      for (int c = 0; c < NT; ++c) acc[c] = s_acc[et * (NT + 1) + c];
-      if (a.mode == CONV_EVAL) {
-        if (valid) {
-          float* o = a.out + m * a.CN + n0;
-#pragma unroll
-          for (int c0 = 0; c0 < NT; c0 += 4) {
-            if (c0 >= bn) break;
-            float rr[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              rr[j] = (acc[c0 + j] - s_coef[c0 + j]) * s_coef[80 + c0 + j] + s_coef[160 + c0 + j];
-              rr[j] += pre[c0 + j];                       // residual (0 when there is none)
-              if (a.relu) rr[j] = fmaxf(rr[j], 0.f);
-            }
-            *reinterpret_cast<float4*>(o + c0) = make_float4(rr[0], rr[1], rr[2], rr[3]);
-          }
-        }
-      } else if (valid) {
-        float* o = a.out + m * a.CN + n0;
-#pragma unroll
-        for (int c0 = 0; c0 < NT; c0 += 4) {
-          if (c0 >= bn) break;
-          // raw: pre == 0; accumulate: pre = previous contents
-          *reinterpret_cast<float4*>(o + c0) = make_float4(acc[c0] + pre[c0], acc[c0 + 1] + pre[c0 + 1],
-                                                           acc[c0 + 2] + pre[c0 + 2], acc[c0 + 3] + pre[c0 + 3]);
-        }
-      }
+      for (int i = 0; i < R; ++i) acc_out[(64 * g + umma::frag_row(wt, i)) * (NT + 1) + umma::frag_col(wt, i)] = accf[i];
+      umma::mbar_arrive(&afull[buf]);
     }
   }
   __syncthreads();
@@ -338,21 +404,26 @@ template <int NT>
 size_t tcp_smem_bytes(const TileGeom& G, int slices, int ps, int bs) {
   const int b_slots = (slices == 1 && NT == 32) ? 9 : bs;
   return (size_t)ps * 2 * G.pbytes + (size_t)b_slots * 2 * NT * 32 * sizeof(float) +
-         (size_t)128 * (NT + 1) * sizeof(float) + 1024;
+         (size_t)2 * 128 * (NT + 1) * sizeof(float) + 1024;
+}
+
+// Deepest pipeline that fits next to the two s_acc tiles: 3 patch stages + 6 weight slots, 3 + 4, 2 + 6, else 2 + 4
+// (two taps in flight hold two slots and two stages at once, so both stay >= 2).  The network's maps: 32x32
+// (resident weights) keeps 2 stages, 8x8 and 4x4 keep 3 + 4, 16x16 goes from 3 + 4 (one s_acc tile) to 2 + 6.
+template <int NT>
+void fit_pipeline(const ConvArgs& a, int* ps, int* bs) {
+  const TileGeom G = tile_geom(a.N, a.Hin, a.Win);
+  const size_t limit = 227 * 1024 - 4096;      // static shared memory (barriers, coefficients) comes on top
+  *ps = 3; *bs = 6;
+  if (tcp_smem_bytes<NT>(G, a.tp_slices, *ps, *bs) > limit) *bs = 4;
+  if (tcp_smem_bytes<NT>(G, a.tp_slices, *ps, *bs) > limit) { *ps = 2; *bs = 6; }
+  if (tcp_smem_bytes<NT>(G, a.tp_slices, *ps, *bs) > limit) *bs = 4;
 }
 
 template <int NT>
 int launch_tcp(ConvArgs a, const ConvPlan& pl, cudaStream_t stream) {
   const TileGeom G = tile_geom(a.N, a.Hin, a.Win);
-  // Deepest pipeline that fits: 3 patch stages + 6 weight slots, 3 + 4, else 2 + 6.  The fit still sets aside the
-  // [128][bn + 1] float scratch of the batch-statistics epilogue this kernel used to have (the smem it allocates does
-  // not include it), so every shape keeps the depth it was measured with; handing that room to deeper pipelines is a
-  // performance change of its own.
-  const size_t limit = 227 * 1024 - 4096      // static shared memory (barriers, coefficients) comes on top
-                       - (size_t)128 * (a.tp_bn + 1) * sizeof(float);
-  a.tp_ps = 3; a.tp_bs = 6;
-  if (tcp_smem_bytes<NT>(G, a.tp_slices, a.tp_ps, a.tp_bs) > limit) a.tp_bs = 4;
-  if (tcp_smem_bytes<NT>(G, a.tp_slices, a.tp_ps, a.tp_bs) > limit) { a.tp_ps = 2; a.tp_bs = 6; }
+  fit_pipeline<NT>(a, &a.tp_ps, &a.tp_bs);
   const size_t smem = tcp_smem_bytes<NT>(G, a.tp_slices, a.tp_ps, a.tp_bs);
   B200OCL_CUDA(raise_smem_limit<conv_tcp_kernel<NT>>(smem));
   a.tp_tiles = G.tiles_m;
@@ -365,6 +436,11 @@ int launch_tcp(ConvArgs a, const ConvPlan& pl, cudaStream_t stream) {
 }
 
 }  // namespace
+
+void conv_tcp_pipeline(const ConvArgs& a, int nt, int* ps, int* bs) {
+  if (nt == 32) fit_pipeline<32>(a, ps, bs);
+  else fit_pipeline<48>(a, ps, bs);
+}
 
 int conv_tcp_grid_x(const ConvArgs& a, int sms) {
   const TileGeom G = tile_geom(a.N, a.Hin, a.Win);

@@ -1204,6 +1204,8 @@ static void report_geom(const b200ocl::ConvPlan& pl, size_t stat_bytes, size_t s
   out->stat_bytes = stat_bytes;
   out->stat_region = stat_region;
   out->sms = sms;
+  out->tp_ps = pl.tp_ps;
+  out->tp_bs = pl.tp_bs;
 }
 
 int b200ocl_conv_selftest_geom(int N, int H, int W, int cin, int cout, int ks, int stride, int dgrad, int path, int mode,

@@ -53,6 +53,13 @@ __device__ __forceinline__ void fence_regs(float (&d)[R]) {
 #pragma unroll
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+// ---- per-warpgroup register reallocation (all four warps of a warpgroup execute it).  The kernel launches with its
+// __launch_bounds__ register count; a warpgroup that needs less gives registers back to the pool and one that needs
+// more blocks in setmaxnreg.inc until the pool holds them.  N: a multiple of 8 in 24 .. 256.
+template <int N>
+__device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(N)); }
 // generic-proxy shared-memory writes -> visible to the async proxy (tensor core operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::); }
 

@@ -50,11 +50,11 @@ class NetWsLayout(ctypes.Structure):
 
 
 class ConvGeom(ctypes.Structure):
-    """b200ocl_conv_geom: the convolution kernel one launch runs, its template parameters and grid, and the statistics
-    partials it writes against the workspace region kept for them."""
+    """b200ocl_conv_geom: the convolution kernel one launch runs, its template parameters and grid, the statistics
+    partials it writes against the workspace region kept for them, and the halo-strip kernel's pipeline depths."""
     _fields_ = [('kernel', c_int), ('nt', c_int), ('bn', c_int), ('pt', c_int), ('kwarps', c_int), ('grid_x', c_int),
                 ('grid_y', c_int), ('th', c_int), ('tw', c_int), ('ti', c_int), ('stat_bytes', c_size_t),
-                ('stat_region', c_size_t), ('sms', c_int)]
+                ('stat_region', c_size_t), ('sms', c_int), ('tp_ps', c_int), ('tp_bs', c_int)]
 
     KERNELS = ('stem', 'tcp', 'tc', 'patch', 'tiled', 'ksplit')
 
