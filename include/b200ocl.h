@@ -67,6 +67,28 @@ int b200ocl_knn_sv(const float* eval_f, const int64_t* eval_y, const float* cand
                    float* sv, float* col_sum, float* col_max, float* col_min,
                    void* workspace, size_t workspace_bytes, void* stream);
 
+/* The launch b200ocl_knn_sv makes for E eval rows, C candidates and width d on a GPU with sms SMs (0: the current
+ * device), with aligned != 0 when eval_f and cand_f are 16-byte aligned and want_red != 0 when any column reduction is
+ * asked for.  family: the fused kernel (C <= 1024) with kpl keys per lane, te eval rows per tile and, for kpl = 32 /
+ * te = 16, the wide phase 1 (wide = 1) or the row-tiled one; or the scratch-line kernel (C > 1024) over cpad keys per
+ * row, sorted in shared-memory blocks of block_keys keys with far_stages compare stages through global memory.
+ * grid: CTAs; tiles_per_cta: the most eval tiles (fused) or rows (large) one CTA takes; smem_bytes: dynamic shared
+ * memory, smem_limit: the limit the launcher raises the kernel to; part_bytes: the column partials the launch writes
+ * (at workspace offset 256); key_offset / key_bytes: the large kernel's key lines; workspace_bytes: what
+ * b200ocl_knn_sv_workspace_bytes returns on a GPU with sms SMs.  Host only, launches nothing; exists so that tests can
+ * check which kernels a shape reaches and that every plan fits on any SM count. */
+#define B200OCL_KNN_FUSED 0
+#define B200OCL_KNN_LARGE 1
+typedef struct {
+  int family;
+  int kpl, te, wide;
+  int cpad, block_keys, far_stages;
+  int grid, n_tiles, tiles_per_cta;
+  size_t smem_bytes, smem_limit, part_bytes, key_offset, key_bytes, workspace_bytes;
+  int sms;
+} b200ocl_knn_launch;
+int b200ocl_knn_sv_plan(int E, int C, int d, int aligned, int want_red, int sms, b200ocl_knn_launch* out);
+
 /* ---------------------------------------------------------------- ranking
  * score[i] = a[i]*sa + (b ? b[i]*sb : 0); idx_out[0..n_out) = positions of the n_out
  * largest scores in descending order, ties lowest index first (the reference's

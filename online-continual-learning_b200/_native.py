@@ -18,6 +18,7 @@ SIGNATURES = {
     'b200ocl_profile_get': (c_int, [c_int, P, c_int, P, P, P]),
     'b200ocl_knn_sv_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'b200ocl_knn_sv': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, P, P, P, P, P, c_size_t, P]),
+    'b200ocl_knn_sv_plan': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, P]),
     'b200ocl_rank_desc': (c_int, [P, c_float, P, c_float, c_int, P, c_int, P, P]),
     'b200ocl_supcon_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'b200ocl_supcon': (c_int, [P, P, c_int, c_int, c_int, c_float, P, P, P, c_size_t, P]),

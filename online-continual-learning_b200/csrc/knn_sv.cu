@@ -130,6 +130,7 @@ __global__ void __launch_bounds__(KNN_THREADS) knn_sv_kernel(KnnSvParams p) {
     // Same per-pair fma order over the features, so the distances are bit-identical to the other tiling.
     bool wide_done = false;
     if constexpr (KPL == 32 && TE == 16) {
+      // knn_wide_form (host, below) restates this predicate for the launch plan: keep the two equal.
       if (p.d % 8 == 0 && (reinterpret_cast<uintptr_t>(p.eval_f) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.cand_f) & 15) == 0) {
         constexpr int DKW = 8;
         float* se_w = se;   // [DKW][16]
@@ -367,51 +368,87 @@ __global__ void __launch_bounds__(KNN_THREADS) knn_sv_kernel(KnnSvParams p) {
   }
 }
 
-template <int KPL, int TE>
-constexpr size_t knn_smem_bytes() {
-  constexpr int CPAD = 32 * KPL;
-  constexpr int NJ = KPL < 8 ? KPL : 8;
-  constexpr int CT = 32 * NJ;
-  return (size_t)(TE * CPAD + KNN_DK * (TE + 1) + KNN_DK * (CT + 1) + 3 * KNN_WARPS * CPAD) * sizeof(float) +
-         (size_t)CPAD * sizeof(long long);
+constexpr size_t knn_smem_bytes(int kpl, int te) {
+  const int cpad = 32 * kpl;
+  const int ct = 32 * (kpl < 8 ? kpl : 8);
+  return (size_t)(te * cpad + KNN_DK * (te + 1) + KNN_DK * (ct + 1) + 3 * KNN_WARPS * cpad) * sizeof(float) +
+         (size_t)cpad * sizeof(long long);
 }
 
-int knn_grid_cap() { return sm_count(); }
+// Host copy of the wide phase-1 predicate that knn_sv_kernel evaluates in phase 1 (KPL == 32, TE == 16, d % 8 == 0,
+// eval_f and cand_f 16-byte aligned).  The kernel decides on its own; this copy only reports the decision in the
+// launch plan, so it must stay equal to the kernel's.
+bool knn_wide_form(int kpl, int te, int d, bool aligned) { return kpl == 32 && te == 16 && d % 8 == 0 && aligned; }
+
+size_t knn_fused_workspace_bytes(int C, int sms) {
+  return 256 + align_up((size_t)sms * 3 * (size_t)C * sizeof(float), 256);
+}
 
 template <int KPL, int TE>
-int launch_knn(const KnnSvParams& p0, cudaStream_t stream) {
+int launch_knn(const KnnSvParams& p0, const b200ocl_knn_launch& L, cudaStream_t stream) {
   KnnSvParams p = p0;
-  constexpr size_t smem = knn_smem_bytes<KPL, TE>();
-  static_assert(smem <= 227 * 1024, "kNN-SV tile does not fit in shared memory");
-  p.n_tiles = (p.E + TE - 1) / TE;
-  int grid = p.n_tiles < knn_grid_cap() ? p.n_tiles : knn_grid_cap();
-  if (grid < 1) grid = 1;
-  B200OCL_CUDA((raise_smem_limit<knn_sv_kernel<KPL, TE>>(smem)));
+  static_assert(knn_smem_bytes(KPL, TE) <= 227 * 1024, "kNN-SV tile does not fit in shared memory");
+  p.n_tiles = L.n_tiles;
+  B200OCL_CUDA((raise_smem_limit<knn_sv_kernel<KPL, TE>>(L.smem_limit)));
   B200OCL_PROF("knn_sv", 4.0 * p.d * ((double)p.E + p.C) + 8.0 * ((double)p.E + p.C) + 4.0 * p.C * 3 + (p.sv ? 4.0 * p.E * p.C : 0.0), stream);
-  knn_sv_kernel<KPL, TE><<<grid, KNN_THREADS, smem, stream>>>(p);
+  knn_sv_kernel<KPL, TE><<<L.grid, KNN_THREADS, L.smem_bytes, stream>>>(p);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }
 
 template <int KPL>
-int dispatch_te(const KnnSvParams& p, cudaStream_t stream) {
-  // Few rows: small tiles so that more SMs take part.  Many rows: 32-row tiles for operand reuse
-  // (KPL=32 keeps 16 so that the three reduction arrays still fit).
-  if (p.E <= 8 * knn_grid_cap()) return launch_knn<KPL, 8>(p, stream);
+int dispatch_te(const KnnSvParams& p, const b200ocl_knn_launch& L, cudaStream_t stream) {
+  if (L.te == 8) return launch_knn<KPL, 8>(p, L, stream);
   if constexpr (KPL == 32) {
-    return launch_knn<KPL, 16>(p, stream);
+    return launch_knn<KPL, 16>(p, L, stream);
   } else {
-    return launch_knn<KPL, 32>(p, stream);
+    return launch_knn<KPL, 32>(p, L, stream);
   }
 }
 
 }  // namespace
 
 // knn_sv_large.cu
-size_t knn_large_workspace_bytes(int C);
+int knn_large_max_d();
+size_t knn_large_workspace_bytes(int C, int sms);
+void knn_large_plan(int E, int C, int d, bool want_red, int sms, b200ocl_knn_launch* L);
 int launch_knn_large(const float* eval_f, const long long* eval_y, const float* cand_f, const long long* cand_y, int E, int C,
                      int d, int k, float* sv, float* col_sum, float* col_max, float* col_min, void* workspace,
-                     size_t workspace_bytes, cudaStream_t stream);
+                     size_t workspace_bytes, const b200ocl_knn_launch& L, cudaStream_t stream);
+
+size_t knn_workspace_bytes(int C, int sms) {
+  if (C < 0) C = 0;
+  return C > B200OCL_KNN_MAX_CAND ? knn_large_workspace_bytes(C, sms) : knn_fused_workspace_bytes(C, sms);
+}
+
+// The one place that decides which kNN-SV kernel a call launches (b200ocl_knn_sv launches what this returns;
+// b200ocl_knn_sv_plan reports it).  Host only.  E, C >= 1; C <= B200OCL_KNN_MAX_CAND_LARGE, and d <= the large kernel's
+// limit when C > B200OCL_KNN_MAX_CAND (the callers check both).
+b200ocl_knn_launch knn_plan(int E, int C, int d, bool aligned, bool want_red, int sms) {
+  b200ocl_knn_launch L{};
+  L.sms = sms;
+  L.workspace_bytes = knn_workspace_bytes(C, sms);
+  if (C > B200OCL_KNN_MAX_CAND) {   // rows too long for the register-resident sort: scratch-line path
+    knn_large_plan(E, C, d, want_red, sms, &L);
+    return L;
+  }
+  L.family = B200OCL_KNN_FUSED;
+  L.kpl = C <= 32 ? 1 : C <= 64 ? 2 : C <= 128 ? 4 : C <= 256 ? 8 : C <= 512 ? 16 : 32;
+  // Few rows: small tiles so that more SMs take part.  Many rows: 32-row tiles for operand reuse
+  // (KPL=32 keeps 16 so that the three reduction arrays still fit).
+  L.te = E <= 8 * sms ? 8 : (L.kpl == 32 ? 16 : 32);
+  L.wide = knn_wide_form(L.kpl, L.te, d, aligned) ? 1 : 0;
+  L.cpad = 32 * L.kpl;
+  L.n_tiles = (E + L.te - 1) / L.te;
+  L.grid = L.n_tiles < sms ? L.n_tiles : sms;
+  if (L.grid < 1) L.grid = 1;
+  L.tiles_per_cta = (L.n_tiles + L.grid - 1) / L.grid;
+  L.smem_bytes = knn_smem_bytes(L.kpl, L.te);
+  L.smem_limit = L.smem_bytes;      // the launcher raises each instantiation to exactly what it uses
+  L.part_bytes = want_red ? (size_t)L.grid * 3 * (size_t)C * sizeof(float) : 0;
+  return L;
+}
+
 }  // namespace b200ocl
 
 extern "C" {
@@ -419,9 +456,7 @@ extern "C" {
 size_t b200ocl_knn_sv_workspace_bytes(int E, int C, int d) {
   (void)E;
   (void)d;
-  if (C < 0) C = 0;
-  if (C > B200OCL_KNN_MAX_CAND) return b200ocl::knn_large_workspace_bytes(C);
-  return 256 + b200ocl::align_up((size_t)b200ocl::knn_grid_cap() * 3 * (size_t)C * sizeof(float), 256);
+  return b200ocl::knn_workspace_bytes(C, b200ocl::sm_count());
 }
 
 int b200ocl_knn_sv(const float* eval_f, const int64_t* eval_y, const float* cand_f, const int64_t* cand_y, int E,
@@ -445,10 +480,16 @@ int b200ocl_knn_sv(const float* eval_f, const int64_t* eval_y, const float* cand
     return B200OCL_OK;
   }
   B200OCL_CHECK_ARG(eval_f && eval_y && cand_f && cand_y, "null input pointer");
-  if (C > B200OCL_KNN_MAX_CAND)      // rows too long for the register-resident sort: scratch-line path
-    return launch_knn_large(eval_f, reinterpret_cast<const long long*>(eval_y), cand_f, reinterpret_cast<const long long*>(cand_y),
-                            E, C, d, k, sv, col_sum, col_max, col_min, workspace, workspace_bytes, stream);
+  if (C > B200OCL_KNN_MAX_CAND && d > knn_large_max_d()) {
+    set_error("b200ocl_knn_sv: d=%d exceeds %d on the large-candidate path", d, knn_large_max_d());
+    return B200OCL_EUNSUPPORTED;
+  }
   const bool want_red = col_sum || col_max || col_min;
+  const bool aligned = (reinterpret_cast<uintptr_t>(eval_f) & 15) == 0 && (reinterpret_cast<uintptr_t>(cand_f) & 15) == 0;
+  const b200ocl_knn_launch L = knn_plan(E, C, d, aligned, want_red, sm_count());
+  if (L.family == B200OCL_KNN_LARGE)
+    return launch_knn_large(eval_f, reinterpret_cast<const long long*>(eval_y), cand_f, reinterpret_cast<const long long*>(cand_y),
+                            E, C, d, k, sv, col_sum, col_max, col_min, workspace, workspace_bytes, L, stream);
   KnnSvParams p{};
   p.eval_f = eval_f;
   p.eval_y = reinterpret_cast<const long long*>(eval_y);
@@ -457,18 +498,37 @@ int b200ocl_knn_sv(const float* eval_f, const int64_t* eval_y, const float* cand
   p.E = E; p.C = C; p.d = d; p.k = k;
   p.sv = sv; p.col_sum = col_sum; p.col_max = col_max; p.col_min = col_min;
   if (want_red) {
-    const int rc = check_workspace("b200ocl_knn_sv", workspace, workspace_bytes, b200ocl_knn_sv_workspace_bytes(E, C, d));
+    const int rc = check_workspace("b200ocl_knn_sv", workspace, workspace_bytes, L.workspace_bytes);
     if (rc) return rc;
     p.counter = static_cast<unsigned int*>(workspace);
     p.part = reinterpret_cast<float*>(static_cast<unsigned char*>(workspace) + 256);
     B200OCL_CUDA(cudaMemsetAsync(p.counter, 0, sizeof(unsigned int), stream));
   }
-  if (C <= 32) return dispatch_te<1>(p, stream);
-  if (C <= 64) return dispatch_te<2>(p, stream);
-  if (C <= 128) return dispatch_te<4>(p, stream);
-  if (C <= 256) return dispatch_te<8>(p, stream);
-  if (C <= 512) return dispatch_te<16>(p, stream);
-  return dispatch_te<32>(p, stream);
+  switch (L.kpl) {
+    case 1: return dispatch_te<1>(p, L, stream);
+    case 2: return dispatch_te<2>(p, L, stream);
+    case 4: return dispatch_te<4>(p, L, stream);
+    case 8: return dispatch_te<8>(p, L, stream);
+    case 16: return dispatch_te<16>(p, L, stream);
+    default: return dispatch_te<32>(p, L, stream);
+  }
+}
+
+int b200ocl_knn_sv_plan(int E, int C, int d, int aligned, int want_red, int sms, b200ocl_knn_launch* out) {
+  using namespace b200ocl;
+  B200OCL_CHECK_ARG(out, "null pointer");
+  B200OCL_CHECK_ARG(E >= 1 && C >= 1 && d >= 1, "need E,C,d >= 1 (b200ocl_knn_sv launches nothing otherwise)");
+  B200OCL_CHECK_ARG(sms >= 0, "sms must be 0 (this device) or an SM count");
+  if (C > B200OCL_KNN_MAX_CAND_LARGE) {
+    set_error("b200ocl_knn_sv_plan: C=%d exceeds the limit of %d candidates", C, B200OCL_KNN_MAX_CAND_LARGE);
+    return B200OCL_EUNSUPPORTED;
+  }
+  if (C > B200OCL_KNN_MAX_CAND && d > knn_large_max_d()) {
+    set_error("b200ocl_knn_sv_plan: d=%d exceeds %d on the large-candidate path", d, knn_large_max_d());
+    return B200OCL_EUNSUPPORTED;
+  }
+  *out = knn_plan(E, C, d, aligned != 0, want_red != 0, sms ? sms : sm_count());
+  return B200OCL_OK;
 }
 
 }  // extern "C"

@@ -223,36 +223,51 @@ int knn_large_cpad(int C) {
   return cp;
 }
 
-size_t knn_large_workspace_bytes(int C) {
-  const size_t grid = (size_t)sm_count();
-  return 256 + align_up(grid * 3 * (size_t)C * sizeof(float), 256) + grid * (size_t)knn_large_cpad(C) * sizeof(unsigned long long);
+int knn_large_max_d() { return KL_MAX_D; }
+
+size_t knn_large_part_region(int C, int sms) { return align_up((size_t)sms * 3 * (size_t)C * sizeof(float), 256); }
+
+size_t knn_large_workspace_bytes(int C, int sms) {
+  return 256 + knn_large_part_region(C, sms) + (size_t)sms * (size_t)knn_large_cpad(C) * sizeof(unsigned long long);
+}
+
+// The scratch-line part of knn_plan (knn_sv.cu): E >= 1, d <= KL_MAX_D.
+void knn_large_plan(int E, int C, int d, bool want_red, int sms, b200ocl_knn_launch* L) {
+  L->family = B200OCL_KNN_LARGE;
+  L->cpad = knn_large_cpad(C);
+  const int S = L->cpad < KL_S ? L->cpad : KL_S;
+  L->block_keys = S;
+  int far = 0;                                                     // the kernel's far-partner loop, counted
+  for (int k2 = 2 * S; k2 <= L->cpad; k2 <<= 1)
+    for (int j = k2 >> 1; j >= S; j >>= 1) ++far;
+  L->far_stages = far;
+  L->grid = E < sms ? E : sms;
+  L->n_tiles = E;                                                  // one eval row per CTA iteration
+  L->tiles_per_cta = (E + L->grid - 1) / L->grid;
+  L->smem_bytes = (size_t)S * sizeof(unsigned long long) + (size_t)(d + KL_THREADS) * sizeof(float);
+  L->smem_limit = 200 * 1024;
+  L->part_bytes = want_red ? (size_t)L->grid * 3 * (size_t)C * sizeof(float) : 0;
+  L->key_offset = 256 + knn_large_part_region(C, sms);
+  L->key_bytes = (size_t)L->grid * L->cpad * sizeof(unsigned long long);
 }
 
 int launch_knn_large(const float* eval_f, const long long* eval_y, const float* cand_f, const long long* cand_y, int E, int C,
                      int d, int k, float* sv, float* col_sum, float* col_max, float* col_min, void* workspace,
-                     size_t workspace_bytes, cudaStream_t stream) {
-  if (d > KL_MAX_D) {
-    set_error("b200ocl_knn_sv: d=%d exceeds %d on the large-candidate path", d, KL_MAX_D);
-    return B200OCL_EUNSUPPORTED;
-  }
-  const int rc = check_workspace("b200ocl_knn_sv", workspace, workspace_bytes, knn_large_workspace_bytes(C));
+                     size_t workspace_bytes, const b200ocl_knn_launch& L, cudaStream_t stream) {
+  const int rc = check_workspace("b200ocl_knn_sv", workspace, workspace_bytes, L.workspace_bytes);
   if (rc) return rc;
   KnnLargeParams p{};
   p.eval_f = eval_f; p.eval_y = eval_y; p.cand_f = cand_f; p.cand_y = cand_y;
-  p.E = E; p.C = C; p.Cpad = knn_large_cpad(C); p.d = d; p.k = k;
+  p.E = E; p.C = C; p.Cpad = L.cpad; p.d = d; p.k = k;
   p.sv = sv; p.col_sum = col_sum; p.col_max = col_max; p.col_min = col_min;
-  const int grid_cap = sm_count();
   unsigned char* w = static_cast<unsigned char*>(workspace);
   p.counter = reinterpret_cast<unsigned int*>(w);
   p.part = reinterpret_cast<float*>(w + 256);
-  p.keys = reinterpret_cast<unsigned long long*>(w + 256 + align_up((size_t)grid_cap * 3 * (size_t)C * sizeof(float), 256));
+  p.keys = reinterpret_cast<unsigned long long*>(w + L.key_offset);
   B200OCL_CUDA(cudaMemsetAsync(p.counter, 0, sizeof(unsigned int), stream));
-  const int S = p.Cpad < KL_S ? p.Cpad : KL_S;
-  const size_t smem = (size_t)S * sizeof(unsigned long long) + (size_t)(d + KL_THREADS) * sizeof(float);
-  B200OCL_CUDA(raise_smem_limit<knn_sv_large_kernel>(200 * 1024));
-  const int grid = E < grid_cap ? E : grid_cap;
+  B200OCL_CUDA(raise_smem_limit<knn_sv_large_kernel>(L.smem_limit));
   B200OCL_PROF("knn_sv", 4.0 * d * ((double)E + C) + 8.0 * ((double)E + C) + 4.0 * C * 3 + (sv ? 4.0 * E * C : 0.0), stream);
-  knn_sv_large_kernel<<<grid, KL_THREADS, smem, stream>>>(p);
+  knn_sv_large_kernel<<<L.grid, KL_THREADS, L.smem_bytes, stream>>>(p);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }

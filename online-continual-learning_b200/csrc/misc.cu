@@ -398,7 +398,7 @@ int b200ocl_aser_replace(const int64_t* order, int n_total, int n_cand_buf, cons
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200OCL_CHECK_ARG(n_cur >= 0 && n_cand_buf >= 0 && n_total == n_cand_buf + n_cur, "need n_total == n_cand_buf + n_cur");
   if (n_cur == 0) return B200OCL_OK;
-  B200OCL_CHECK_ARG(order && cand_slot && cur_x && cur_y && buffer_img && buffer_label, "null pointer");
+  B200OCL_CHECK_ARG(order && (cand_slot || n_cand_buf == 0) && cur_x && cur_y && buffer_img && buffer_label, "null pointer");
   B200OCL_CHECK_ARG(row_bytes % 16 == 0 && ((reinterpret_cast<uintptr_t>(cur_x) | reinterpret_cast<uintptr_t>(buffer_img)) & 15) == 0,
                     "rows must be 16-byte aligned multiples of 16 bytes");
   B200OCL_PROF("move_rows", 2.0 * n_cur * (double)row_bytes, stream);

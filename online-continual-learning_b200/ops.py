@@ -78,6 +78,39 @@ def knn_sv(eval_f, eval_y, cand_f, cand_y, k, want_matrix=False, want_sum=True, 
     return out
 
 
+class KnnLaunch(ctypes.Structure):
+    """b200ocl_knn_launch: the kernel one b200ocl_knn_sv call runs."""
+    _fields_ = [('family', ctypes.c_int), ('kpl', ctypes.c_int), ('te', ctypes.c_int), ('wide', ctypes.c_int),
+                ('cpad', ctypes.c_int), ('block_keys', ctypes.c_int), ('far_stages', ctypes.c_int),
+                ('grid', ctypes.c_int), ('n_tiles', ctypes.c_int), ('tiles_per_cta', ctypes.c_int),
+                ('smem_bytes', ctypes.c_size_t), ('smem_limit', ctypes.c_size_t), ('part_bytes', ctypes.c_size_t),
+                ('key_offset', ctypes.c_size_t), ('key_bytes', ctypes.c_size_t), ('workspace_bytes', ctypes.c_size_t),
+                ('sms', ctypes.c_int)]
+
+    FAMILIES = ('fused', 'large')
+
+    @property
+    def name(self):
+        return self.FAMILIES[self.family]
+
+    @property
+    def kernel(self):
+        """(KPL, TE, 'wide' | 'rows') of a fused launch, ('large', block keys, far stages) of a scratch-line one."""
+        if self.name == 'large':
+            return ('large', self.block_keys, self.far_stages)
+        return (self.kpl, self.te, 'wide' if self.wide else 'rows')
+
+
+def knn_sv_plan(E, C, d, aligned=True, want_red=True, sms=0):
+    """Host-only test hook (b200ocl_knn_sv_plan): the launch knn_sv() makes for E eval rows, C candidates of width d on
+    a GPU with sms SMs (0: the current device); aligned: both feature pointers are 16-byte aligned; want_red: any of
+    the column reductions is asked for."""
+    out = KnnLaunch()
+    _native.check(_native.lib().b200ocl_knn_sv_plan(int(E), int(C), int(d), 1 if aligned else 0, 1 if want_red else 0,
+                                                    int(sms), ctypes.byref(out)), 'b200ocl_knn_sv_plan')
+    return out
+
+
 def rank_desc(a, n_out=None, sa=1.0, b=None, sb=0.0, return_scores=False):
     """Indices of the n_out largest entries of a*sa + b*sb, descending, ties lowest index
     first (sv.argsort(descending=True)[:n], aser_retrieve.py:88-91)."""

@@ -112,3 +112,123 @@ def order_mismatch_explained(sorted_a, sorted_b, dist64, rel_tol=4e-6):
         if np.any(np.abs(da[pos] - db[pos]) > rel_tol * scale[pos]):
             n_bad += 1
     return n_diff, n_bad
+
+
+# --------------------------------------------------------------------------- the kernel's own fp32 ordering
+# The kernels (csrc/knn_sv.cu, csrc/knn_sv_large.cu) rank candidates by their fp32 distances, ties lowest index first.
+# Where two fp64 distances are closer than fp32 rounding, the fp32 order is the kernel's own choice.  The functions
+# below reproduce those fp32 distances bit for bit with float64 torch ops, so that the stable sort of them *is* the
+# kernel's order and the fp64 recurrence on it differs from the kernel by rounding only.
+#   fused kernel  acc = 0; for f in 0..d-1: df = u_f - v_f (fp32); acc = fmaf(df, df, acc)      (both phase-1 forms)
+#   large kernel  lane l in 0..31: the same chain over f = l, l+32, ...; then warp_sum's xor butterfly,
+#                 v_l <- fl32(v_l + v_(l^o)) for o = 16, 8, 4, 2, 1, and lane 0's value
+# fmaf is emulated without contraction, one torch op per step: df^2 is exact in fp64 (a 24-bit significand squared);
+# TwoSum gives df^2 + acc = s + e exactly; fl32(s + e) is fl32(s), except when s is exactly halfway between two fp32
+# values, where the sign of e decides (e = 0: ties to even, which fl32(s) already did).
+
+def _round_fp32(s, e):
+    """fl32(s + e) for fp64 tensors s, e with |e| <= ulp64(s) / 2 (s + e exact, e.g. from TwoSum)."""
+    import torch
+    r = s.to(torch.float32)
+    r64 = r.to(torch.float64)
+    toward = torch.where(s > r64, torch.full_like(r, float('inf')), torch.full_like(r, float('-inf')))
+    other = torch.nextafter(r, toward)
+    other64 = other.to(torch.float64)
+    mid = (r64 + other64) * 0.5                       # exact: two neighbouring fp32 values
+    flip = (s == mid) & (e != 0) & ((e > 0) == (other64 > r64))
+    return torch.where(flip, other, r)
+
+
+def fmaf_sq(df, acc):
+    """fmaf(df, df, acc) for fp32 tensors, correctly rounded, from fp64 torch ops."""
+    import torch
+    p = df.to(torch.float64) * df.to(torch.float64)   # exact
+    a = acc.to(torch.float64)
+    s = p + a                                         # TwoSum(p, a): s + e == p + a exactly
+    bb = s - a
+    e = (a - (s - bb)) + (p - bb)
+    return _round_fp32(s, e)
+
+
+def dist_fp32_fused(ef, cf):
+    """[E,C] fp32 distances of the fused kernel: one sequential fmaf chain over the features.  fp32 torch tensors."""
+    import torch
+    acc = torch.zeros((ef.shape[0], cf.shape[0]), dtype=torch.float32, device=ef.device)
+    for f in range(ef.shape[1]):
+        acc = fmaf_sq(ef[:, f, None] - cf[None, :, f], acc)
+    return acc
+
+
+def dist_fp32_large(ef, cf, lanes=32):
+    """[E,C] fp32 distances of the scratch-line kernel: 32 lane-strided fmaf chains, then the xor butterfly."""
+    import torch
+    E, d = ef.shape
+    C = cf.shape[0]
+    steps = -(-d // lanes)
+    pad = steps * lanes - d                           # fmaf(0, 0, acc) == acc: idle lanes add nothing
+    ep = torch.nn.functional.pad(ef, (0, pad))
+    cp = torch.nn.functional.pad(cf, (0, pad))
+    out = torch.empty((E, C), dtype=torch.float32, device=ef.device)
+    idx = torch.arange(lanes, device=ef.device)
+    for r in range(E):
+        acc = torch.zeros((C, lanes), dtype=torch.float32, device=ef.device)
+        for t in range(steps):
+            sl = slice(t * lanes, (t + 1) * lanes)
+            acc = fmaf_sq(ep[r, None, sl] - cp[:, sl], acc)
+        for o in (16, 8, 4, 2, 1):
+            acc = acc + acc[:, idx ^ o]
+        out[r] = acc[:, 0]
+    return out
+
+
+def kernel_order(ef, cf, large=None):
+    """The kernels' per-row candidate order [E,C] (int64) and fp32 distances: the stable sort of the emulated fp32
+    distances.  large: the scratch-line kernel's distances (default: when C > 1024, as b200ocl_knn_sv picks)."""
+    import torch
+    if large is None:
+        large = cf.shape[0] > 1024
+    dist = dist_fp32_large(ef, cf) if large else dist_fp32_fused(ef, cf)
+    return torch.sort(dist, dim=1, stable=True).indices, dist
+
+
+def knn_sv_torch(order, eval_y, cand_y, k, block=64):
+    """fp64 SV matrix [E,C] in candidate order from an explicit per-row order [E,C] (torch, any device), in blocks of
+    rows so that C = 262 144 fits.  Also returns each row's sum of |terms| of the recurrence (the scale its fp32
+    rounding is relative to)."""
+    import torch
+    E, C = order.shape
+    dev = order.device
+    factor = torch.from_numpy(sv_factor(C, k)).to(dev)
+    sv = torch.empty((E, C), dtype=torch.float64, device=dev)
+    abs_sum = torch.empty(E, dtype=torch.float64, device=dev)
+    for s in range(0, E, block):
+        o = order[s:s + block]
+        match = (cand_y[o] == eval_y[s:s + block, None]).to(torch.float64)
+        nxt = torch.zeros_like(match)
+        nxt[:, :C - 1] = match[:, 1:]
+        term = (match - nxt) * factor
+        sv[s:s + block].scatter_(1, o, term.flip(1).cumsum(1).flip(1))
+        abs_sum[s:s + block] = term.abs().sum(1)
+    return sv, abs_sum
+
+
+EPS32 = 2.0 ** -24
+
+
+def gamma(n):
+    return n * EPS32 / (1 - n * EPS32)
+
+
+def kernel_add_depth(plan):
+    """Additions an exact term passes through before it reaches an SV entry (see tests/test_gpu_knn_sv_fp64.py):
+    fused: KPL in-lane + 5 shuffle levels + 1 (the lanes above); large: the per-thread run L = Cpad / 1024 twice, the
+    5-level block scan, its exclusive subtraction, the 31-block carry chain and the carry's addition."""
+    if plan.name == 'large':
+        return 2 * (plan.cpad // 1024) + 5 + 1 + 31 + 1
+    return plan.kpl + 6
+
+
+def sv_row_bound(abs_sum, plan, C):
+    """Per-row bound on |SV_kernel - SV_fp64| on the kernel's own order: gamma_(n+2) * sum |terms| (n additions and
+    the two roundings of the factor, fl32(rank * k) and the division) plus the fp64 oracle's own cumsum rounding."""
+    return (gamma(kernel_add_depth(plan) + 2) + C * 2.0 ** -52) * abs_sum
