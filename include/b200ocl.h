@@ -429,10 +429,14 @@ int b200ocl_ewc_consolidate(const b200ocl_net_desc* desc, const b200ocl_net_stat
                             void* workspace, size_t workspace_bytes, void* stream);
 
 /* Mean cross-entropy (agents/base.py:95,113) over logits [N,C], labels [N]:
- * loss[1]; per_sample [N] (F.cross_entropy(reduction='none'), mir_retrieve.py:26-27);
- * dlogits [N,C] = d(mean CE)/dlogits; n_correct[1] = #(argmax == label).  Each output nullable. */
+ * loss[1]; per_sample [N] (F.cross_entropy(reduction='none'), mir_retrieve.py:26-27), formed as
+ * (max - logit[label]) + log sum exp(logits - max) so that a small loss at large logits keeps its relative precision;
+ * dlogits [N,C] = d(mean CE)/dlogits; n_correct[1] = #(argmax == label) (ties lowest index).  Each output nullable.
+ * A label outside [0,C) sets *err_flag = 1 (nullable, never cleared): its row's dlogits are 0, its per_sample is NaN,
+ * and it adds nothing to loss (which still divides by N) or n_correct.  One CTA, fixed-order sums, no atomics:
+ * repeated launches are bit-identical. */
 int b200ocl_ce_loss(const float* logits, const int64_t* labels, int N, int C, float* loss, float* per_sample,
-                    float* dlogits, int64_t* n_correct, void* stream);
+                    float* dlogits, int64_t* n_correct, int* err_flag, void* stream);
 
 /* The training-trick criteria of agents/base.py:93-107 with the distillation term of utils/kd_manager.py:6-28 mixed in
  * (exp_replay.py:41-47, agem.py:40-46, lwf.py:38-40), over logits [N,C], labels [N], in one launch:

@@ -60,7 +60,7 @@ SIGNATURES = {
     'b200ocl_net_adam_step_ewc': (c_int, [P, P, P, P, P, c_int, c_float, c_int, c_float, c_float, P, P, c_size_t, P]),
     'b200ocl_ewc_consolidate_workspace_bytes': (c_size_t, [P]),
     'b200ocl_ewc_consolidate': (c_int, [P, P, P, P, c_size_t, P]),
-    'b200ocl_ce_loss': (c_int, [P, P, c_int, c_int, P, P, P, P, P]),
+    'b200ocl_ce_loss': (c_int, [P, P, c_int, c_int, P, P, P, P, P, P]),
     'b200ocl_cls_loss': (c_int, [P, P, c_int, c_int, c_int, P, c_int, c_int, P, c_int, P, c_float, c_float, P, P, P, P,
                                  P]),
     'b200ocl_icarl_loss': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, P, P, P, P]),

@@ -699,11 +699,14 @@ __global__ void __launch_bounds__(256) l2norm_fwd_kernel(const float* __restrict
 
 // ----------------------------------------------------------------------------- cross-entropy
 // Warp-wide maximum (ties to the lowest index) and log-sum-exp of the K values get(0..K-1) of one row.  Lanes take
-// strided elements and reduce through shuffles, so the summation order is the same on every call.
+// strided elements and reduce through shuffles, so the summation order is the same on every call.  lz = log z with
+// z = sum exp(v - mx) is kept apart from lse = mx + lz: a loss (mx - v_y) + lz does not round lse first, which would
+// cost up to ulp(mx) / 2 absolute (3.8e-6 at mx = 100) on a loss that can be 1e-3 or smaller.
 struct RowLse {
   float mx;
   int arg;
   float lse;
+  float lz;
 };
 
 template <class Get>
@@ -723,12 +726,14 @@ __device__ __forceinline__ RowLse row_lse(Get get, int K, int lane) {
   float z = 0.f;
   for (int c = lane; c < K; c += 32) z += expf(get(c) - mx);
   z = warp_sum(z);
-  return RowLse{mx, arg, mx + logf(z)};
+  const float lz = logf(z);
+  return RowLse{mx, arg, mx + lz, lz};
 }
 
 __global__ void __launch_bounds__(256) ce_kernel(const float* __restrict__ logits, const long long* __restrict__ labels,
                                                  int N, int C, float* __restrict__ loss, float* __restrict__ per_sample,
-                                                 float* __restrict__ dlogits, long long* __restrict__ n_correct) {
+                                                 float* __restrict__ dlogits, long long* __restrict__ n_correct,
+                                                 int* __restrict__ err) {
   __shared__ float s_loss[8];
   __shared__ int s_corr[8];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -736,11 +741,20 @@ __global__ void __launch_bounds__(256) ce_kernel(const float* __restrict__ logit
   int corr = 0;
   for (int n = warp; n < N; n += 8) {   // fixed assignment of rows to warps: deterministic sum
     const float* lr = logits + (size_t)n * C;
+    const long long y = labels[n];
+    if (y < 0 || y >= C) {              // the reference raises (target out of bounds); the row adds nothing
+      if (lane == 0) {
+        if (err) *err = 1;
+        if (per_sample) per_sample[n] = NAN;
+      }
+      if (dlogits)
+        for (int c = lane; c < C; c += 32) dlogits[(size_t)n * C + c] = 0.f;
+      continue;
+    }
     const RowLse r = row_lse([=](int c) { return __ldg(lr + c); }, C, lane);
     const float lse = r.lse;
     const int arg = r.arg;
-    const long long y = labels[n];
-    const float l = lse - lr[y];
+    const float l = (r.mx - lr[y]) + r.lz;
     if (per_sample && lane == 0) per_sample[n] = l;
     if (dlogits) {
       const float invN = 1.f / (float)N;
@@ -824,15 +838,17 @@ __global__ void __launch_bounds__(256) cls_loss_kernel(ClsLossArgs a) {
     }
     const RowLse all = row_lse([=](int c) { return __ldg(lr + c); }, C, lane);     // arg-max over every column (meters)
     const int arg = all.arg;
-    float lse = all.lse, tgt = lr[y];
+    RowLse crit = all;                   // the softmax the criterion takes
+    float tgt = lr[y];
     if (a.mode == B200OCL_CLS_LABELS) {
-      lse = row_lse([=](int c) { return s_on[c] ? __ldg(lr + c) : -INFINITY; }, C, lane).lse;
+      crit = row_lse([=](int c) { return s_on[c] ? __ldg(lr + c) : -INFINITY; }, C, lane);
     } else if (a.mode == B200OCL_CLS_SEPARATED) {
       const long long* cs = a.cols + s0;
-      lse = row_lse([=](int k) { return __ldg(lr + __ldg(cs + k)); }, s1 - s0, lane).lse;
+      crit = row_lse([=](int k) { return __ldg(lr + __ldg(cs + k)); }, s1 - s0, lane);
       tgt = lr[a.cols[p]];
     }
-    ce_sum += lse - tgt;
+    const float lse = crit.lse;
+    ce_sum += (crit.mx - tgt) + crit.lz;
     corr += (arg == (int)y) ? 1 : 0;
     float lse_s = 0.f, lse_t = 0.f;
     if (tr) {                            // T^2 * sum_c -softmax(t/T)_c * log_softmax(s/T)_c
@@ -1677,13 +1693,13 @@ int b200ocl_net_apply_running_stats(const b200ocl_net_desc* desc, const b200ocl_
 }
 
 int b200ocl_ce_loss(const float* logits, const int64_t* labels, int N, int C, float* loss, float* per_sample,
-                    float* dlogits, int64_t* n_correct, void* stream_) {
+                    float* dlogits, int64_t* n_correct, int* err_flag, void* stream_) {
   using namespace b200ocl;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200OCL_CHECK_ARG(logits && labels && N >= 1 && C >= 1, "need logits, labels, N >= 1, C >= 1");
   B200OCL_PROF("ce_loss", 8.0 * N * C, stream);
   ce_kernel<<<1, 256, 0, stream>>>(logits, reinterpret_cast<const long long*>(labels), N, C, loss, per_sample, dlogits,
-                                   reinterpret_cast<long long*>(n_correct));
+                                   reinterpret_cast<long long*>(n_correct), err_flag);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }
@@ -1707,6 +1723,7 @@ int b200ocl_cls_loss(const float* logits, const int64_t* labels, int N, int C, i
                 reinterpret_cast<const long long*>(pos_table), table_len, teacher, w_ce, w_kd, loss, dlogits,
                 reinterpret_cast<long long*>(n_correct), err_flag};
   const size_t smem = mode == B200OCL_CLS_LABELS ? (size_t)C * sizeof(int) : 0;
+  B200OCL_CUDA(raise_smem_limit<cls_loss_kernel>(smem));   // the presence map passes 48 KB near B200OCL_CLS_MAX_C
   B200OCL_PROF("cls_loss", (teacher ? 12.0 : 8.0) * N * C, stream);
   cls_loss_kernel<<<1, 256, smem, stream>>>(a);
   B200OCL_LAUNCHED();

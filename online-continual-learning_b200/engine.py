@@ -515,9 +515,19 @@ class Engine:
         return ewc.penalty if want_penalty else None
 
 
-def ce_loss(logits, labels, want_grad=True, want_per_sample=False, want_correct=False):
-    """Mean cross-entropy; returns dict(loss[1], dlogits, per_sample, n_correct[1])."""
-    _need_cuda(logits, labels)
+def _check_labels(logits, labels):
+    """One label per row: the kernels read labels[0..N-1] and nothing else tells them the length."""
+    if labels.dim() != 1 or labels.shape[0] != logits.shape[0]:
+        raise ValueError('labels must be 1-D with one entry per logits row: got %s for logits %s'
+                         % (tuple(labels.shape), tuple(logits.shape)))
+
+
+def ce_loss(logits, labels, want_grad=True, want_per_sample=False, want_correct=False, err=None):
+    """Mean cross-entropy (b200ocl_ce_loss) of logits [N,C] at labels [N]; returns dict(loss[1], dlogits,
+    per_sample, n_correct[1]).  err: int32 device flag [1] set to 1 by a label outside [0,C); such a row has zero
+    dlogits and a NaN per_sample and adds nothing to loss (still divided by N) or n_correct."""
+    _need_cuda(logits, labels, err)
+    _check_labels(logits, labels)
     logits = logits.detach().to(torch.float32).contiguous()
     labels = labels.detach().to(torch.int64).contiguous()
     n, c = logits.shape
@@ -528,7 +538,7 @@ def ce_loss(logits, labels, want_grad=True, want_per_sample=False, want_correct=
     out['n_correct'] = torch.empty(1, dtype=torch.int64, device=dev) if want_correct else None
     ptr = lambda t: 0 if t is None else t.data_ptr()
     rc = _lib().b200ocl_ce_loss(logits.data_ptr(), labels.data_ptr(), n, c, out['loss'].data_ptr(),
-                                ptr(out['per_sample']), ptr(out['dlogits']), ptr(out['n_correct']), _stream())
+                                ptr(out['per_sample']), ptr(out['dlogits']), ptr(out['n_correct']), ptr(err), _stream())
     _native.check(rc, 'b200ocl_ce_loss')
     return out
 
@@ -543,6 +553,7 @@ def cls_loss(logits, labels, mode='ce', cols=None, n_old=0, pos_table=None, teac
     device tensor), the boundary n_old and pos_table (label -> position, -1 unmapped).  teacher: teacher logits or None
     (no distillation term).  err: int32 device flag [1] set to 1 by an unmapped label."""
     _need_cuda(logits, labels, cols, pos_table, teacher, err)
+    _check_labels(logits, labels)
     logits = logits.detach().to(torch.float32).contiguous()
     labels = labels.detach().to(torch.int64).contiguous()
     n, c = logits.shape

@@ -364,10 +364,11 @@ class ContinualLearner(torch.nn.Module):
 
     def criterion(self, logits, labels, teacher_logits=None, w_ce=1.0, w_kd=0.0, want_grad=True, want_correct=False):
         """self.criterion(logits, labels) on the device, times w_ce, plus w_kd times the distillation loss against
-        teacher_logits when given: dict(loss[1], dlogits, n_correct[1]).  Plain CE goes through b200ocl_ce_loss as
-        before; the tricks and the distillation mixing through b200ocl_cls_loss."""
+        teacher_logits when given: dict(loss[1], dlogits, n_correct[1]).  Plain CE goes through b200ocl_ce_loss; the
+        tricks and the distillation mixing through b200ocl_cls_loss.  Both raise the same device flag on a label they
+        cannot map, read once per task by _raise_label_errors."""
         if self._mode == 'ce' and teacher_logits is None and w_ce == 1.0:
-            return ce_loss(logits, labels, want_grad=want_grad, want_correct=want_correct)
+            return ce_loss(logits, labels, want_grad=want_grad, want_correct=want_correct, err=self._err_flag())
         cols, n_old, pos = self._sep if self._mode == 'separated_softmax' else (None, 0, None)
         return cls_loss(logits, labels, self._mode, cols=cols, n_old=n_old, pos_table=pos, teacher=teacher_logits,
                         w_ce=w_ce, w_kd=w_kd, err=self._err_flag(), want_grad=want_grad, want_correct=want_correct)

@@ -27,6 +27,18 @@ def test_library_exports_every_declared_symbol():
     assert lib.b200ocl_version() >= 100
 
 
+def test_ctypes_signatures_take_the_declared_number_of_arguments():
+    """A parameter added to a declaration but not to its ctypes signature shifts every argument after it."""
+    from b200ocl import _native
+    text = re.sub(r'/\*.*?\*/', '', open(os.path.join(ROOT, 'include', 'b200ocl.h')).read(), flags=re.S)
+    decls = dict(re.findall(r'\b(b200ocl_[a-z0-9_]+)\s*\(([^()]*)\)\s*;', text))
+    assert set(decls) == set(_native.SIGNATURES)
+    for name, params in decls.items():
+        params = params.strip()
+        n = 0 if params in ('', 'void') else params.count(',') + 1
+        assert len(_native.SIGNATURES[name][1]) == n, name
+
+
 def test_workspace_queries_are_pure_host_calls():
     from b200ocl import _native
     lib = _native.lib()
