@@ -108,6 +108,24 @@ def separated_softmax_table(old_labels, new_labels, lbl_inv_map):
     return cols, len(old_labels), pos
 
 
+def ncm_class_ids(old_labels):
+    """The classes nearest-class-mean evaluation keeps one mean for: the distinct labels of old_labels in
+    first-occurrence order, the keys of the reference's cls_exemplar dict (agents/base.py:124).  Under new-instance
+    streams old_labels repeats every label once per task; the reference's repeated means are identical and its arg-min
+    takes the first, so classifying against the distinct labels predicts what it predicts.  Without repeats this is
+    old_labels itself."""
+    return list(dict.fromkeys(int(c) for c in old_labels))
+
+
+def ncm_fill_empty(means, counts):
+    """agents/base.py:135-138: each class without exemplars (counts 0) gets one unit-norm direction drawn by
+    torch.normal from the default CPU generator, in class order."""
+    for k in (counts == 0).nonzero().flatten().tolist():
+        mu = torch.normal(0, 1, size=(1, means.size(1))).to(means.device).squeeze()
+        means[k] = mu / mu.norm()
+    return means
+
+
 def kd_mix(task_seen, kd_trick=False, kd_trick_star=False, lwf=False):
     """(w_ce, w_kd): the loss is w_ce * criterion + w_kd * distillation.  kd_trick: a = 1/(task_seen+1),
     a * loss + (1-a) * kd; kd_trick_star: the same with 1/sqrt(task_seen+1), applied after kd_trick when both are set
@@ -444,16 +462,13 @@ class ContinualLearner(torch.nn.Module):
         ncm = self._ncm()
         if ncm:
             n = self.buffer.current_index
-            class_ids = torch.tensor(self.old_labels, dtype=torch.int64, device=self.device)
+            class_ids = torch.tensor(ncm_class_ids(self.old_labels), dtype=torch.int64, device=self.device)
             feats = torch.cat([eng.features_eval(self.buffer.buffer_img[s:s + 500]) for s in range(0, n, 500)]) \
                 if n else torch.zeros((0, eng.dim_in), device=self.device)
             if n and not bool(torch.isin(self.buffer.buffer_label[:n], class_ids).all()):
                 raise KeyError('a buffered label was never seen in training (the reference raises here, base.py:126)')
             means, counts = ops.ncm_class_means(feats, self.buffer.buffer_label[:n], class_ids)
-            empty = (counts == 0).nonzero().flatten().tolist()
-            for k in empty:         # base.py:135-137: a random direction for a class without exemplars
-                mu = torch.normal(0, 1, size=(1, eng.dim_in)).to(self.device).squeeze()
-                means[k] = mu / mu.norm()
+            ncm_fill_empty(means, counts)
         else:
             if isinstance(self.model, EngineModel):
                 W, b = self.model.linear__weight, self.model.linear__bias
@@ -805,6 +820,11 @@ class Icarl(ContinualLearner):
     def train_learner(self, x_train, y_train):
         self._begin_call()
         self.before_train(x_train, y_train)
+        K = self._pos[2] if self._pos is not None else 0
+        if K > self.engine.out_dim:
+            # replay_step's refusal, raised before this call launches anything (new-instance streams reach it at
+            # their second task: every label recurs)
+            raise ValueError('iCaRL: %d label positions exceed the %d logits' % (K, self.engine.out_dim))
         self.engine.pack()
         self.model = self.model.train()
         self._updated[:] = False                                                     # icarl.py:35, once per call

@@ -127,9 +127,10 @@ def Reduced_ResNet18(nclasses, nf=20, bias=True, in_hw=32):
 
 
 def SupConResNet(dim_in=160, head='mlp', feat_dim=128, in_hw=None):
-    """models/resnet.py:140-157.  dim_in selects the dataset like the reference does
-    (160: 32x32 inputs, 640: 84x84 inputs; setup_elements.py:49-51).  The reference builds no SupConResNet for
-    128x128 inputs: SCR on CORe50 is refused by check_supcon."""
+    """models/resnet.py:140-157.  in_hw is the input size; without it dim_in selects the dataset like the reference
+    does (160: 32x32 inputs, 640: 84x84 inputs; setup_elements.py:49-51).  OpenLORIS's 50x50 inputs also give 160
+    features, so setup_architecture always passes in_hw.  The reference builds no SupConResNet for 128x128 inputs: SCR
+    on CORe50 is refused by check_supcon."""
     if in_hw is None:
         in_hw = {160: 32, 640: 84}[dim_in]
     return EngineModel(in_hw, 100, head=head, feat_dim=feat_dim)
@@ -160,8 +161,8 @@ def setup_architecture(params):
     if params.agent in ['SCR', 'SCP']:
         dim_in = 640 if params.data == 'mini_imagenet' else 160
         check_supcon(in_hw, params.head, dim_in)
-        return SupConResNet(dim_in, head=params.head)
-    if params.data in ('cifar100', 'cifar10', 'mini_imagenet', 'core50'):
+        return SupConResNet(dim_in, head=params.head, in_hw=in_hw)
+    if params.data in ('cifar100', 'cifar10', 'mini_imagenet', 'core50', 'openloris'):
         return Reduced_ResNet18(nclass, in_hw=in_hw)
     raise NotImplementedError('dataset %s is outside the replay-path scope (SURVEY section 8)' % params.data)
 
@@ -181,7 +182,8 @@ def reference_init(data, num_classes, in_hw):
     generator by the torch.nn.init calls the layers' reset_parameters() make: kaiming_uniform_(a=sqrt(5)) for every
     convolution and linear weight, uniform_(+-1/sqrt(fan_in)) for the linear bias; BatchNorm weights 1 and biases 0
     take no draws.  For mini_imagenet and core50 the 160-input classifier Reduced_ResNet18 builds is drawn and then
-    replaced by a 640- / 2560-input one (setup_elements.py:59-66), so both are drawn and the first is discarded."""
+    replaced by a 640- / 2560-input one (setup_elements.py:59-66), so both are drawn and the first is discarded.
+    openloris keeps the 160-input classifier (setup_elements.py:67-68): its 50x50 inputs pool to 1x1 like 32x32 ones."""
     dim_in = reduced_resnet_dim_in(in_hw)
 
     def linear(fan_in):
