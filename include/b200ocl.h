@@ -152,6 +152,19 @@ int b200ocl_ncm_classify(const float* feats, int B, int d, const float* means, i
                          const int64_t* truth, int64_t* pred, uint64_t* n_correct, void* stream);
 int b200ocl_linear_argmax(const float* feats, int B, int d, const float* weight, const float* bias, int C,
                           const int64_t* truth, int64_t* pred, uint64_t* n_correct, void* stream);
+/* linear_argmax with the error analysis of base.py:144-226 (--error_analysis): the same pred and *n_correct, bit for
+ * bit, and per row b, with p the predicted class: pred_task[b] = class_task[p] (-1: unmapped); set_sums[2b+j] = the
+ * row's logits f.w_c + b_c summed in fp64, in class order, over the classes c with bit j of class_sets[c] (bit 0: the
+ * last task's labels, bit 1: the older labels without them); counts[0..2] += 1 when truth[b] != p and p has bit 0 /
+ * bit 1 / neither; counts[3] += 1 when class_task[p] == -1.  class_sets [C] uint8, class_task [C]; truth, class_sets,
+ * class_task, pred_task, set_sums and counts are required, pred and n_correct nullable.
+ * rows_mean: out[0] = mean of weight[rows] ([n, d] elements), out[1] = mean of bias[rows], each summed in fp64 and
+ * rounded to fp32 once; n == 0 gives NaN.  rows must lie in [0, C). */
+int b200ocl_linear_argmax_ea(const float* feats, int B, int d, const float* weight, const float* bias, int C,
+                             const int64_t* truth, const uint8_t* class_sets, const int64_t* class_task, int64_t* pred,
+                             uint64_t* n_correct, int64_t* pred_task, double* set_sums, uint64_t* counts, void* stream);
+int b200ocl_rows_mean(const float* weight, const float* bias, int C, int d, const int64_t* rows, int n, float* out,
+                      void* stream);
 
 /* The network's linear layer on its own: y [N,out] = x [N,in] . W[out,in]^T + b (relu != 0: then ReLU), the kernel the
  * classifier and projection heads run.  Each output sums its lane-strided products in a fixed order (no atomics).

@@ -29,6 +29,8 @@ SIGNATURES = {
     'b200ocl_ncm_class_means': (c_int, [P, P, c_int, c_int, P, c_int, P, P, P]),
     'b200ocl_ncm_classify': (c_int, [P, c_int, c_int, P, c_int, P, P, P, P, P]),
     'b200ocl_linear_argmax': (c_int, [P, c_int, c_int, P, P, c_int, P, P, P, P]),
+    'b200ocl_linear_argmax_ea': (c_int, [P, c_int, c_int, P, P, c_int, P, P, P, P, P, P, P, P, P]),
+    'b200ocl_rows_mean': (c_int, [P, P, c_int, c_int, P, c_int, P, P]),
     'b200ocl_linear_fwd': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, P]),
     'b200ocl_agem_project_workspace_bytes': (c_size_t, []),
     'b200ocl_agem_project': (c_int, [P, P, P, c_size_t, P, P, c_size_t, P]),

@@ -10,6 +10,9 @@
 //   ncm_classify      one warp per test sample: normalise, squared distance to every class mean with the
 //                     reference's (f - mu)^2 form, first arg-min, label lookup, correct count (integer atomic)
 //   linear_argmax     the non-NCM branch (base.py:172-175): arg-max of the classifier logits
+//   linear_argmax_ea  the same launch with the error analysis of base.py:144-226 (--error_analysis) riding along:
+//                     predicted task, per-row fp64 logit sums over the new / old class sets, wrong rows bucketed by
+//                     the set they were predicted into; rows_mean the classifier's weight / bias means over a row set
 #include <float.h>
 
 #include "common.cuh"
@@ -84,13 +87,24 @@ __global__ void __launch_bounds__(256) ncm_class_means_kernel(const float* __res
   }
 }
 
+// Side outputs of the error-analysis arg-max (EA): every pointer is set when EA is.
+struct EaArgs {
+  const unsigned char* sets;    // [C] bit 0: class of the last task (new_labels_zombie); bit 1: set(old_labels) - zombie
+  const long long* task_of;     // [C] class_task_map, -1 where a class has no entry
+  long long* pred_task;         // [B] task of the predicted class
+  double* set_sums;             // [B,2] the row's logits summed over the bit-0 / bit-1 classes, in class order, in fp64
+  unsigned long long* counts;   // [4] wrong rows predicted into a bit-0 / bit-1 / neither class; rows predicted unmapped
+};
+
 // NCM: score = squared distance, smaller wins.  LINEAR: score = -(f.w + b), so that one arg-min serves both.
-template <bool NCM>
+// EA (LINEAR only) adds the error-analysis outputs; the arg-max and the hit count run the same instructions either way.
+template <bool NCM, bool EA = false>
 __global__ void __launch_bounds__(256) classify_kernel(const float* __restrict__ feats, int B, int d,
                                                        const float* __restrict__ means, const float* __restrict__ bias, int K,
                                                        const long long* __restrict__ class_ids,
                                                        const long long* __restrict__ truth, long long* __restrict__ pred,
-                                                       unsigned long long* __restrict__ n_correct) {
+                                                       unsigned long long* __restrict__ n_correct, EaArgs ea = EaArgs()) {
+  static_assert(!(NCM && EA), "the error analysis reads logits: linear branch only");
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (b >= B) return;
@@ -103,6 +117,7 @@ __global__ void __launch_bounds__(256) classify_kernel(const float* __restrict__
   }
   float best = FLT_MAX;
   int best_k = 0;
+  double sum_new = 0.0, sum_old = 0.0;
   for (int k = 0; k < K; ++k) {
     const float* mu = means + (size_t)k * d;
     float s = 0.f;
@@ -116,6 +131,11 @@ __global__ void __launch_bounds__(256) classify_kernel(const float* __restrict__
     }
     s = warp_sum(s);
     if (!NCM) s = -(s + bias[k]);
+    if (EA) {                                              // -s is the logit f.w + b exactly
+      const unsigned m = ea.sets[k];
+      if (m & 1u) sum_new += (double)(-s);
+      if (m & 2u) sum_old += (double)(-s);
+    }
     if (s < best) {                                        // strict: the first minimum wins
       best = s;
       best_k = k;
@@ -125,6 +145,44 @@ __global__ void __launch_bounds__(256) classify_kernel(const float* __restrict__
     const long long label = class_ids ? class_ids[best_k] : (long long)best_k;
     if (pred) pred[b] = label;
     if (truth && n_correct && truth[b] == label) atomicAdd(n_correct, 1ull);
+    if (EA) {
+      const long long t = ea.task_of[best_k];
+      ea.pred_task[b] = t;
+      ea.set_sums[2 * (size_t)b] = sum_new;
+      ea.set_sums[2 * (size_t)b + 1] = sum_old;
+      if (t < 0) atomicAdd(&ea.counts[3], 1ull);           // class_task_map[p] raises KeyError in the reference
+      if (truth[b] != label) {
+        const unsigned m = ea.sets[best_k];
+        atomicAdd(&ea.counts[(m & 1u) ? 0 : (m & 2u) ? 1 : 2], 1ull);
+      }
+    }
+  }
+}
+
+// One CTA: mean of weight[rows] (n x d elements) and of bias[rows], each summed in fp64 in a fixed order (thread-strided
+// partial sums, then a fixed tree) and rounded to fp32 once.  n == 0 gives NaN, as torch's mean of an empty tensor.
+__global__ void __launch_bounds__(256) rows_mean_kernel(const float* __restrict__ weight, const float* __restrict__ bias,
+                                                        int d, const long long* __restrict__ rows, int n,
+                                                        float* __restrict__ out) {
+  __shared__ double s_w[256], s_b[256];
+  const int tid = threadIdx.x;
+  const long long total = (long long)n * d;
+  double w = 0.0, bb = 0.0;
+  for (long long i = tid; i < total; i += 256) w += (double)weight[(size_t)rows[i / d] * d + i % d];
+  for (int i = tid; i < n; i += 256) bb += (double)bias[rows[i]];
+  s_w[tid] = w;
+  s_b[tid] = bb;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (tid < o) {
+      s_w[tid] += s_w[tid + o];
+      s_b[tid] += s_b[tid + o];
+    }
+    __syncthreads();
+  }
+  if (tid == 0) {
+    out[0] = (float)(s_w[0] / (double)total);
+    out[1] = (float)(s_b[0] / (double)n);
   }
 }
 
@@ -180,6 +238,42 @@ int b200ocl_linear_argmax(const float* feats, int B, int d, const float* weight,
                                                           reinterpret_cast<const long long*>(truth),
                                                           reinterpret_cast<long long*>(pred),
                                                           reinterpret_cast<unsigned long long*>(n_correct));
+  B200OCL_LAUNCHED();
+  return B200OCL_OK;
+}
+
+int b200ocl_linear_argmax_ea(const float* feats, int B, int d, const float* weight, const float* bias, int C,
+                             const int64_t* truth, const uint8_t* class_sets, const int64_t* class_task, int64_t* pred,
+                             uint64_t* n_correct, int64_t* pred_task, double* set_sums, uint64_t* counts, void* stream_) {
+  using namespace b200ocl;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200OCL_CHECK_ARG(B >= 0 && d >= 1 && C >= 1, "need B >= 0, d >= 1, C >= 1");
+  if (B == 0) return B200OCL_OK;
+  B200OCL_CHECK_ARG(feats && weight && bias && truth && class_sets && class_task && pred_task && set_sums && counts,
+                    "null pointer");
+  B200OCL_PROF("ncm", 4.0 * B * (double)d + 4.0 * C * (double)d, stream);
+  EaArgs ea;
+  ea.sets = class_sets;
+  ea.task_of = reinterpret_cast<const long long*>(class_task);
+  ea.pred_task = reinterpret_cast<long long*>(pred_task);
+  ea.set_sums = set_sums;
+  ea.counts = reinterpret_cast<unsigned long long*>(counts);
+  classify_kernel<false, true><<<(B + 7) / 8, 256, 0, stream>>>(feats, B, d, weight, bias, C, nullptr,
+                                                                reinterpret_cast<const long long*>(truth),
+                                                                reinterpret_cast<long long*>(pred),
+                                                                reinterpret_cast<unsigned long long*>(n_correct), ea);
+  B200OCL_LAUNCHED();
+  return B200OCL_OK;
+}
+
+int b200ocl_rows_mean(const float* weight, const float* bias, int C, int d, const int64_t* rows, int n, float* out,
+                      void* stream_) {
+  using namespace b200ocl;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200OCL_CHECK_ARG(C >= 1 && d >= 1 && n >= 0, "need C >= 1, d >= 1, n >= 0");
+  B200OCL_CHECK_ARG(weight && bias && out && (n == 0 || rows), "null pointer");
+  B200OCL_PROF("ncm", 4.0 * n * (double)d, stream);
+  rows_mean_kernel<<<1, 256, 0, stream>>>(weight, bias, d, reinterpret_cast<const long long*>(rows), n, out);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }

@@ -12,6 +12,8 @@ branch the reference computes and then discards two backward passes (exp_replay.
 their forwards are kept for the BN side effect, their backwards are skipped.
 """
 import collections
+import math
+import pickle
 
 import numpy as np
 import torch
@@ -108,6 +110,32 @@ def separated_softmax_table(old_labels, new_labels, lbl_inv_map):
     return cols, len(old_labels), pos
 
 
+def error_analysis_tables(old_labels, zombie, class_task_map, n_classes):
+    """The per-class tables of the error analysis (agents/base.py:186-205): sets, uint8 [n_classes], bit 0 for the
+    labels of new_labels_zombie (the last task's) and bit 1 for set(old_labels) - set(zombie); task, int64
+    [n_classes], class_task_map with -1 where a class has no entry (the reference raises KeyError on predicting it).
+    A label of either set outside the classifier's rows raises IndexError, as the reference's column indexing does."""
+    zombie = set(int(c) for c in zombie)
+    old = set(int(c) for c in old_labels) - zombie
+    bad = sorted(c for c in zombie | old if c < 0 or c >= n_classes)
+    if bad:
+        raise IndexError('labels %s lie outside the %d classifier rows' % (bad, n_classes))
+    sets = np.zeros(n_classes, dtype=np.uint8)
+    sets[sorted(zombie)] |= 1
+    sets[sorted(old)] |= 2
+    task = np.full(n_classes, -1, dtype=np.int64)
+    for c, t in class_task_map.items():
+        if 0 <= int(c) < n_classes:
+            task[int(c)] = int(t)
+    return sets, task
+
+
+class ErrorAnalysisUnsupported(NotImplementedError, UnboundLocalError):
+    """error_analysis on the nearest-class-mean branch (SCR, iCaRL, ncm_trick).  The reference reads logits there that
+    this branch never computes and dies with UnboundLocalError (agents/base.py:194,203); this is raised instead, before
+    anything launches, and is caught wherever either exception is."""
+
+
 def ncm_class_ids(old_labels):
     """The classes nearest-class-mean evaluation keeps one mean for: the distinct labels of old_labels in
     first-occurrence order, the keys of the reference's cls_exemplar dict (agents/base.py:124).  Under new-instance
@@ -167,6 +195,13 @@ class ContinualLearner(torch.nn.Module):
         self.task_seen = 0
         self.lbl_inv_map = {}
         self.class_task_map = {}
+        self.error_list = []       # the error analysis' history, one entry per evaluate (agents/base.py:33-39)
+        self.new_class_score = []
+        self.old_class_score = []
+        self.fc_norm_new = []
+        self.fc_norm_old = []
+        self.bias_norm_new = []
+        self.bias_norm_old = []
         trick = getattr(params, 'trick', None) or {}
         self._trick = {k: bool(trick.get(k)) for k in ('labels_trick', 'separated_softmax', 'kd_trick', 'kd_trick_star')}
         contrastive = params.agent in ('SCR', 'SCP')
@@ -452,14 +487,18 @@ class ContinualLearner(torch.nn.Module):
         ncm_trick, arg-max of the classifier otherwise.  Encoder features come from the engine's batched
         eval pass (the reference runs model.features once per buffered image, base.py:125-134); class
         means, nearest-mean / arg-max and the hit count are the kernels of csrc/ncm.cu; one device -> host
-        read per test loader.  error_analysis is not implemented."""
-        if getattr(self.params, 'error_analysis', False):
-            raise NotImplementedError('error_analysis is outside the replay-path scope')
+        read per test loader.  With params.error_analysis the arg-max runs as b200ocl_linear_argmax_ea and the
+        analysis of base.py:144-226 follows (_error_analysis); on the nearest-class-mean branch it is refused."""
+        ea = getattr(self.params, 'error_analysis', False)
+        ncm = self._ncm()
+        if ea and ncm:
+            raise ErrorAnalysisUnsupported('error_analysis reads classifier logits, which the nearest-class-mean '
+                                           'evaluation of %s does not compute (the reference fails with '
+                                           'UnboundLocalError there)' % self.params.agent)
         eng = self.engine
         eng.pack()                  # the caller may have written the Parameters since the last step
         self.model.eval()           # base.py:119 (the next train_learner switches back)
         acc_array = np.zeros(len(test_loaders))
-        ncm = self._ncm()
         if ncm:
             n = self.buffer.current_index
             class_ids = torch.tensor(ncm_class_ids(self.old_labels), dtype=torch.int64, device=self.device)
@@ -474,6 +513,12 @@ class ContinualLearner(torch.nn.Module):
                 W, b = self.model.linear__weight, self.model.linear__bias
             else:
                 W, b = self.model.linear.weight, self.model.linear.bias
+        if ea:
+            zombie = list(getattr(self, 'new_labels_zombie', []))
+            sets, task_of = error_analysis_tables(self.old_labels, zombie, self.class_task_map, W.shape[0])
+            sets_t, task_t = torch.from_numpy(sets).to(self.device), torch.from_numpy(task_of).to(self.device)
+            counts = torch.zeros((len(test_loaders), 4), dtype=torch.int64, device=self.device)
+            recs, batches = [], []
         for task, loader in enumerate(test_loaders):
             hits = torch.zeros(1, dtype=torch.int64, device=self.device)
             total = 0
@@ -482,12 +527,81 @@ class ContinualLearner(torch.nn.Module):
                 f = eng.features_eval(batch_x)
                 if ncm:
                     ops.ncm_classify(f, means, class_ids, truth=batch_y, n_correct=hits)
+                elif ea:
+                    pred_task, sums = ops.linear_argmax_ea(f, W, b, batch_y, sets_t, task_t, counts[task], n_correct=hits)
+                    recs += [pred_task, sums.view(torch.int64).reshape(-1)]
+                    batches.append((task, batch_y.numel()))
                 else:
                     ops.linear_argmax(f, W, b, truth=batch_y, n_correct=hits)
                 total += batch_y.numel()
             acc_array[task] = int(hits) / max(total, 1)
-        print(acc_array)
+        if ea:
+            # the weight / bias means of base.py:217-220 (NaN for an empty row set), then one read of everything
+            old = sorted(set(int(c) for c in self.old_labels) - set(int(c) for c in zombie))
+            wb = torch.cat((ops.rows_mean(W, b, zombie), ops.rows_mean(W, b, old))).view(torch.int64)
+            host = torch.cat([counts.reshape(-1), wb] + recs).cpu().numpy()
+            self._error_analysis(host, len(test_loaders), batches, int((sets & 1).astype(bool).sum()), int((sets & 2).astype(bool).sum()),
+                                 acc_array)
+        else:
+            print(acc_array)
         return acc_array
+
+    def _error_analysis(self, host, n_loaders, batches, n_new, n_old, acc_array):
+        """The host side of the error analysis (agents/base.py:182-226) from the one read of evaluate: per loader the
+        counts of b200ocl_linear_argmax_ea, the weight / bias means, then per batch the predicted tasks and the two
+        logit sums of every row.  A prediction without a task raises KeyError before anything is appended, printed
+        or written, as the reference's class_task_map lookup leaves it."""
+        counts = host[:4 * n_loaders].reshape(n_loaders, 4)
+        if counts[:, 3].any():
+            raise KeyError('a test sample was predicted as a class never trained on (class_task_map has no entry; the '
+                           'reference raises at agents/base.py:185)')
+        wb = host[4 * n_loaders:4 * n_loaders + 2].view(np.float32)
+        off = 4 * n_loaders + 2
+        no = nn = oo = on = 0
+        new_class_score, old_class_score = AverageMeter(), AverageMeter()
+        correct_lb, predict_lb = [], []
+        for task, n in batches:
+            pred_task = host[off:off + n]
+            sums = host[off + n:off + 3 * n].view(np.float64).reshape(n, 2)
+            off += 3 * n
+            correct_lb += [task] * n
+            predict_lb += pred_task.tolist()
+            if task < self.task_seen - 1:                                            # old test (:186-194)
+                old_class_score.update(_set_mean(sums[:, 1], n * n_old), n)
+            elif task == self.task_seen - 1:                                         # new test (:195-203)
+                new_class_score.update(_set_mean(sums[:, 0], n * n_new), n)
+        for task in range(n_loaders):
+            if task < self.task_seen - 1:                # wrong into the last task's classes: on; anywhere else: oo
+                on += int(counts[task, 0])
+                oo += int(counts[task, 1] + counts[task, 2])
+            elif task == self.task_seen - 1:             # wrong into the older classes: no; anywhere else: nn
+                no += int(counts[task, 1])
+                nn += int(counts[task, 0] + counts[task, 2])
+        print(acc_array)
+        self.error_list.append((no, nn, oo, on))                                     # :209-226
+        self.new_class_score.append(new_class_score.avg())
+        self.old_class_score.append(old_class_score.avg())
+        print("no ratio: {}\non ratio: {}".format(no / (no + nn + 0.1), on / (oo + on + 0.1)))
+        print(self.error_list)
+        print(self.new_class_score)
+        print(self.old_class_score)
+        self.fc_norm_new.append(float(wb[0]))
+        self.fc_norm_old.append(float(wb[2]))
+        self.bias_norm_new.append(float(wb[1]))
+        self.bias_norm_old.append(float(wb[3]))
+        print(self.fc_norm_old)
+        print(self.fc_norm_new)
+        print(self.bias_norm_old)
+        print(self.bias_norm_new)
+        with open('confusion', 'wb') as fp:
+            pickle.dump([correct_lb, predict_lb], fp)
+
+
+def _set_mean(row_sums, n):
+    """logits[:, S].mean().item() of one batch from the rows' fp64 sums over S: their correctly rounded total over the
+    number of elements, rounded to fp32 once (NaN when S is empty)."""
+    with np.errstate(invalid='ignore', divide='ignore'):
+        return float(np.float32(np.float64(math.fsum(row_sums.tolist())) / np.float64(n)))
 
 
 class ExperienceReplay(ContinualLearner):

@@ -272,6 +272,60 @@ def linear_argmax(feats, weight, bias, truth=None, n_correct=None):
     return pred
 
 
+def linear_argmax_ea(feats, weight, bias, truth, class_sets, class_task, counts, n_correct=None, pred=None):
+    """linear_argmax with the error analysis of agents/base.py:177-205 in the same launch (b200ocl_linear_argmax_ea):
+    the prediction written to pred and the hits added to n_correct are linear_argmax's, bit for bit.  class_sets
+    (uint8 [C]: bit 0 for the last task's labels, bit 1 for the older labels without them) and class_task (int64 [C],
+    -1 where unmapped) are the tables of learners.error_analysis_tables on the device; counts (int64 [4]) gains the
+    wrong rows predicted into a bit-0 / bit-1 / neither class and the rows predicted into an unmapped class.
+    Returns (pred_task [B] int64, set_sums [B,2] float64: each row's logits summed over the bit-0 / bit-1 classes)."""
+    _need_cuda(feats, weight, bias, truth, class_sets, class_task, counts, n_correct, pred)
+    feats, weight, bias = _f32(feats), _f32(weight), _f32(bias).reshape(-1)
+    B, d = feats.shape
+    C = weight.shape[0]
+    if weight.dim() != 2 or weight.shape[1] != d:
+        raise ValueError('weight [C,d] must have the features\' width d=%d' % d)
+    if bias.numel() != C:
+        raise ValueError('bias must hold one entry per weight row')
+    truth = _check_truth(truth, B)
+    if class_sets.dtype != torch.uint8 or class_sets.numel() != C or not class_sets.is_contiguous():
+        raise ValueError('class_sets must be a contiguous uint8 tensor with one entry per class')
+    if class_task.dtype != torch.int64 or class_task.numel() != C or not class_task.is_contiguous():
+        raise ValueError('class_task must be a contiguous int64 tensor with one entry per class')
+    if counts.dtype != torch.int64 or counts.numel() != 4 or not counts.is_contiguous():
+        raise ValueError('counts must be a contiguous int64 tensor of 4')
+    if pred is not None and (pred.dtype != torch.int64 or pred.numel() != B or not pred.is_contiguous()):
+        raise ValueError('pred must be a contiguous int64 tensor with one entry per row')
+    out = torch.empty(3 * B, dtype=torch.int64, device=feats.device)
+    pred_task, set_sums = out[:B], out[B:].view(torch.float64).view(B, 2)
+    rc = _native.lib().b200ocl_linear_argmax_ea(_ptr(feats), B, d, _ptr(weight), _ptr(bias), C, _ptr(truth),
+                                                _ptr(class_sets), _ptr(class_task), _ptr(pred), _ptr(n_correct),
+                                                _ptr(pred_task), _ptr(set_sums), _ptr(counts), _stream())
+    _native.check(rc, 'b200ocl_linear_argmax_ea')
+    return pred_task, set_sums
+
+
+def rows_mean(weight, bias, rows, out=None):
+    """(mean of weight[rows], mean of bias[rows]) as a float32 tensor [2] on the device, each summed in fp64 and
+    rounded once (b200ocl_rows_mean); an empty row list gives NaN.  rows: a sequence of ints in [0, C)."""
+    _need_cuda(weight, bias, out)
+    weight, bias = _f32(weight), _f32(bias).reshape(-1)
+    C, d = weight.shape
+    if bias.numel() != C:
+        raise ValueError('bias must hold one entry per weight row')
+    rows = [int(r) for r in rows]
+    if any(r < 0 or r >= C for r in rows):
+        raise IndexError('rows %s lie outside the %d classifier rows' % (sorted(r for r in rows if r < 0 or r >= C), C))
+    if out is None:
+        out = torch.empty(2, dtype=torch.float32, device=weight.device)
+    elif out.dtype != torch.float32 or out.numel() != 2 or not out.is_contiguous():
+        raise ValueError('out must be a contiguous float32 tensor of 2')
+    idx = torch.tensor(rows, dtype=torch.int64).to(weight.device) if rows else None
+    rc = _native.lib().b200ocl_rows_mean(_ptr(weight), _ptr(bias), C, d, _ptr(idx), len(rows), _ptr(out), _stream())
+    _native.check(rc, 'b200ocl_rows_mean')
+    return out
+
+
 def linear_fwd(x, weight, bias, relu=False):
     """x @ weight.T + bias (then ReLU when relu) with the network heads' kernel: y [N, out] for x [N, in], in <= 4096."""
     _need_cuda(x, weight, bias)
