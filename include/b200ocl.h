@@ -191,6 +191,14 @@ int b200ocl_grad_cosine(const float* mem_grads, const float* g, int K, size_t n,
  * reference's CPU ToTensor).  perm may be NULL (identity).  h*w*3 % 4 == 0. */
 int b200ocl_stream_prepare(const uint8_t* src_hwc, const int64_t* perm, int n, int h, int w, float* dst_chw, void* stream);
 
+/* Stream feeder for the non-stationary tasks (continuum/non_stationary.py:9-124 hand the agents float64 HWC images in
+ * [0,1]; continuum/data_utils.py:38-54 applies ToTensor, a transpose only for float input, then .float()): dst[i] =
+ * image src[perm[i]] converted float64 HWC -> fp32 CHW, rounded to nearest even as the CPU's conversion does
+ * (subnormals kept, overflow to inf, NaN kept with its sign and payload).  perm may be NULL (identity).  src 8-byte
+ * aligned; offsets are 64-bit. */
+int b200ocl_stream_prepare_f64(const double* src_hwc, const int64_t* perm, int n, int h, int w, float* dst_chw,
+                               void* stream);
+
 /* ASER memory replacement on the device (reference utils/buffer/aser_update.py:88-112: current samples ranked
  * inside the first n_cand_buf places of the descending SV ranking replace, pairwise in rank order, the buffered
  * candidates ranked below).  order[n_total] ranks positions of [buffered candidates | current batch];

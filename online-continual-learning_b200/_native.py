@@ -26,6 +26,7 @@ SIGNATURES = {
     'b200ocl_gather_rows': (c_int, [P, P, c_int, c_size_t, P, P]),
     'b200ocl_scatter_rows': (c_int, [P, P, c_int, c_size_t, P, P]),
     'b200ocl_stream_prepare': (c_int, [P, P, c_int, c_int, c_int, P, P]),
+    'b200ocl_stream_prepare_f64': (c_int, [P, P, c_int, c_int, c_int, P, P]),
     'b200ocl_ncm_class_means': (c_int, [P, P, c_int, c_int, P, c_int, P, P, P]),
     'b200ocl_ncm_classify': (c_int, [P, c_int, c_int, P, c_int, P, P, P, P, P]),
     'b200ocl_linear_argmax': (c_int, [P, c_int, c_int, P, P, c_int, P, P, P, P]),

@@ -183,6 +183,66 @@ __global__ void __launch_bounds__(256) stream_prepare_kernel(const unsigned char
   }
 }
 
+// float64 -> fp32 as the host CPU's conversion does it (torch's .float(), x86 cvtsd2ss): IEEE round to nearest even with
+// subnormal results kept (no .ftz), overflow to inf, and a NaN kept with its sign and the top 22 bits of its payload,
+// quiet bit set.  cvt.rn.f32.f64 alone would return the canonical NaN.
+__device__ __forceinline__ float f64_to_f32_host(double v) {
+  if (v != v) {
+    const unsigned long long b = (unsigned long long)__double_as_longlong(v);
+    return __uint_as_float(((unsigned)(b >> 32) & 0x80000000u) | 0x7fc00000u | ((unsigned)(b >> 29) & 0x3fffffu));
+  }
+  return __double2float_rn(v);
+}
+
+// Stream feeder for the reference's non-stationary tasks (continuum/non_stationary.py:9-124 give float64 HWC images in
+// [0,1]; ToTensor on them only transposes, then .float(), continuum/data_utils.py:38-54): image i of the output = source
+// image perm[i], float64 HWC -> fp32 CHW.  One CTA per chunk of PREP64_PIX consecutive pixels of one image (any
+// number of rows, or part of one): its 3 * PREP64_PIX source doubles are contiguous and read once with 16-byte loads,
+// converted and staged as fp32 (12 KB, not a whole image), then written as three contiguous plane segments.
+constexpr int PREP64_THREADS = 256;
+constexpr int PREP64_PIX = 1024;
+constexpr int PREP64_LOADS = 3 * PREP64_PIX / 2 / PREP64_THREADS;   // double2 loads per thread
+
+__global__ void __launch_bounds__(PREP64_THREADS) stream_prepare_f64_kernel(const double* __restrict__ src,
+                                                                            const long long* __restrict__ perm,
+                                                                            float* __restrict__ dst, long long hw,
+                                                                            int chunks) {
+  __shared__ float s_val[3 * PREP64_PIX];
+  const long long img = blockIdx.x / chunks;
+  const long long p0 = (long long)(blockIdx.x - img * chunks) * PREP64_PIX;
+  const int pix = (int)min((long long)PREP64_PIX, hw - p0);
+  const int cnt = 3 * pix;
+  const double* in = src + ((perm ? perm[img] : img) * hw + p0) * 3;
+  // a chunk starts 16-byte aligned or one double past it: the odd leading and trailing doubles load alone
+  const int lead = (int)((reinterpret_cast<uintptr_t>(in) >> 3) & 1);
+  const int pairs = (cnt - lead) >> 1;
+  const double2* in2 = reinterpret_cast<const double2*>(in + lead);
+  double2 v[PREP64_LOADS];
+#pragma unroll
+  for (int j = 0; j < PREP64_LOADS; ++j) {
+    const int k = threadIdx.x + j * PREP64_THREADS;
+    if (k < pairs) v[j] = __ldg(in2 + k);
+  }
+#pragma unroll
+  for (int j = 0; j < PREP64_LOADS; ++j) {
+    const int k = threadIdx.x + j * PREP64_THREADS;
+    if (k < pairs) {
+      s_val[lead + 2 * k] = f64_to_f32_host(v[j].x);
+      s_val[lead + 2 * k + 1] = f64_to_f32_host(v[j].y);
+    }
+  }
+  if (threadIdx.x == 0) {
+    if (lead) s_val[0] = f64_to_f32_host(__ldg(in));
+    if ((cnt - lead) & 1) s_val[cnt - 1] = f64_to_f32_host(__ldg(in + cnt - 1));
+  }
+  __syncthreads();
+  float* out = dst + img * 3 * hw + p0;
+  for (int o = threadIdx.x; o < cnt; o += PREP64_THREADS) {
+    const int c = o / pix, p = o - c * pix;
+    out[c * hw + p] = s_val[p * 3 + c];
+  }
+}
+
 // A-GEM projection (agents/agem.py:60-80): g <- g - (g.g_ref / g_ref.g_ref) g_ref when g.g_ref < 0, else g.
 // Launch 1: per-CTA fp64 partials of the two dot products over the flat gradient arenas; launch 2: every thread
 // re-reduces the (<= 296) partials in CTA order -- same value everywhere, deterministic -- and writes the result.
@@ -340,6 +400,24 @@ int b200ocl_stream_prepare(const uint8_t* src_hwc, const int64_t* perm, int n, i
   B200OCL_CUDA(raise_smem_limit<stream_prepare_kernel>(200 * 1024));
   B200OCL_PROF("stream_prepare", 5.0 * n * (double)row, stream);
   stream_prepare_kernel<<<n, 256, row, stream>>>(src_hwc, reinterpret_cast<const long long*>(perm), dst_chw, h * w);
+  B200OCL_LAUNCHED();
+  return B200OCL_OK;
+}
+
+int b200ocl_stream_prepare_f64(const double* src_hwc, const int64_t* perm, int n, int h, int w, float* dst_chw,
+                               void* stream_) {
+  using namespace b200ocl;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200OCL_CHECK_ARG(n >= 0 && h > 0 && w > 0, "need n >= 0 and positive h, w");
+  if (n == 0) return B200OCL_OK;
+  B200OCL_CHECK_ARG(src_hwc && dst_chw, "null pointer");
+  B200OCL_CHECK_ARG((reinterpret_cast<uintptr_t>(src_hwc) & 7) == 0, "source must be 8-byte aligned");
+  const long long hw = (long long)h * w;
+  const long long chunks = (hw + PREP64_PIX - 1) / PREP64_PIX;
+  B200OCL_CHECK_ARG(chunks * n <= 0x7fffffffLL, "more than 2^31 - 1 pixel chunks");
+  B200OCL_PROF("stream_prepare_f64", 12.0 * n * 3.0 * (double)hw, stream);
+  stream_prepare_f64_kernel<<<(unsigned)(chunks * n), PREP64_THREADS, 0, stream>>>(
+      src_hwc, reinterpret_cast<const long long*>(perm), dst_chw, hw, (int)chunks);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }

@@ -62,10 +62,24 @@ class AverageMeter(object):
 class StreamFeeder(object):
     """One task's stream: uint8 NHWC images -> fp32 NCHW in [0,1] on the device (ToTensor,
     continuum/data_utils.py:38-54), shuffled, batches of `batch`, last partial batch dropped
-    (exp_replay.py:21-23).  The whole task is converted once; batches are views."""
+    (exp_replay.py:21-23).  The whole task is converted once; batches are views.
+
+    The non-stationary tasks (--cl_type ni --ns_type noise|occlusion|blur, continuum/non_stationary.py:9-124) arrive as
+    float64 NHWC [n,H,W,3] in [0,1] (H = W), on which ToTensor only transposes and .float() rounds to fp32.  Float NCHW
+    [n,3,H,W] is taken as it is; any other float layout raises ValueError before anything is drawn or uploaded."""
 
     def __init__(self, x_train, y_train, batch, device):
         self.batch = batch
+        x = np.asarray(x_train)
+        if x.dtype == np.uint8:
+            kind = 'u8'
+        elif x.dtype.kind == 'f' and x.ndim == 4 and x.shape[1] == 3:
+            kind = 'nchw'
+        elif x.dtype == np.float64 and x.ndim == 4 and x.shape[3] == 3 and x.shape[1] == x.shape[2]:
+            kind = 'f64'
+        else:
+            raise ValueError('stream images must be uint8 [n,H,W,3], float64 [n,H,H,3] in [0,1] (non-stationary tasks) '
+                             'or float [n,3,H,W]; got %s %s' % (x.dtype, tuple(x.shape)))
         y = np.asarray(y_train).astype(np.int64)
         if memory.parity():
             # the reference's DataLoader(shuffle=True, drop_last=True) itself, over slot numbers: consumes the
@@ -76,12 +90,14 @@ class StreamFeeder(object):
             perm = torch.cat(order).numpy() if order else np.zeros(0, dtype=np.int64)
         else:
             perm = torch.randperm(len(y)).numpy()        # DataLoader(shuffle=True) draws from the torch CPU generator
-        x = torch.from_numpy(np.ascontiguousarray(np.asarray(x_train)))
-        if x.dtype == torch.uint8 and torch.device(device).type == 'cuda':
-            # one upload of the raw bytes, then shuffle + HWC->CHW + /255 in one kernel (csrc/misc.cu)
+        x = torch.from_numpy(np.ascontiguousarray(x))
+        if kind in ('u8', 'f64') and torch.device(device).type == 'cuda':
+            # one upload of the raw values, then shuffle + HWC->CHW (+ /255 for uint8) in one kernel (csrc/misc.cu)
             x = ops.stream_prepare(x.to(device), torch.from_numpy(perm).to(device))
-        elif x.dtype == torch.uint8:
+        elif kind == 'u8':
             x = x[torch.from_numpy(perm)].permute(0, 3, 1, 2).to(torch.float32).div_(255.0).contiguous()
+        elif kind == 'f64':
+            x = x[torch.from_numpy(perm)].permute(0, 3, 1, 2).to(torch.float32).contiguous()
         else:                                             # already float NCHW
             x = x[torch.from_numpy(perm)].to(device=device, dtype=torch.float32).contiguous()
         self.x = x

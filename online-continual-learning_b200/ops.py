@@ -200,17 +200,20 @@ def gather_rows(src, idx, out=None):
 
 
 def stream_prepare(x_u8_nhwc, perm=None):
-    """uint8 [n,H,W,3] (device) -> fp32 [n,3,H,W] in [0,1], rows taken in `perm` order (ToTensor + shuffle)."""
+    """uint8 [n,H,W,3] (device) -> fp32 [n,3,H,W] in [0,1], rows taken in `perm` order (ToTensor + shuffle).
+    float64 [n,H,W,3] in [0,1] (the non-stationary tasks) -> fp32 [n,3,H,W] rounded to nearest even, bit-identical to
+    the CPU's x.permute(0,3,1,2).float()."""
     _need_cuda(x_u8_nhwc, perm)
-    if x_u8_nhwc.dtype != torch.uint8 or x_u8_nhwc.dim() != 4 or x_u8_nhwc.shape[3] != 3:
-        raise ValueError('expected uint8 images [n,H,W,3]')
+    if x_u8_nhwc.dtype not in (torch.uint8, torch.float64) or x_u8_nhwc.dim() != 4 or x_u8_nhwc.shape[3] != 3:
+        raise ValueError('expected uint8 or float64 images [n,H,W,3]')
     x = x_u8_nhwc.contiguous()
     n, h, w = (perm.numel() if perm is not None else x.shape[0]), x.shape[1], x.shape[2]
     out = torch.empty((n, 3, h, w), dtype=torch.float32, device=x.device)
     if perm is not None:
         perm = _i64(perm).reshape(-1)
-    rc = _native.lib().b200ocl_stream_prepare(_ptr(x), _ptr(perm), n, h, w, _ptr(out), _stream())
-    _native.check(rc, 'b200ocl_stream_prepare')
+    name = 'b200ocl_stream_prepare' if x.dtype == torch.uint8 else 'b200ocl_stream_prepare_f64'
+    rc = getattr(_native.lib(), name)(_ptr(x), _ptr(perm), n, h, w, _ptr(out), _stream())
+    _native.check(rc, name)
     return out
 
 
