@@ -170,6 +170,26 @@ def ncm_fill_empty(means, counts):
     return means
 
 
+def _drain(steps):
+    for _ in steps:
+        pass
+
+
+def _after_train_steps(self):
+    """ContinualLearner.after_train (agents/base.py:56-91) as a generator: yields after every step of the review trick's
+    pass.  A function rather than a method, so that after_train also serves objects that only borrow it."""
+    self.old_labels += self.new_labels
+    self.new_labels_zombie = list(self.new_labels)
+    self.new_labels.clear()
+    self.task_seen += 1
+    self._task_tables()
+    if (getattr(self.params, 'trick', None) or {}).get('review_trick') and hasattr(self, 'buffer'):
+        yield from self._review_steps()
+    if self._takes_teacher:                                                     # base.py:90-91, after the review
+        self.engine.update_teacher()
+        self._teacher_live = True
+
+
 def kd_mix(task_seen, kd_trick=False, kd_trick_star=False, lwf=False):
     """(w_ce, w_kd): the loss is w_ce * criterion + w_kd * distillation.  kd_trick: a = 1/(task_seen+1),
     a * loss + (1-a) * kd; kd_trick_star: the same with 1/sqrt(task_seen+1), applied after kd_trick when both are set
@@ -397,16 +417,7 @@ class ContinualLearner(torch.nn.Module):
         self._task_tables()
 
     def after_train(self):
-        self.old_labels += self.new_labels
-        self.new_labels_zombie = list(self.new_labels)
-        self.new_labels.clear()
-        self.task_seen += 1
-        self._task_tables()
-        if (getattr(self.params, 'trick', None) or {}).get('review_trick') and hasattr(self, 'buffer'):
-            self._review()
-        if self._takes_teacher:                                                     # base.py:90-91, after the review
-            self.engine.update_teacher()
-            self._teacher_live = True
+        _drain(_after_train_steps(self))
 
     # ------------------------------------------------------------------ criterion (agents/base.py:93-113)
     def _task_tables(self):
@@ -451,6 +462,9 @@ class ContinualLearner(torch.nn.Module):
                               want_correct=want_correct)
 
     def _review(self):
+        _drain(self._review_steps())
+
+    def _review_steps(self):
         """Review trick (agents/base.py:62-88, the published SCR setting config_CVPR/agent/scr/scr_5k.yml:10): one
         pass over the filled memory in shuffled batches of eps_mem_batch (drop_last), gradients divided by 10.
         g/10 followed by SGD(lr, wd) is p -= lr*(g/10 + wd*p) = SGD(lr/10, 10*wd) on g: folded into the step."""
@@ -486,8 +500,15 @@ class ContinualLearner(torch.nn.Module):
                 eng.backward(bx, ce['dlogits'], ws)
             self._optimizer_step(spec, review=True)                                  # base.py:83-88
             self._throttle()
+            yield
 
     def train_learner(self, x_train, y_train):
+        _drain(self._steps(x_train, y_train))
+
+    def _steps(self, x_train, y_train):
+        """train_learner as a generator that yields after every replay step (and every step of the review trick), so
+        that a driver can interleave the steps of several learners (multirun.run_group).  Draining it is
+        train_learner: the same launches in the same order."""
         raise NotImplementedError
 
     def forward(self, x):
@@ -691,7 +712,7 @@ class ExperienceReplay(ContinualLearner):
         self.buffer.update(batch_x, batch_y, y_host=batch_y_host)                   # :92
         self._throttle()
 
-    def train_learner(self, x_train, y_train):
+    def _steps(self, x_train, y_train):
         self._begin_call()
         self.before_train(x_train, y_train)
         self.engine.pack()          # the caller may have written the Parameters (load_state_dict, weight surgery)
@@ -701,13 +722,14 @@ class ExperienceReplay(ContinualLearner):
             stream = StreamFeeder(x_train, y_train, self.batch, self.device)   # DataLoader(shuffle=True): new order per epoch
             for i, (batch_x, batch_y, y_host) in enumerate(stream):
                 self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
+                yield
                 if i % 100 == 1 and self.verbose:
                     print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
                           .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
                     print('==>>> it: {}, mem avg. loss: {:.6f}, running mem acc: {:.3f}'
                           .format(i, meters['losses_mem'].avg(), meters['acc_mem'].avg()))
         self._raise_label_errors()
-        self.after_train()
+        yield from _after_train_steps(self)
         self._end_call()
 
 
@@ -764,7 +786,7 @@ class SupContrastReplay(ContinualLearner):
         self.buffer.update(batch_x, batch_y, y_host=batch_y_host)                   # :63
         self._throttle()
 
-    def train_learner(self, x_train, y_train):
+    def _steps(self, x_train, y_train):
         self._begin_call()
         self.before_train(x_train, y_train)
         self.engine.pack()          # the caller may have written the Parameters (load_state_dict, weight surgery)
@@ -774,9 +796,10 @@ class SupContrastReplay(ContinualLearner):
             stream = StreamFeeder(x_train, y_train, self.batch, self.device)   # DataLoader(shuffle=True): new order per epoch
             for i, (batch_x, batch_y, y_host) in enumerate(stream):
                 self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
+                yield
                 if i % 100 == 1 and self.verbose:
                     print('==>>> it: {}, avg. loss: {:.6f}, '.format(i, meters['losses'].avg()))
-        self.after_train()
+        yield from _after_train_steps(self)
         self._end_call()
 
 
@@ -817,7 +840,7 @@ class AGEM(ContinualLearner):
         self.buffer.update(batch_x, batch_y, y_host=batch_y_host)                    # :83
         self._throttle()
 
-    def train_learner(self, x_train, y_train):
+    def _steps(self, x_train, y_train):
         self._begin_call()
         self.before_train(x_train, y_train)
         self.engine.pack()
@@ -827,11 +850,12 @@ class AGEM(ContinualLearner):
             stream = StreamFeeder(x_train, y_train, self.batch, self.device)
             for i, (batch_x, batch_y, y_host) in enumerate(stream):
                 self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
+                yield
                 if i % 100 == 1 and self.verbose:
                     print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
                           .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
         self._raise_label_errors()
-        self.after_train()
+        yield from _after_train_steps(self)
         self._end_call()
 
 
@@ -854,7 +878,7 @@ class Lwf(ContinualLearner):
         self.last_loss = out['loss']
         self._throttle()
 
-    def train_learner(self, x_train, y_train):
+    def _steps(self, x_train, y_train):
         self._begin_call()
         self.before_train(x_train, y_train)
         self.engine.pack()
@@ -864,11 +888,12 @@ class Lwf(ContinualLearner):
             stream = StreamFeeder(x_train, y_train, self.batch, self.device)
             for i, (batch_x, batch_y, y_host) in enumerate(stream):
                 self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
+                yield
                 if i % 100 == 1 and self.verbose:
                     print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
                           .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
         self._raise_label_errors()
-        self.after_train()
+        yield from _after_train_steps(self)
         self._end_call()
 
 
@@ -947,7 +972,7 @@ class Icarl(ContinualLearner):
         self._updated[np.asarray(slots, dtype=np.int64)] = True
         self._throttle()
 
-    def train_learner(self, x_train, y_train):
+    def _steps(self, x_train, y_train):
         self._begin_call()
         self.before_train(x_train, y_train)
         K = self._pos[2] if self._pos is not None else 0
@@ -962,13 +987,14 @@ class Icarl(ContinualLearner):
             stream = StreamFeeder(x_train, y_train, self.batch, self.device)
             for batch_x, batch_y, y_host in stream:
                 self.replay_step(batch_x, batch_y, y_host)
+                yield
         if self._pos_err is not None and int(self._pos_err.item()):
             self._pos_err.zero_()
             raise ValueError("iCaRL trained on a label outside the task's labels (icarl.py:44 raises there)")
         self.engine.update_teacher()                                                 # icarl.py:31, before after_train
         self._prev_live = True
         self._raise_label_errors()
-        self.after_train()
+        yield from _after_train_steps(self)
         self._end_call()
 
 
@@ -999,6 +1025,10 @@ class Gdumb(ContinualLearner):
 
     def train_mem(self):
         """gdumb.py:52-83."""
+        _drain(self._train_mem_steps())
+
+    def _train_mem_steps(self):
+        """train_mem as a generator: yields after every memory batch."""
         if self.grad_sync is not None:
             raise NotImplementedError('data-parallel GDumb: the clipping would have to follow the gradient all-reduce')
         order = self.memory.order()
@@ -1025,16 +1055,17 @@ class Gdumb(ContinualLearner):
                 eng.sgd_step_clipped(lr, wd, clip)                                             # :82-83
                 self.last_loss = out['loss']
                 self._throttle()
+                yield
 
-    def train_learner(self, x_train, y_train):
+    def _steps(self, x_train, y_train):
         self.before_train(x_train, y_train)
         stream = StreamFeeder(x_train, y_train, self.batch, self.device)                       # :35-38 (drop_last)
         n = len(stream) * self.batch
         slots, sources = self.memory.plan(stream.y_host[:n])                                   # :40-47
         self.memory.write(stream.x, stream.y_host, slots, sources)
-        self.train_mem()                                                                       # :49
+        yield from self._train_mem_steps()                                                     # :49
         self._raise_label_errors()
-        self.after_train()                                                                     # :50
+        yield from _after_train_steps(self)                                                   # :50
 
 
 def ewc_ema_schedule(n_batches, epochs, fisher_update_after):
@@ -1117,7 +1148,7 @@ class EWC_pp(ContinualLearner):
             meters['losses_batch'].update(loss, batch_y.size(0))
         self._throttle()
 
-    def train_learner(self, x_train, y_train):
+    def _steps(self, x_train, y_train):
         self._begin_call()
         self.before_train(x_train, y_train)
         self.engine.pack()
@@ -1131,11 +1162,12 @@ class EWC_pp(ContinualLearner):
             for i, (batch_x, batch_y, y_host) in enumerate(stream):
                 self.replay_step(batch_x, batch_y, y_host, schedule[ep * len(stream) + i],
                                  meters if self.verbose else None)
+                yield
                 if i % 100 == 1 and self.verbose:
                     print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
                           .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
         self.engine.ewc_consolidate()                                                # :71-78
         self._penalty_live = True
         self._raise_label_errors()
-        self.after_train()                                                           # :79
+        yield from _after_train_steps(self)                                         # :79
         self._end_call()

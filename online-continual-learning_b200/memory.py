@@ -222,6 +222,32 @@ def flush_pending(owner=None):
     _pending.extend(keep)
 
 
+class RunHostState(object):
+    """The module-level host state of the replay path that belongs to one run when several runs share the process
+    (multirun.run_group): the class-level state of ClassBalancedRandomSampling, which the buffers of one run share as
+    the reference's do, and the queued host-mirror updates of that run's buffers.  enter() makes it current, leave()
+    takes it back; between the two nothing else may enter.  Swapping moves references only: no copy, no device wait
+    (queued updates stay queued until their own run flushes them)."""
+    __slots__ = ('sampler', 'pending')
+
+    def __init__(self):
+        self.sampler = None
+        self.pending = []
+
+    def enter(self):
+        if _pending:
+            raise RuntimeError('host-mirror updates of another run are still queued')
+        ClassBalancedRandomSampling.load_state(self.sampler)
+        _pending.extend(self.pending)
+        self.pending = []
+
+    def leave(self):
+        self.sampler = ClassBalancedRandomSampling.export_state()
+        self.pending = list(_pending)
+        del _pending[:]
+        ClassBalancedRandomSampling.load_state(None)
+
+
 def pinned_i64(n):
     for i, t in enumerate(_pinned_pool):
         if t.numel() >= n:
@@ -251,6 +277,19 @@ class ClassBalancedRandomSampling:
     _tab = None                  # int64 [num_class, cap]
     _cnt = None                  # int64 [num_class]
     _pos = None                  # int64 [mem]
+
+    _STATE = ('class_index_cache', 'class_num_cache', 'labels_host', 'n_valid', '_member', '_tab', '_cnt', '_pos')
+
+    @classmethod
+    def export_state(cls):
+        """The class-level state as a dict (references, no copies): load_state(export_state()) restores it."""
+        return {k: getattr(cls, k) for k in cls._STATE}
+
+    @classmethod
+    def load_state(cls, state):
+        """Replace the class-level state (None: the state of a sampler that was never filled)."""
+        for k in cls._STATE:
+            setattr(cls, k, 0 if k == 'n_valid' else None) if state is None else setattr(cls, k, state[k])
 
     @classmethod
     def reset(cls):

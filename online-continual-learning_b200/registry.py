@@ -11,6 +11,10 @@ The agents registered here are ER, SCR, AGEM, LWF, ICARL and GDUMB.  `extra_agen
 registered on request, `install(extra=('EWC',))` (or `B200OCL_EXTRA_AGENTS=EWC` with b200ocl.launch): EWC (EWC++).
 Every other agent / plugin of the reference (EWC unless requested, CNDPM, the match retrievals) stays registered and
 untouched.
+
+With B200OCL_CONCURRENT_RUNS=R (an integer > 1) install() also replaces experiment.run.multiple_run with
+multirun.multiple_run, which trains R repetitions of the experiment at once (general_main.py and main_config.py import it
+by name after install()).  Unset or 1 leaves it alone; any other value raises ValueError before anything is replaced.
 """
 from .learners import AGEM, EWC_pp, ExperienceReplay, Gdumb, Icarl, Lwf, SupContrastReplay
 from .retrieve import ASER_retrieve, MIR_retrieve, Random_retrieve
@@ -54,6 +58,9 @@ def install(reference_name_match=None, extra=()):
     if unknown:
         raise ValueError('unknown extra agent(s) %s; available: %s' % (', '.join(map(repr, unknown)),
                                                                       ', '.join(sorted(extra_agents))))
+    from . import multirun
+    n_concurrent = multirun.concurrent_runs()
+    multirun.check_concurrent(n_concurrent)
     if reference_name_match is None:
         reference_name_match = importlib.import_module('utils.name_match')
     nm = reference_name_match
@@ -78,6 +85,10 @@ def install(reference_name_match=None, extra=()):
             continue
         replaced[(mod_name, attr)] = getattr(mod, attr, None)
         setattr(mod, attr, obj)
+    if n_concurrent > 1:
+        run = importlib.import_module('experiment.run')
+        replaced[('experiment.run', 'multiple_run')] = run.multiple_run
+        run.multiple_run = multirun.multiple_run
     _installed.update(replaced)
     return replaced
 
