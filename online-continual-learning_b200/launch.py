@@ -3,7 +3,8 @@
     python -m b200ocl.launch /path/to/reference/general_main.py --agent ER --retrieve ASER --update ASER ...
 
 The reference tree is put first on sys.path, its registries are patched in place
-(b200ocl.registry.install) and general_main.py is executed with runpy, byte-identical.
+(b200ocl.registry.install) and general_main.py is executed with runpy, byte-identical.  Any entry point of the reference
+runs the same way, main_tune.py included.
 B200OCL_EXTRA_AGENTS (comma-separated, e.g. EWC) also registers those opt-in agents (registry.extra_agents)."""
 import os
 import runpy

@@ -14,7 +14,11 @@ untouched.
 
 With B200OCL_CONCURRENT_RUNS=R (an integer > 1) install() also replaces experiment.run.multiple_run with
 multirun.multiple_run, which trains R repetitions of the experiment at once (general_main.py and main_config.py import it
-by name after install()).  Unset or 1 leaves it alone; any other value raises ValueError before anything is replaced.
+by name after install()), and, when experiment.run defines it, experiment.run.multiple_run_tune_separate with
+multirun.multiple_run_tune_separate, which trains R of main_tune.py's tuning and final trainings at once (main_tune.py
+imports it by name after install()).  uninstall() puts both back; an attribute experiment.run lacked stays absent.  Unset
+or 1 leaves them alone; any other value, and every refusal of multirun.check_concurrent, raises ValueError before
+anything is replaced.
 """
 from .learners import AGEM, EWC_pp, ExperienceReplay, Gdumb, Icarl, Lwf, SupContrastReplay
 from .retrieve import ASER_retrieve, MIR_retrieve, Random_retrieve
@@ -89,6 +93,9 @@ def install(reference_name_match=None, extra=()):
         run = importlib.import_module('experiment.run')
         replaced[('experiment.run', 'multiple_run')] = run.multiple_run
         run.multiple_run = multirun.multiple_run
+        if hasattr(run, 'multiple_run_tune_separate'):     # a reference without main_tune.py's loop keeps none
+            replaced[('experiment.run', 'multiple_run_tune_separate')] = run.multiple_run_tune_separate
+            run.multiple_run_tune_separate = multirun.multiple_run_tune_separate
     _installed.update(replaced)
     return replaced
 
