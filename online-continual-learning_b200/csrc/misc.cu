@@ -1,4 +1,4 @@
-// misc.cu -- ranking, buffer row gather/scatter, flat SGD (sm_90a).
+// misc.cu -- ranking, buffer row gather/scatter (sm_90a).
 #include <float.h>
 
 #include "common.cuh"
@@ -148,19 +148,6 @@ __global__ void __launch_bounds__(256) aser_replace_kernel(const long long* __re
   for (size_t v = threadIdx.x; v < row_bytes / 16; v += blockDim.x) d[v] = s[v];
   if (threadIdx.x == 0) buffer_label[s_dst] = cur_y[s_src];
 }
-
-// ----------------------------------------------------------------------------- SGD
-__global__ void __launch_bounds__(256) sgd_kernel(const float* __restrict__ p, const float* __restrict__ g,
-                                                  float* __restrict__ out, size_t n, float lr, float wd) {
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const float w = p[i];
-    float gi = g[i];
-    if (wd != 0.f) gi = fmaf(wd, w, gi);
-    out[i] = w - lr * gi;
-  }
-}
-
 
 // Stream feeder (continuum/data_utils.py:38-54 + ToTensor): image i of the output = source image perm[i],
 // uint8 HWC -> fp32 CHW, value / 255 with an IEEE division (bit-identical to torchvision's CPU ToTensor).
@@ -487,20 +474,6 @@ int b200ocl_aser_replace(const int64_t* order, int n_total, int n_cand_buf, cons
                                                  static_cast<unsigned char*>(buffer_img),
                                                  reinterpret_cast<long long*>(buffer_label),
                                                  reinterpret_cast<long long*>(pairs_out));
-  B200OCL_LAUNCHED();
-  return B200OCL_OK;
-}
-
-int b200ocl_sgd_step(const float* p, const float* g, float* out, size_t n, float lr, float wd, void* stream_) {
-  using namespace b200ocl;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  B200OCL_CHECK_ARG(n == 0 || (p && g && out), "null pointer");
-  if (n == 0) return B200OCL_OK;
-  size_t blocks = (n + 255) / 256;
-  const size_t cap = (size_t)8 * sm_count();
-  if (blocks > cap) blocks = cap;
-  B200OCL_PROF("sgd", 12.0 * n, stream);
-  sgd_kernel<<<(unsigned)blocks, 256, 0, stream>>>(p, g, out, n, lr, wd);
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }

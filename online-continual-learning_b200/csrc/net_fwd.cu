@@ -1,9 +1,8 @@
-// net_fwd.cu -- Reduced-ResNet18 / SupConResNet forward passes, weight packing, SGD, CE loss.
+// net_fwd.cu -- Reduced-ResNet18 / SupConResNet forward passes, weight packing, CE loss.
 //
 // Replaces model.features / model.forward of reference models/resnet.py:90-109,159-168 in
 // eval mode (ASER deep features, utils/utils.py:45-90) and train mode (exp_replay.py:40,62,84;
-// scr.py:55; mir_retrieve.py:24-25), torch.optim.SGD.step (setup_elements.py:73-75) and
-// F.cross_entropy (agents/base.py:95,113; mir_retrieve.py:26-27).
+// scr.py:55; mir_retrieve.py:24-25) and F.cross_entropy (agents/base.py:95,113; mir_retrieve.py:26-27).
 #include <float.h>
 #include <math.h>
 
@@ -133,6 +132,8 @@ __global__ void __launch_bounds__(256) tp_pack_kernel(TpPackTable t, const float
   }
 }
 
+}  // namespace
+
 int launch_pack(const NetPlan& p, const float* params, float* packed, cudaStream_t stream) {
   PackTable t{};
   t.n = p.n_conv;
@@ -190,365 +191,7 @@ int launch_pack(const NetPlan& p, const float* params, float* packed, cudaStream
   return B200OCL_OK;
 }
 
-// ----------------------------------------------------------------------------- SGD over the arena
-// CLIP: the gradient is first scaled by the clipping coefficient *coef (grad_norm_kernel) and the scaled value is
-// written back to the gradient arena through g_out (== g).  Each element is read and then written by one thread only,
-// so the read-only load of g cannot see a stale value.
-template <bool CLIP>
-__global__ void __launch_bounds__(256) net_sgd_kernel(const float* __restrict__ p, const float* __restrict__ g,
-                                                      float* __restrict__ out, size_t n, float lr, float wd,
-                                                      size_t skip_lo, size_t skip_hi, const float* coef, float* g_out) {
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  float c = 1.f;
-  if (CLIP) c = *coef;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const float w = p[i];
-    if (i >= skip_lo && i < skip_hi) {  // tensors that never receive a gradient: torch skips them
-      out[i] = w;
-      continue;
-    }
-    float gi = g[i];
-    if (CLIP) {
-      gi = gi * c;                      // torch._foreach_mul_(grads, clip_coef_clamped)
-      g_out[i] = gi;
-    }
-    if (wd != 0.f) gi = fmaf(wd, w, gi);
-    out[i] = w - lr * gi;
-  }
-}
-
-// L2 norm of the gradient arena outside [skip_lo, skip_hi) and torch's clipping coefficient
-// (torch/nn/utils/clip_grad.py, _clip_grads_with_norm_): coef = min(max_norm / (norm + 1e-6), 1) in fp32, with torch's roundings.
-// Per-CTA fp64 partial sums of squares in a fixed order; the last CTA to arrive adds them in CTA order.
-constexpr int NORM_MAX_GRID = 1024;
-
-// Workspace of the arena reductions (grad_norm_kernel, the EWC++ kernels): one 8-byte partial per CTA (up to
-// NORM_MAX_GRID), then, at the next 256-byte boundary, the arrival counter followed by the reduction's fp32 results.
-constexpr size_t REDUCE_TAIL_OFF = (NORM_MAX_GRID * sizeof(double) + 255) / 256 * 256;
-constexpr size_t REDUCE_WS_BYTES = REDUCE_TAIL_OFF + 256;
-inline unsigned int* reduce_counter(void* ws) {
-  return reinterpret_cast<unsigned int*>(static_cast<unsigned char*>(ws) + REDUCE_TAIL_OFF);
-}
-inline float* reduce_scalars(void* ws) { return reinterpret_cast<float*>(reduce_counter(ws) + 1); }
-
-// The tensors that never receive a gradient (the SupCon network's unused classifier): every pass that steps the
-// arenas leaves [lo, hi) out.
-inline void sgd_skip_range(const NetPlan& p, size_t& lo, size_t& hi) {
-  lo = hi = 0;
-  if (p.head != 0) {
-    lo = p.lin[0].w_off;
-    hi = p.lin[0].b_off + p.lin[0].out;
-  }
-}
-
-// Grid of a grid-stride pass of 256-thread CTAs over the parameter arena: at most per_sm CTAs per SM and `cap`.
-inline unsigned arena_grid(const NetPlan& p, int per_sm, size_t cap) {
-  size_t blocks = (p.n_params + 255) / 256;
-  const size_t sm_cap = (size_t)per_sm * sm_count();
-  if (blocks > sm_cap) blocks = sm_cap;
-  return (unsigned)(blocks < cap ? blocks : cap);
-}
-
-__global__ void __launch_bounds__(256) grad_norm_kernel(const float* __restrict__ g, size_t n, size_t skip_lo,
-                                                        size_t skip_hi, float max_norm, double* __restrict__ part,
-                                                        unsigned int* counter, float* coef, float* norm_out) {
-  __shared__ double s_red[8];
-  __shared__ bool is_last;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  double acc = 0.0;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    if (i >= skip_lo && i < skip_hi) continue;
-    const double v = (double)g[i];
-    acc = fma(v, v, acc);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(FULL_MASK, acc, o);
-  if (lane == 0) s_red[warp] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) t += s_red[w];
-    part[blockIdx.x] = t;
-    __threadfence();
-    is_last = (atomicAdd(counter, 1u) == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (is_last && threadIdx.x == 0) {
-    __threadfence();
-    double t = 0.0;
-    for (unsigned int b = 0; b < gridDim.x; ++b) t += __ldcg(part + b);
-    const float norm = (float)sqrt(t);
-    // torch forms max_norm / (norm + 1e-6) as Tensor.__rdiv__: (norm + 1e-6).reciprocal() * max_norm, two roundings
-    const float q = __fmul_rn(__frcp_rn(norm + 1e-6f), max_norm);
-    *coef = q > 1.f ? 1.f : q;          // torch.clamp(max=1.0): a NaN norm stays NaN
-
-    if (norm_out) *norm_out = norm;
-  }
-}
-
-// ----------------------------------------------------------------------------- EWC++ step and consolidation
-// One pass per element in the order of agents/ewc_pp.py: the EMA of update_running_fisher (EMA), the penalty's gradient
-// added to the network's (PEN), accum_fisher's tmp += g*g, then the SGD update of net_sgd_kernel.  Every torch op is
-// its own rounding, so the products and sums are spelled with __f*_rn: nvcc would contract them to fma.  The SGD
-// update is written as net_sgd_kernel writes it, so that it compiles to the same instructions.  With PEN and pen_out,
-// sum F*d^2 over the pre-step weights goes to pen_out: per-CTA fp64 partials, added in CTA order by the last CTA.
-template <bool EMA, bool PEN>
-__global__ void __launch_bounds__(256) net_sgd_ewc_kernel(float* __restrict__ p, float* __restrict__ g,
-                                                          float* __restrict__ running, float* __restrict__ tmp,
-                                                          const float* __restrict__ fisher,
-                                                          const float* __restrict__ prev, size_t n, size_t skip_lo,
-                                                          size_t skip_hi, float lr, float wd, float up, float ema_keep,
-                                                          float ema_add, double* __restrict__ part,
-                                                          unsigned int* counter, float* pen_out) {
-  double acc = 0.0;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    if (i >= skip_lo && i < skip_hi) continue;   // tensors that never receive a gradient: untouched in every arena
-    const float w = p[i];
-    float gi = g[i];
-    float t = tmp[i];
-    if (EMA) {
-      // (1 - alpha) * running + (1/fua * alpha) * tmp, then tmp = 0 (ewc_pp.py:104-108)
-      running[i] = __fadd_rn(__fmul_rn(ema_keep, running[i]), __fmul_rn(ema_add, t));
-      t = 0.f;
-    }
-    if (PEN) {
-      // autograd of lambda * (F * (p - prev)**2).sum(): (up * F) * (2 * d), added once to the network's gradient
-      const float f = fisher[i];
-      const float d = __fsub_rn(w, prev[i]);
-      gi = __fadd_rn(gi, __fmul_rn(__fmul_rn(up, f), __fmul_rn(2.f, d)));
-      g[i] = gi;
-      const double dd = (double)d;
-      acc = fma((double)f * dd, dd, acc);
-    }
-    tmp[i] = __fadd_rn(t, __fmul_rn(gi, gi));   // accum_fisher: tmp += grad ** 2 (pow 2 is grad * grad)
-    if (wd != 0.f) gi = fmaf(wd, w, gi);
-    p[i] = w - lr * gi;
-  }
-  if (!PEN || !pen_out) return;
-  __shared__ double s_red[8];
-  __shared__ bool is_last;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(FULL_MASK, acc, o);
-  if (lane == 0) s_red[warp] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double s = 0.0;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) s += s_red[k];
-    part[blockIdx.x] = s;
-    __threadfence();
-    is_last = (atomicAdd(counter, 1u) == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (is_last && threadIdx.x == 0) {
-    __threadfence();
-    double s = 0.0;
-    for (unsigned int b = 0; b < gridDim.x; ++b) s += __ldcg(part + b);
-    *pen_out = (float)s;
-  }
-}
-
-// End of an EWC++ call, first half: prev = params, and the global min / max of running (per-CTA partials, combined by
-// the last CTA, which stores mn and the denominator (mx - mn) + 1e-32 with torch's fp32 roundings).
-__global__ void __launch_bounds__(256) ewc_minmax_kernel(const float* __restrict__ p, const float* __restrict__ running,
-                                                         float* __restrict__ prev, size_t n, size_t skip_lo,
-                                                         size_t skip_hi, float2* __restrict__ part,
-                                                         unsigned int* counter, float* range) {
-  __shared__ float s_mn[8], s_mx[8];
-  __shared__ bool is_last;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  float mn = INFINITY, mx = -INFINITY;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    if (i >= skip_lo && i < skip_hi) continue;
-    prev[i] = p[i];
-    const float v = running[i];
-    mn = fminf(mn, v);
-    mx = fmaxf(mx, v);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    mn = fminf(mn, __shfl_xor_sync(FULL_MASK, mn, o));
-    mx = fmaxf(mx, __shfl_xor_sync(FULL_MASK, mx, o));
-  }
-  if (lane == 0) {
-    s_mn[warp] = mn;
-    s_mx[warp] = mx;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int k = 1; k < 8; ++k) {
-      s_mn[0] = fminf(s_mn[0], s_mn[k]);
-      s_mx[0] = fmaxf(s_mx[0], s_mx[k]);
-    }
-    part[blockIdx.x] = make_float2(s_mn[0], s_mx[0]);
-    __threadfence();
-    is_last = (atomicAdd(counter, 1u) == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (is_last && threadIdx.x == 0) {
-    __threadfence();
-    float a = INFINITY, b = -INFINITY;
-    for (unsigned int k = 0; k < gridDim.x; ++k) {
-      const float2 v = __ldcg(part + k);
-      a = fminf(a, v.x);
-      b = fmaxf(b, v.y);
-    }
-    range[0] = a;
-    range[1] = __fadd_rn(__fsub_rn(b, a), 1e-32f);
-  }
-}
-
-// Second half: normalized = (running - mn) / ((mx - mn) + 1e-32), an IEEE division.
-__global__ void __launch_bounds__(256) ewc_normalize_kernel(const float* __restrict__ running,
-                                                            float* __restrict__ normalized, size_t n, size_t skip_lo,
-                                                            size_t skip_hi, const float* __restrict__ range) {
-  const float mn = range[0], den = range[1];
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    if (i >= skip_lo && i < skip_hi) continue;
-    normalized[i] = __fdiv_rn(__fsub_rn(running[i], mn), den);
-  }
-}
-
-// ----------------------------------------------------------------------------- Adam over the arena
-// torch.optim.Adam's update (amsgrad, maximize and decoupled weight decay off) as torch's CUDA kernels round it, one op
-// at a time, so that the step is bit-identical to the optimizer the caller built:
-//   g' = fma(wd, p, g)                   grad.add(param, alpha=wd), only when wd != 0 (a temporary: g is not written)
-//   m  = lerp(m, g', w1)                 exp_avg.lerp_(grad, 1 - beta1), ATen/native/Lerp.h as nvcc contracts it:
-//                                        fma(w1, g' - m, m) for |w1| < 0.5, else fma(-(g' - m), 1 - w1, g')
-//   v  = fma(c2, g' * g', v * b2)        exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value=1 - beta2)
-//                                        (DeviceAddCmulCdiv.cuh: fma(g', g', v * b2) when the value is 1)
-//   d  = sqrt(v) / bc2_sqrt + eps        FOREACH (torch's default on CUDA, _foreach_div_ by a scalar list): an IEEE
-//                                        division; otherwise CUDA Tensor / Python float, which multiplies by the fp32
-//                                        rounding of the double reciprocal: `bc2` holds that reciprocal
-//   p  = fma(step_size, m / d, p)        param.addcdiv_(exp_avg, denom, value=-(lr / bc1))
-// GDIV first replaces g by the review trick's p.grad.clone() / 10. (also Tensor / Python float: g * fp32(1 / 10.),
-// `gmul`) and writes it back, as p.grad.data.copy_ does.
-struct AdamCoef {
-  float wd, w1, w1c, b2, c2, bc2, eps, step, gmul;   // w1c = 1 - w1 in fp32, as Lerp.h forms it on the device
-};
-
-template <bool FOREACH>
-__device__ __forceinline__ void adam_update(float& w, float gi, float& m, float& v, const AdamCoef& c) {
-  if (c.wd != 0.f) gi = __fmaf_rn(c.wd, w, gi);
-  const float diff = __fsub_rn(gi, m);
-  m = fabsf(c.w1) < 0.5f ? __fmaf_rn(c.w1, diff, m) : __fmaf_rn(-diff, c.w1c, gi);
-  const float vb = __fmul_rn(v, c.b2);
-  v = c.c2 == 1.f ? __fmaf_rn(gi, gi, vb) : __fmaf_rn(c.c2, __fmul_rn(gi, gi), vb);
-  const float s = __fsqrt_rn(v);
-  const float d = __fadd_rn(FOREACH ? __fdiv_rn(s, c.bc2) : __fmul_rn(s, c.bc2), c.eps);
-  w = __fmaf_rn(c.step, __fdiv_rn(m, d), w);
-}
-
-template <bool FOREACH, bool GDIV>
-__global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
-                                                   float* __restrict__ v, size_t n, size_t skip_lo, size_t skip_hi,
-                                                   AdamCoef c) {
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    if (i >= skip_lo && i < skip_hi) continue;   // tensors without a gradient: torch creates no state, steps nothing
-    float gi = g[i];
-    if (GDIV) {
-      gi = __fmul_rn(gi, c.gmul);
-      g[i] = gi;
-    }
-    float w = p[i], mi = m[i], vi = v[i];
-    adam_update<FOREACH>(w, gi, mi, vi, c);
-    p[i] = w;
-    m[i] = mi;
-    v[i] = vi;
-  }
-}
-
-// EWC++ under Adam: the per-element pass of net_sgd_ewc_kernel (EMA, penalty gradient, tmp += g*g) followed by the
-// Adam update in place of the SGD one, in one launch (ewc_pp.py:58-63).
-template <bool EMA, bool PEN, bool FOREACH>
-__global__ void __launch_bounds__(256) net_adam_ewc_kernel(float* __restrict__ p, float* __restrict__ g,
-                                                           float* __restrict__ m, float* __restrict__ v,
-                                                           float* __restrict__ running, float* __restrict__ tmp,
-                                                           const float* __restrict__ fisher,
-                                                           const float* __restrict__ prev, size_t n, size_t skip_lo,
-                                                           size_t skip_hi, AdamCoef c, float up, float ema_keep,
-                                                           float ema_add, double* __restrict__ part,
-                                                           unsigned int* counter, float* pen_out) {
-  double acc = 0.0;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    if (i >= skip_lo && i < skip_hi) continue;
-    float w = p[i];
-    float gi = g[i];
-    float t = tmp[i];
-    if (EMA) {
-      running[i] = __fadd_rn(__fmul_rn(ema_keep, running[i]), __fmul_rn(ema_add, t));
-      t = 0.f;
-    }
-    if (PEN) {
-      const float f = fisher[i];
-      const float d = __fsub_rn(w, prev[i]);
-      gi = __fadd_rn(gi, __fmul_rn(__fmul_rn(up, f), __fmul_rn(2.f, d)));
-      g[i] = gi;
-      const double dd = (double)d;
-      acc = fma((double)f * dd, dd, acc);
-    }
-    tmp[i] = __fadd_rn(t, __fmul_rn(gi, gi));
-    float mi = m[i], vi = v[i];
-    adam_update<FOREACH>(w, gi, mi, vi, c);
-    p[i] = w;
-    m[i] = mi;
-    v[i] = vi;
-  }
-  if (!PEN || !pen_out) return;
-  __shared__ double s_red[8];
-  __shared__ bool is_last;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(FULL_MASK, acc, o);
-  if (lane == 0) s_red[warp] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double s = 0.0;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) s += s_red[k];
-    part[blockIdx.x] = s;
-    __threadfence();
-    is_last = (atomicAdd(counter, 1u) == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (is_last && threadIdx.x == 0) {
-    __threadfence();
-    double s = 0.0;
-    for (unsigned int b = 0; b < gridDim.x; ++b) s += __ldcg(part + b);
-    *pen_out = (float)s;
-  }
-}
-
-// The kernel's coefficients from the caller's scalars; false for unknown flags.
-inline bool adam_coef(const b200ocl_adam_scalars& s, int flags, AdamCoef& c) {
-  if (flags & ~(B200OCL_ADAM_FOREACH | B200OCL_ADAM_GRAD_SCALE)) return false;
-  c.wd = s.weight_decay;
-  c.w1 = s.beta1_c;
-  c.w1c = 1.f - s.beta1_c;
-  c.b2 = s.beta2;
-  c.c2 = s.beta2_c;
-  c.bc2 = (flags & B200OCL_ADAM_FOREACH) ? s.bc2_sqrt : s.bc2_sqrt_inv;
-  c.eps = s.eps;
-  c.step = s.step_size;
-  c.gmul = (flags & B200OCL_ADAM_GRAD_SCALE) ? s.grad_scale : 1.f;
-  return true;
-}
-
-template <bool FOREACH>
-void launch_adam(unsigned grid, cudaStream_t stream, float* p, float* g, float* m, float* v, size_t n, size_t skip_lo,
-                 size_t skip_hi, const AdamCoef& c, bool gdiv) {
-  if (gdiv) adam_kernel<FOREACH, true><<<grid, 256, 0, stream>>>(p, g, m, v, n, skip_lo, skip_hi, c);
-  else adam_kernel<FOREACH, false><<<grid, 256, 0, stream>>>(p, g, m, v, n, skip_lo, skip_hi, c);
-}
+namespace {
 
 // ----------------------------------------------------------------------------- train-mode BN apply
 struct BnApplyArgs {
@@ -1084,6 +727,8 @@ __global__ void bump_tracked_kernel(long long* t, int n) {
   if (i < n) t[i] += 1;
 }
 
+}  // namespace
+
 int check_state(const b200ocl_net_desc* desc, const b200ocl_net_state* st, NetPlan& p) {
   if (!desc || !st || !st->params || !st->packed || !st->bn_stats) {
     set_error("net: null descriptor/state pointer");
@@ -1094,7 +739,6 @@ int check_state(const b200ocl_net_desc* desc, const b200ocl_net_state* st, NetPl
   return rc;
 }
 
-}  // namespace
 }  // namespace b200ocl
 
 extern "C" {
@@ -1290,217 +934,6 @@ int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N
     a.relu = mode == 4;
   }
   return launch_conv(a, sms, stream);
-}
-
-int b200ocl_net_sgd_step(const b200ocl_net_desc* desc, const b200ocl_net_state* st, float lr, float weight_decay,
-                         const b200ocl_net_state* dst, void* stream_) {
-  using namespace b200ocl;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  NetPlan p;
-  int rc = check_state(desc, st, p);
-  if (rc) return rc;
-  B200OCL_CHECK_ARG(st->grads, "state has no gradient arena");
-  float* out_params = dst ? dst->params : st->params;
-  float* out_packed = dst ? dst->packed : st->packed;
-  B200OCL_CHECK_ARG(out_params && out_packed, "destination state incomplete");
-  size_t skip_lo, skip_hi;
-  sgd_skip_range(p, skip_lo, skip_hi);
-  const unsigned blocks = arena_grid(p, 8, (size_t)-1);
-  B200OCL_PROF("sgd", 12.0 * p.n_params, stream);
-  net_sgd_kernel<false><<<blocks, 256, 0, stream>>>(st->params, st->grads, out_params, p.n_params, lr,
-                                                              weight_decay, skip_lo, skip_hi, nullptr, nullptr);
-  B200OCL_LAUNCHED();
-  return launch_pack(p, out_params, out_packed, stream);
-}
-
-// The workspace of the entry points that reduce over the arenas (b200ocl::REDUCE_WS_BYTES); 0 for a bad description.
-static size_t reduce_workspace_bytes(const b200ocl_net_desc* desc) {
-  using namespace b200ocl;
-  NetPlan p;
-  if (!desc || build_plan(*desc, p)) return 0;
-  return REDUCE_WS_BYTES;
-}
-
-size_t b200ocl_net_sgd_step_clipped_workspace_bytes(const b200ocl_net_desc* desc) {
-  return reduce_workspace_bytes(desc);   // partials, then counter and coefficient
-}
-
-int b200ocl_net_sgd_step_clipped(const b200ocl_net_desc* desc, const b200ocl_net_state* st, float lr,
-                                 float weight_decay, float max_norm, float* norm_out, void* workspace,
-                                 size_t workspace_bytes, void* stream_) {
-  using namespace b200ocl;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  NetPlan p;
-  int rc = check_state(desc, st, p);
-  if (rc) return rc;
-  B200OCL_CHECK_ARG(st->grads, "state has no gradient arena");
-  if ((rc = check_workspace("b200ocl_net_sgd_step_clipped", workspace, workspace_bytes,
-                            b200ocl_net_sgd_step_clipped_workspace_bytes(desc)))) return rc;
-  double* part = static_cast<double*>(workspace);
-  unsigned int* counter = reduce_counter(workspace);
-  float* coef = reduce_scalars(workspace);
-  size_t skip_lo, skip_hi;
-  sgd_skip_range(p, skip_lo, skip_hi);
-  const unsigned norm_grid = arena_grid(p, 2, NORM_MAX_GRID);
-  B200OCL_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), stream));
-  B200OCL_PROF("grad_norm", 4.0 * p.n_params, stream);
-  grad_norm_kernel<<<norm_grid, 256, 0, stream>>>(st->grads, p.n_params, skip_lo, skip_hi, max_norm, part, counter, coef,
-                                                  norm_out);
-  B200OCL_LAUNCHED();
-  B200OCL_PROF("sgd", 16.0 * p.n_params, stream);
-  net_sgd_kernel<true><<<arena_grid(p, 8, (size_t)-1), 256, 0, stream>>>(st->params, st->grads, st->params, p.n_params, lr,
-                                                             weight_decay, skip_lo, skip_hi, coef, st->grads);
-  B200OCL_LAUNCHED();
-  return launch_pack(p, st->params, st->packed, stream);
-}
-
-static int ewc_setup(const char* entry, const b200ocl_net_desc* desc, const b200ocl_net_state* st,
-                     const b200ocl_ewc_state* ewc, void* workspace, size_t workspace_bytes, b200ocl::NetPlan& p) {
-  using namespace b200ocl;
-  int rc = check_state(desc, st, p);
-  if (rc) return rc;
-  B200OCL_CHECK_ARG(ewc && ewc->running && ewc->tmp && ewc->normalized && ewc->prev, "EWC state incomplete");
-  return check_workspace(entry, workspace, workspace_bytes, REDUCE_WS_BYTES);
-}
-
-size_t b200ocl_net_sgd_step_ewc_workspace_bytes(const b200ocl_net_desc* desc) { return reduce_workspace_bytes(desc); }
-
-int b200ocl_net_sgd_step_ewc(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const b200ocl_ewc_state* ewc,
-                             float lr, float weight_decay, float up, int flags, float ema_keep, float ema_add,
-                             float* penalty_out, void* workspace, size_t workspace_bytes, void* stream_) {
-  using namespace b200ocl;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  NetPlan p;
-  int rc = ewc_setup("b200ocl_net_sgd_step_ewc", desc, st, ewc, workspace, workspace_bytes, p);
-  if (rc) return rc;
-  size_t skip_lo, skip_hi;
-  sgd_skip_range(p, skip_lo, skip_hi);
-  const unsigned grid = arena_grid(p, 8, NORM_MAX_GRID);
-  unsigned int* counter = reduce_counter(workspace);
-  B200OCL_CHECK_ARG(st->grads, "state has no gradient arena");
-  B200OCL_CHECK_ARG((flags & ~(B200OCL_EWC_PENALTY | B200OCL_EWC_EMA)) == 0, "unknown EWC flags");
-  const bool pen = flags & B200OCL_EWC_PENALTY, ema = flags & B200OCL_EWC_EMA;
-  double* part = static_cast<double*>(workspace);
-  float* pen_out = pen ? penalty_out : nullptr;
-  if (pen_out) B200OCL_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), stream));
-  auto kernel = pen ? (ema ? net_sgd_ewc_kernel<true, true> : net_sgd_ewc_kernel<false, true>)
-                    : (ema ? net_sgd_ewc_kernel<true, false> : net_sgd_ewc_kernel<false, false>);
-  B200OCL_PROF("sgd_ewc", 4.0 * p.n_params * (5 + (pen ? 3 : 0) + (ema ? 2 : 0)), stream);
-  kernel<<<grid, 256, 0, stream>>>(st->params, st->grads, ewc->running, ewc->tmp, ewc->normalized, ewc->prev,
-                                   p.n_params, skip_lo, skip_hi, lr, weight_decay, up, ema_keep, ema_add, part, counter,
-                                   pen_out);
-  B200OCL_LAUNCHED();
-  if (penalty_out && !pen) B200OCL_CUDA(cudaMemsetAsync(penalty_out, 0, sizeof(float), stream));
-  return launch_pack(p, st->params, st->packed, stream);
-}
-
-size_t b200ocl_ewc_consolidate_workspace_bytes(const b200ocl_net_desc* desc) { return reduce_workspace_bytes(desc); }
-
-int b200ocl_ewc_consolidate(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const b200ocl_ewc_state* ewc,
-                            void* workspace, size_t workspace_bytes, void* stream_) {
-  using namespace b200ocl;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  NetPlan p;
-  int rc = ewc_setup("b200ocl_ewc_consolidate", desc, st, ewc, workspace, workspace_bytes, p);
-  if (rc) return rc;
-  size_t skip_lo, skip_hi;
-  sgd_skip_range(p, skip_lo, skip_hi);
-  const unsigned grid = arena_grid(p, 8, NORM_MAX_GRID);
-  unsigned int* counter = reduce_counter(workspace);
-  float* range = reduce_scalars(workspace);
-  B200OCL_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), stream));
-  B200OCL_PROF("ewc_consolidate", 12.0 * p.n_params, stream);
-  ewc_minmax_kernel<<<grid, 256, 0, stream>>>(st->params, ewc->running, ewc->prev, p.n_params, skip_lo, skip_hi,
-                                              static_cast<float2*>(workspace), counter, range);
-  B200OCL_LAUNCHED();
-  B200OCL_PROF("ewc_consolidate", 8.0 * p.n_params, stream);
-  ewc_normalize_kernel<<<grid, 256, 0, stream>>>(ewc->running, ewc->normalized, p.n_params, skip_lo, skip_hi, range);
-  B200OCL_LAUNCHED();
-  return B200OCL_OK;
-}
-
-int b200ocl_adam_step(float* p, float* g, float* m, float* v, size_t n, const b200ocl_adam_scalars* s, int flags,
-                      void* stream_) {
-  using namespace b200ocl;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  B200OCL_CHECK_ARG(s && (n == 0 || (p && g && m && v)), "null pointer");
-  AdamCoef c;
-  B200OCL_CHECK_ARG(adam_coef(*s, flags, c), "unknown Adam flags");
-  if (n == 0) return B200OCL_OK;
-  size_t blocks = (n + 255) / 256;
-  const size_t cap = (size_t)8 * sm_count();
-  if (blocks > cap) blocks = cap;
-  B200OCL_PROF("adam", 28.0 * n, stream);
-  if (flags & B200OCL_ADAM_FOREACH) launch_adam<true>((unsigned)blocks, stream, p, g, m, v, n, 0, 0, c,
-                                                      flags & B200OCL_ADAM_GRAD_SCALE);
-  else launch_adam<false>((unsigned)blocks, stream, p, g, m, v, n, 0, 0, c, flags & B200OCL_ADAM_GRAD_SCALE);
-  B200OCL_LAUNCHED();
-  return B200OCL_OK;
-}
-
-int b200ocl_net_adam_step(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const b200ocl_adam_state* adam,
-                          const b200ocl_adam_scalars* s, int flags, void* stream_) {
-  using namespace b200ocl;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  NetPlan p;
-  int rc = check_state(desc, st, p);
-  if (rc) return rc;
-  B200OCL_CHECK_ARG(st->grads, "state has no gradient arena");
-  B200OCL_CHECK_ARG(adam && adam->exp_avg && adam->exp_avg_sq && s, "Adam state incomplete");
-  AdamCoef c;
-  B200OCL_CHECK_ARG(adam_coef(*s, flags, c), "unknown Adam flags");
-  size_t skip_lo, skip_hi;
-  sgd_skip_range(p, skip_lo, skip_hi);
-  const unsigned blocks = arena_grid(p, 8, (size_t)-1);
-  const bool gdiv = flags & B200OCL_ADAM_GRAD_SCALE;
-  B200OCL_PROF("adam", (gdiv ? 32.0 : 28.0) * p.n_params, stream);
-  if (flags & B200OCL_ADAM_FOREACH) launch_adam<true>(blocks, stream, st->params, st->grads, adam->exp_avg,
-                                                      adam->exp_avg_sq, p.n_params, skip_lo, skip_hi, c, gdiv);
-  else launch_adam<false>(blocks, stream, st->params, st->grads, adam->exp_avg, adam->exp_avg_sq, p.n_params, skip_lo,
-                          skip_hi, c, gdiv);
-  B200OCL_LAUNCHED();
-  return launch_pack(p, st->params, st->packed, stream);
-}
-
-int b200ocl_net_adam_step_ewc(const b200ocl_net_desc* desc, const b200ocl_net_state* st, const b200ocl_ewc_state* ewc,
-                              const b200ocl_adam_state* adam, const b200ocl_adam_scalars* s, int adam_flags, float up,
-                              int flags, float ema_keep, float ema_add, float* penalty_out, void* workspace,
-                              size_t workspace_bytes, void* stream_) {
-  using namespace b200ocl;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  NetPlan p;
-  int rc = ewc_setup("b200ocl_net_adam_step_ewc", desc, st, ewc, workspace, workspace_bytes, p);
-  if (rc) return rc;
-  B200OCL_CHECK_ARG(st->grads, "state has no gradient arena");
-  B200OCL_CHECK_ARG(adam && adam->exp_avg && adam->exp_avg_sq && s, "Adam state incomplete");
-  B200OCL_CHECK_ARG((adam_flags & ~B200OCL_ADAM_FOREACH) == 0, "unknown Adam flags for the EWC++ step");
-  AdamCoef c;
-  B200OCL_CHECK_ARG(adam_coef(*s, adam_flags, c), "unknown Adam flags");
-  B200OCL_CHECK_ARG((flags & ~(B200OCL_EWC_PENALTY | B200OCL_EWC_EMA)) == 0, "unknown EWC flags");
-  size_t skip_lo, skip_hi;
-  sgd_skip_range(p, skip_lo, skip_hi);
-  const unsigned grid = arena_grid(p, 8, NORM_MAX_GRID);
-  unsigned int* counter = reduce_counter(workspace);
-  const bool pen = flags & B200OCL_EWC_PENALTY, ema = flags & B200OCL_EWC_EMA;
-  const bool fe = adam_flags & B200OCL_ADAM_FOREACH;
-  double* part = static_cast<double*>(workspace);
-  float* pen_out = pen ? penalty_out : nullptr;
-  if (pen_out) B200OCL_CUDA(cudaMemsetAsync(counter, 0, sizeof(unsigned int), stream));
-  using K = void (*)(float*, float*, float*, float*, float*, float*, const float*, const float*, size_t, size_t, size_t,
-                     AdamCoef, float, float, float, double*, unsigned int*, float*);
-  static const K kernels[8] = {
-      net_adam_ewc_kernel<false, false, false>, net_adam_ewc_kernel<false, false, true>,
-      net_adam_ewc_kernel<false, true, false>,  net_adam_ewc_kernel<false, true, true>,
-      net_adam_ewc_kernel<true, false, false>,  net_adam_ewc_kernel<true, false, true>,
-      net_adam_ewc_kernel<true, true, false>,   net_adam_ewc_kernel<true, true, true>};
-  const K kernel = kernels[(ema ? 4 : 0) + (pen ? 2 : 0) + (fe ? 1 : 0)];
-  B200OCL_PROF("adam_ewc", 4.0 * p.n_params * (10 + (pen ? 3 : 0) + (ema ? 2 : 0)), stream);
-  kernel<<<grid, 256, 0, stream>>>(st->params, st->grads, adam->exp_avg, adam->exp_avg_sq, ewc->running, ewc->tmp,
-                                   ewc->normalized, ewc->prev, p.n_params, skip_lo, skip_hi, c, up, ema_keep, ema_add,
-                                   part, counter, pen_out);
-  B200OCL_LAUNCHED();
-  if (penalty_out && !pen) B200OCL_CUDA(cudaMemsetAsync(penalty_out, 0, sizeof(float), stream));
-  return launch_pack(p, st->params, st->packed, stream);
 }
 
 size_t b200ocl_net_eval_workspace_bytes(const b200ocl_net_desc* desc, int N) {

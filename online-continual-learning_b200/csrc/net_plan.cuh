@@ -229,4 +229,9 @@ inline int build_plan(const b200ocl_net_desc& d, NetPlan& p) {
   return B200OCL_OK;
 }
 
+// net_fwd.cu: the plan of a network state whose pointers and description check out (otherwise the error is set and
+// returned), and the refresh of the packed arena from a parameter arena.
+int check_state(const b200ocl_net_desc* desc, const b200ocl_net_state* st, NetPlan& p);
+int launch_pack(const NetPlan& p, const float* params, float* packed, cudaStream_t stream);
+
 }  // namespace b200ocl

@@ -91,7 +91,8 @@ def time_kernel(iters):
         if name.value.decode() == 'adam':
             kernel_ms = ms.value / cnt.value
     nbytes = 28.0 * n
-    return {'kernel': 'adam_kernel', 'n_params': n, 'kernel_us': kernel_ms * 1e3, 'entry_with_repack_us': ms_entry * 1e3,
+    return {'kernel': 'arena_step_kernel<Adam<true>>', 'n_params': n, 'kernel_us': kernel_ms * 1e3,
+            'entry_with_repack_us': ms_entry * 1e3,
             'bytes': nbytes, 'bytes_per_s': nbytes / (kernel_ms * 1e-3),
             'hbm_lower_bound_us': nbytes / HBM_BYTES_PER_S * 1e6}
 

@@ -118,7 +118,7 @@ def main():
                           'launches_per_step': float(np.median([t[1] for t in r])),
                           'runs_ms_per_step': [t[0] for t in r], 'steps': args.steps}), flush=True)
     n, k = time_kernel(args.kernel_iters)
-    print(json.dumps({'kernel': 'net_sgd_ewc_kernel', 'n_params': n, **k}), flush=True)
+    print(json.dumps({'kernel': 'arena_step_kernel<Sgd, EWC, EMA, PEN>', 'n_params': n, **k}), flush=True)
 
 
 if __name__ == '__main__':
