@@ -19,6 +19,11 @@ multirun.multiple_run_tune_separate, which trains R of main_tune.py's tuning and
 imports it by name after install()).  uninstall() puts both back; an attribute experiment.run lacked stays absent.  Unset
 or 1 leaves them alone; any other value, and every refusal of multirun.check_concurrent, raises ValueError before
 anything is replaced.
+
+With B200OCL_RUN_DEVICES (a comma-separated list of CUDA ordinals, e.g. 0,1,2,3 or 0,0) install() replaces the same
+two drivers whatever R is: their trainings then run in worker processes, one per list entry, R at a time in each.  A
+non-integer, a negative ordinal or an empty entry raises ValueError, as do the refusals of R > 1.  Unset or empty
+changes nothing.
 """
 from .learners import AGEM, EWC_pp, ExperienceReplay, Gdumb, Icarl, Lwf, SupContrastReplay
 from .retrieve import ASER_retrieve, MIR_retrieve, Random_retrieve
@@ -51,6 +56,7 @@ update_methods = {
 }
 
 _installed = {}
+installed_extra = ()      # the extra agents of the last install(); worker processes install the same
 
 
 def install(reference_name_match=None, extra=()):
@@ -64,7 +70,8 @@ def install(reference_name_match=None, extra=()):
                                                                       ', '.join(sorted(extra_agents))))
     from . import multirun
     n_concurrent = multirun.concurrent_runs()
-    multirun.check_concurrent(n_concurrent)
+    devices = multirun.run_devices()
+    multirun.check_concurrent(n_concurrent, devices=devices)
     if reference_name_match is None:
         reference_name_match = importlib.import_module('utils.name_match')
     nm = reference_name_match
@@ -89,7 +96,7 @@ def install(reference_name_match=None, extra=()):
             continue
         replaced[(mod_name, attr)] = getattr(mod, attr, None)
         setattr(mod, attr, obj)
-    if n_concurrent > 1:
+    if n_concurrent > 1 or devices:
         run = importlib.import_module('experiment.run')
         replaced[('experiment.run', 'multiple_run')] = run.multiple_run
         run.multiple_run = multirun.multiple_run
@@ -97,6 +104,8 @@ def install(reference_name_match=None, extra=()):
             replaced[('experiment.run', 'multiple_run_tune_separate')] = run.multiple_run_tune_separate
             run.multiple_run_tune_separate = multirun.multiple_run_tune_separate
     _installed.update(replaced)
+    global installed_extra
+    installed_extra = extra
     return replaced
 
 
@@ -114,3 +123,5 @@ def uninstall(reference_name_match=None):
         elif old is not None:
             setattr(importlib.import_module(where), key, old)
     _installed.clear()
+    global installed_extra
+    installed_extra = ()
