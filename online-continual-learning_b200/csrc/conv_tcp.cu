@@ -50,8 +50,9 @@ constexpr int TP_THREADS = 32 * 16;
 constexpr int TP_EPI_WARP = 8;                      // first epilogue warp
 constexpr int TP_WLOAD_WARP = 12;                   // weight loader
 constexpr int TP_LOADER_WARP = 13;                  // first patch-loader warp
-constexpr int TP_LOADERS = 96;                      // patch-loader threads: 8 chunks x 12 rows per pass
+constexpr int TP_LOADERS = 96;                      // patch-loader threads: nch chunks x 96 / nch rows per pass
 constexpr int TP_LD = (16 * TP_LD_MAX + 11) / 12;   // loads per patch-loader thread: the rows tcp_strip_fits allows
+                                                    // at 12 rows per pass (a full 32-channel slice)
 constexpr int TP_PS_MAX = 3;                        // patch stages: 3 when shared memory allows, else 2
 constexpr int TP_BS_MAX = 6;                        // weight ring depth (streaming mode): 6 or 4
 constexpr int TP_CONSUMER_WARPS = 8;                // arrivals that release a patch stage or a weight slot
@@ -65,6 +66,39 @@ static_assert(128 * TP_REG_LOAD + 256 * TP_REG_MMA + 128 * TP_REG_EPI <= 65536, 
 
 using umma::mbar_expect_tx;
 using umma::bulk_g2s;
+
+// Timeline build (-DB200OCL_TCP_TRACE, tools/tcp_trace.py; never in the shipped library): one thread per role writes
+// %clock64 stamps into the buffer b200ocl_tcp_trace_set installs, laid out [CTA][role][unit][TCP_EV] (unit: the CTA's
+// tap, slice or tile counter).  Role TCP_HDR holds %globaltimer / %clock64 at the CTA's start and end and its SM.
+// Events per unit --
+//   consumer warpgroup 0 / 1, per tap: 0 issue start (pfull wait), 1 bfull wait, 2 MMA issue, 3 committed,
+//     4 wait_group, 5 promotion, 6 retired; the tile's last tap: 7 aempty waited, 8 s_acc stored and afull arrived
+//   weight loader, per tap: 0 bempty wait, 1 copy issue, 2 issued
+//   patch loaders, per slice: 0 loads issued from, 1 pempty wait, 2 split and store, 3 pfull arrived
+//   epilogue, per tile: 0 residual loads, 1 afull wait, 2 store, 3 aempty arrived
+#ifdef B200OCL_TCP_TRACE
+enum { TCP_C0, TCP_C1, TCP_WLOAD, TCP_PLOAD, TCP_EPI, TCP_HDR, TCP_ROLES };
+constexpr int TCP_EV = 9;
+__device__ unsigned long long* g_tcp_trace;
+__device__ int g_tcp_trace_units;
+__device__ __forceinline__ unsigned long long tcp_globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+// tcp_units / tcp_cta are read once per CTA (TCP_TRACE_SETUP), so that a stamp is a clock read and a store
+#define TCP_TRACE_SETUP                                                                                          \
+  const int tcp_units = g_tcp_trace_units;                                                                      \
+  unsigned long long* const tcp_cta =                                                                           \
+      g_tcp_trace + ((unsigned long long)blockIdx.y * gridDim.x + blockIdx.x) * TCP_ROLES * tcp_units * TCP_EV
+#define TCP_AT(role, unit, ev) tcp_cta[((role) * tcp_units + (unit)) * TCP_EV + (ev)]
+#define TCP_STAMP(on, role, unit, ev)                                          \
+  do {                                                                         \
+    if ((on) && (unit) < tcp_units) TCP_AT(role, unit, ev) = clock64();        \
+  } while (0)
+#else
+#define TCP_STAMP(on, role, unit, ev) do { } while (0)
+#endif
 
 struct TileGeom {
   int wp, pp;        // strip row length W + 1, strip image size (H + 1) * (W + 1)
@@ -140,6 +174,13 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
     s_fail = 0;
   }
   __syncthreads();
+#ifdef B200OCL_TCP_TRACE
+  TCP_TRACE_SETUP;
+  if (tid == 0) {
+    TCP_AT(TCP_HDR, 0, 0) = tcp_globaltimer();
+    TCP_AT(TCP_HDR, 0, 1) = clock64();
+  }
+#endif
   const float* wimg = a.w_tp + (size_t)blockIdx.y * slices * 9 * B_BLOCK;
 
   if (warp >= TP_LOADER_WARP) {
@@ -148,14 +189,17 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
     int pc = 0;
     for (int tile = blockIdx.x; tile < a.tp_tiles; tile += gridDim.x) {
       for (int sl = 0; sl < slices; ++sl, ++pc) {
+        TCP_STAMP(lt == 0, TCP_PLOAD, pc, 0);
         const int ch_valid = min(32, a.CK - sl * 32);       // real channels in this slice (multiple of 4)
         const int nch = 2 * ((ch_valid + 7) / 8);            // 16-byte chunks the MMAs will read per row
-        // thread -> (patch row lt/8 + 12*i, chunk lt%8): lanes with chunk >= nch idle
-        const int ch = lt & 7, r0 = lt >> 3;
+        // thread -> (patch row lt/nch + step*i, chunk lt%nch): every lane loads, so a slice of 8 / 16 / 24 channels
+        // takes 1/4 / 1/2 / 3/4 of a full slice's passes (nch = 2, 4, 6 or 8 divides the 96 threads)
+        const int step = TP_LOADERS / nch;                   // rows per pass: 48, 24, 16 or 12
+        const int ch = lt % nch, r0 = lt / nch;
         const int nrow = G.prow;
-        const bool ch_live = ch < nch, ch_real = ch * 4 < ch_valid;
+        const bool ch_real = ch * 4 < ch_valid;
         float4 v[TP_LD];
-        // strip position of this thread's first row, then 12 rows further per pass (no divisions in the loop)
+        // strip position of this thread's first row, then step rows further per pass (no divisions in the loop)
         int img, yp, xp;
         {
           const int sp = tile * 128 + r0;
@@ -167,14 +211,15 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
         const int hp = a.Hin + 1;                             // strip rows per image: the zero row, then H pixel rows
 #pragma unroll
         for (int i = 0; i < TP_LD; ++i) {
+          const int ri = r0 + step * i;
+          if (ri >= nrow) break;
           v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-          const int ri = r0 + 12 * i;
-          if (ch_real && ri < nrow) {
+          if (ch_real) {
             const int y = yp - 1, x = xp - 1;
             if (img < a.N && (unsigned)y < (unsigned)a.Hin && (unsigned)x < (unsigned)a.Win)
               v[i] = __ldg(reinterpret_cast<const float4*>(a.in + ((size_t)(img * a.Hin + y) * a.Win + x) * a.CK + sl * 32) + ch);
           }
-          xp += 12;
+          xp += step;
           while (xp >= G.wp) {
             xp -= G.wp;
             if (++yp == hp) {
@@ -184,25 +229,25 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
           }
         }
         const int ps = pc % PS;
+        TCP_STAMP(lt == 0, TCP_PLOAD, pc, 1);
         if (!umma::mbar_wait(&pempty[ps], (uint32_t)(((pc / PS) & 1) ^ 1))) s_fail = 1;
+        TCP_STAMP(lt == 0, TCP_PLOAD, pc, 2);
         float* ph = reinterpret_cast<float*>(patch0 + (size_t)ps * 2 * G.pbytes);
         float* pl = ph + G.pbytes / 4;
-        if (ch_live) {
 #pragma unroll
-          for (int i = 0; i < TP_LD; ++i) {
-            const int ri = r0 + 12 * i;
-            if (ri < nrow) {
-              float4 h, l;
-              umma::split_tf32(v[i].x, h.x, l.x); umma::split_tf32(v[i].y, h.y, l.y);
-              umma::split_tf32(v[i].z, h.z, l.z); umma::split_tf32(v[i].w, h.w, l.w);
-              const int off = umma::sw128_offset_f32(ri, ch);
-              *reinterpret_cast<float4*>(ph + off) = h;
-              *reinterpret_cast<float4*>(pl + off) = l;
-            }
-          }
+        for (int i = 0; i < TP_LD; ++i) {
+          const int ri = r0 + step * i;
+          if (ri >= nrow) break;
+          float4 h, l;
+          umma::split_tf32(v[i].x, h.x, l.x); umma::split_tf32(v[i].y, h.y, l.y);
+          umma::split_tf32(v[i].z, h.z, l.z); umma::split_tf32(v[i].w, h.w, l.w);
+          const int off = umma::sw128_offset_f32(ri, ch);
+          *reinterpret_cast<float4*>(ph + off) = h;
+          *reinterpret_cast<float4*>(pl + off) = l;
         }
         umma::fence_proxy_async_smem();
         umma::mbar_arrive(&pfull[ps]);
+        TCP_STAMP(lt == 0, TCP_PLOAD, pc, 3);
       }
     }
   } else if (warp == TP_WLOAD_WARP) {
@@ -211,8 +256,11 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
     if (resident) {
       if (umma::elect_one_sync()) {
         for (int b = 0; b < 9; ++b) {
+          TCP_STAMP(true, TCP_WLOAD, b, 0);
+          TCP_STAMP(true, TCP_WLOAD, b, 1);
           mbar_expect_tx(&bfull[b], bytes);
           bulk_g2s(sB + (size_t)b * B_BLOCK, wimg + (size_t)b * B_BLOCK, bytes, &bfull[b]);
+          TCP_STAMP(true, TCP_WLOAD, b, 2);
         }
       }
     } else {
@@ -221,12 +269,15 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
         for (int sl = 0; sl < slices; ++sl)
           for (int tap = 0; tap < 9; ++tap, ++q) {
             const int bs = q % BS;
+            TCP_STAMP((tid & 31) == 0, TCP_WLOAD, q, 0);
             if (!umma::mbar_wait(&bempty[bs], (uint32_t)(((q / BS) & 1) ^ 1))) s_fail = 1;
+            TCP_STAMP((tid & 31) == 0, TCP_WLOAD, q, 1);
             if (umma::elect_one_sync()) {
               mbar_expect_tx(&bfull[bs], bytes);
               bulk_g2s(sB + (size_t)bs * B_BLOCK, wimg + (size_t)(sl * 9 + tap) * B_BLOCK, bytes, &bfull[bs]);
             }
             __syncwarp();
+            TCP_STAMP((tid & 31) == 0, TCP_WLOAD, q, 2);
           }
     }
   } else if (warp >= TP_EPI_WARP) {
@@ -245,6 +296,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
     int k = 0;                                           // tiles this CTA has finished
     for (int tile = blockIdx.x; tile < a.tp_tiles; tile += gridDim.x, ++k) {
       const int buf = k & 1;
+      TCP_STAMP(et == 0, TCP_EPI, k, 0);
       const int sp = tile * 128 + et;                    // strip position of this MMA row
       const int img = sp / G.pp, rem = sp - img * G.pp;
       const int y = rem / G.wp, x = rem - y * G.wp;
@@ -267,7 +319,9 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
           pre[c0] = v.x; pre[c0 + 1] = v.y; pre[c0 + 2] = v.z; pre[c0 + 3] = v.w;
         }
       }
+      TCP_STAMP(et == 0, TCP_EPI, k, 1);
       if (!umma::mbar_wait(&afull[buf], (uint32_t)((k >> 1) & 1))) s_fail = 1;
+      TCP_STAMP(et == 0, TCP_EPI, k, 2);
       const float* row = s_acc + (size_t)buf * ACC_TILE + et * (NT + 1);
       if (valid) {
         float* o = a.out + m * a.CN + n0;
@@ -290,6 +344,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
         }
       }
       umma::mbar_arrive(&aempty[buf]);
+      TCP_STAMP(et == 0, TCP_EPI, k, 3);
     }
   } else {
     // =========================================================== consumers (warps 0-7)
@@ -309,6 +364,10 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
     int ips = 0, ib = 0, rps = 0, rb = 0;
     uint32_t ipph = 0, ibph = 0;
     bool b_ready = false;
+#ifdef B200OCL_TCP_TRACE
+    const bool tr = wt == 0;
+    int tu_i = 0, tu_r = 0;                  // the CTA's taps issued / retired
+#endif
     int k = 0;                               // tiles this CTA has finished
     for (int tile = blockIdx.x; tile < a.tp_tiles; tile += gridDim.x, ++k) {
       float accf[R];
@@ -319,11 +378,14 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
       // completes the last MMA reading it has returned.
       int is = 0, it = 0, rt = 0;
       auto issue = [&](float (&d)[R]) {
+        TCP_STAMP(tr, g, tu_i, 0);
         if (it == 0)
           if (!umma::mbar_wait(&pfull[ips], ipph)) s_fail = 1;
+        TCP_STAMP(tr, g, tu_i, 1);
         const int b = resident ? it : ib;
         if (!(resident && b_ready))
           if (!umma::mbar_wait(&bfull[b], resident ? 0u : ibph)) s_fail = 1;
+        TCP_STAMP(tr, g, tu_i, 2);
         const int kh = it / 3, kw = it - 3 * kh;
         const uint64_t dAh = dA0 + (uint64_t)(ips * A_STAGE) + (uint64_t)((kh * G.wp + kw) * 8);   // + (kh*(W+1) + kw) rows
         const uint64_t dAl = dAh + A_LO;
@@ -335,6 +397,10 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
           case 3: issue_tap<NT, 3>(d, dAh, dAl, dBh, dBl); break;
           default: issue_tap<NT, 4>(d, dAh, dAl, dBh, dBl); break;
         }
+#ifdef B200OCL_TCP_TRACE
+        TCP_STAMP(tr, g, tu_i, 3);
+        ++tu_i;
+#endif
         if (!resident && ++ib == BS) {
           ib = 0;
           ibph ^= 1u;
@@ -350,6 +416,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
         }
       };
       auto retire = [&](float (&d)[R]) {
+        TCP_STAMP(tr, g, tu_r, 5);
         umma::fence_regs(d);
 #pragma unroll
         for (int i = 0; i < R; ++i) accf[i] += d[i];
@@ -362,6 +429,10 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
           if (++rps == PS) rps = 0;
         }
         if (++rt == 9) rt = 0;
+#ifdef B200OCL_TCP_TRACE
+        TCP_STAMP(tr, g, tu_r, 6);
+        ++tu_r;
+#endif
       };
       // Every exit drains with wait<0> in the block that leaves the loop, so that the compiler sees no fragment
       // in flight past it.
@@ -370,32 +441,47 @@ __global__ void __launch_bounds__(TP_THREADS, 1) conv_tcp_kernel(ConvArgs a) {
 #pragma unroll 1
       for (int j = 0;; j += 2) {   // fa holds tap j, fb tap j + 1
         if (j + 1 >= T) {
+          TCP_STAMP(tr, g, tu_r, 4);
           umma::wait<0>();
           retire(fa);
           break;
         }
         issue(fb);
+        TCP_STAMP(tr, g, tu_r, 4);
         umma::wait<1>();
         retire(fa);
         if (j + 2 >= T) {
+          TCP_STAMP(tr, g, tu_r, 4);
           umma::wait<0>();
           retire(fb);
           break;
         }
         issue(fa);
+        TCP_STAMP(tr, g, tu_r, 4);
         umma::wait<1>();
         retire(fb);
       }
       // ---- fragments -> pixel rows of s_acc[k % 2], once the epilogue has read that buffer's previous tile
       const int buf = k & 1;
       if (!umma::mbar_wait(&aempty[buf], (uint32_t)(((k >> 1) & 1) ^ 1))) s_fail = 1;
+      TCP_STAMP(tr, g, tu_r - 1, 7);
       float* acc_out = s_acc + (size_t)buf * ACC_TILE;
 #pragma unroll
       for (int i = 0; i < R; ++i) acc_out[(64 * g + umma::frag_row(wt, i)) * (NT + 1) + umma::frag_col(wt, i)] = accf[i];
       umma::mbar_arrive(&afull[buf]);
+      TCP_STAMP(tr, g, tu_r - 1, 8);
     }
   }
   __syncthreads();
+#ifdef B200OCL_TCP_TRACE
+  if (tid == 0) {
+    TCP_AT(TCP_HDR, 0, 2) = tcp_globaltimer();
+    TCP_AT(TCP_HDR, 0, 3) = clock64();
+    unsigned smid;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+    TCP_AT(TCP_HDR, 0, 4) = smid;
+  }
+#endif
   // a timed-out barrier (must never happen) poisons the output instead of hanging the GPU
   if (s_fail && tid == 0) a.out[(size_t)n0] = __int_as_float(0x7fc00000);
 }
@@ -470,3 +556,14 @@ int launch_conv_tcp(const ConvArgs& a, const ConvPlan& pl, cudaStream_t stream) 
 }
 
 }  // namespace b200ocl
+
+#ifdef B200OCL_TCP_TRACE
+// Timeline build only: the stamp buffer of the conv_tcp launches that follow, `units` per CTA and role
+// ([CTA][role][unit][TCP_EV] uint64).  Declared by the tool that loads that build, not in include/b200ocl.h.
+extern "C" int b200ocl_tcp_trace_set(unsigned long long* buf, int units) {
+  using namespace b200ocl;
+  B200OCL_CUDA(cudaMemcpyToSymbol(g_tcp_trace, &buf, sizeof(buf)));
+  B200OCL_CUDA(cudaMemcpyToSymbol(g_tcp_trace_units, &units, sizeof(units)));
+  return B200OCL_OK;
+}
+#endif
