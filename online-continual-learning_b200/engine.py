@@ -241,6 +241,55 @@ class Engine:
         _native.check(_lib().b200ocl_net_pack(ctypes.byref(self.desc), ctypes.byref(st.c), _stream()),
                       'b200ocl_net_pack')
 
+    # ------------------------------------------------------------------ snapshot / restore (checkpoint.py)
+    def snapshot(self):
+        """The arenas a resumed run reads, on the host: parameters, BN running statistics and bn_tracked, and when they
+        exist the teacher's (parameters, statistics, bn_tracked), EWC++'s running / tmp / normalized Fisher and previous
+        parameters, and Adam's moments and step count.  The current stream is synchronised once, then each arena is one
+        device-to-host copy.  Packed weights, gradients, workspaces and MIR's virtual copy are rebuilt or overwritten
+        before they are read, so they are not kept."""
+        torch.cuda.current_stream(self.device).synchronize()
+        host = lambda t: t.to('cpu')                                                 # noqa: E731
+        out = {'params': host(self.state.params), 'bn_stats': host(self.state.bn_stats),
+               'bn_tracked': host(self.state.bn_tracked)}
+        if self._teacher is not None:
+            t = self._teacher
+            out['teacher'] = {'params': host(t.params), 'bn_stats': host(t.bn_stats), 'bn_tracked': host(t.bn_tracked)}
+        if getattr(self, '_ewc', None) is not None:
+            out['ewc'] = {k: host(getattr(self._ewc, k)) for k in ('running', 'tmp', 'normalized', 'prev')}
+        if getattr(self, '_adam', None) is not None:
+            out['adam'] = {'exp_avg': host(self._adam.exp_avg), 'exp_avg_sq': host(self._adam.exp_avg_sq),
+                           'step': self._adam.step}
+        return out
+
+    def restore(self, state):
+        """Copy a snapshot() back into the arenas, in place (the Parameters, EWC++ views and optimizer state that alias
+        them stay valid), allocating the teacher, EWC++ and Adam arenas it holds, then rebuild the packed weights with
+        pack().  One host-to-device copy per arena on the current stream."""
+        def put(dst, src):
+            if dst.shape != src.shape or dst.dtype != src.dtype:
+                raise ValueError('snapshot arena %s %s does not fit %s %s' % (tuple(src.shape), src.dtype,
+                                                                          tuple(dst.shape), dst.dtype))
+            dst.copy_(src)
+        for k in ('params', 'bn_stats', 'bn_tracked'):
+            put(getattr(self.state, k), state[k])
+        if 'teacher' in state:
+            if self._teacher is None:
+                self._teacher = ArenaState(self.info, self.device, with_grads=False)
+            for k in ('params', 'bn_stats', 'bn_tracked'):
+                put(getattr(self._teacher, k), state['teacher'][k])
+            self.pack(self._teacher)
+        if 'ewc' in state:
+            st = self.ewc_state()
+            for k in ('running', 'tmp', 'normalized', 'prev'):
+                put(getattr(st, k), state['ewc'][k])
+        if 'adam' in state:
+            st = self.adam_state()
+            put(st.exp_avg, state['adam']['exp_avg'])
+            put(st.exp_avg_sq, state['adam']['exp_avg_sq'])
+            st.step = int(state['adam']['step'])
+        self.pack()
+
     def virtual_state(self):
         if self._virtual is None:
             self._virtual = ArenaState(self.info, self.device, with_grads=False)

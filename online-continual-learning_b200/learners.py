@@ -407,6 +407,37 @@ class ContinualLearner(torch.nn.Module):
                                  'exp_avg': st.exp_avg[o:o + n].view(p.shape),
                                  'exp_avg_sq': st.exp_avg_sq[o:o + n].view(p.shape)}
 
+    # ------------------------------------------------------------------ snapshot / restore (checkpoint.py)
+    _TABLES = ('old_labels', 'new_labels', 'task_seen', 'lbl_inv_map', 'class_task_map', 'error_list', 'new_class_score',
+               'old_class_score', 'fc_norm_new', 'fc_norm_old', 'bias_norm_new', 'bias_norm_old')
+
+    def snapshot(self):
+        """What train_learner and evaluate read next, at a task boundary: the engine's arenas (Engine.snapshot), the
+        buffer's (Buffer.snapshot) when the learner has one, the label bookkeeping, the error-analysis history, whether
+        the teacher is live and whether Adam has started.  restore() on a learner built with the same params takes it
+        back."""
+        out = {k: pickle.loads(pickle.dumps(getattr(self, k))) for k in self._TABLES}
+        out['new_labels_zombie'] = list(getattr(self, 'new_labels_zombie', []))
+        out['teacher_live'], out['adam_started'] = self._teacher_live, self._adam_started
+        out['engine'] = self.engine.snapshot()
+        if isinstance(getattr(self, 'buffer', None), Buffer):
+            out['buffer'] = self.buffer.snapshot()
+        return out
+
+    def restore(self, state):
+        """The inverse of snapshot(), on a learner built with the same params and not trained yet.  The derived device
+        tables (separated softmax) are uploaded again and, with a torch.optim.Adam, opt.state shows the restored
+        moments, as after a train_learner call."""
+        self.engine.restore(state['engine'])
+        for k in self._TABLES:
+            setattr(self, k, state[k])
+        self.new_labels_zombie = list(state['new_labels_zombie'])
+        self._teacher_live, self._adam_started = state['teacher_live'], state['adam_started']
+        if 'buffer' in state:
+            self.buffer.restore(state['buffer'])
+        self._task_tables()
+        self._adam_export()
+
     def before_train(self, x_train, y_train):
         new_labels = list(set(np.asarray(y_train).tolist()))
         self.new_labels += new_labels
@@ -921,6 +952,15 @@ class Icarl(ContinualLearner):
         # the reference fails here in list.index (ValueError, icarl.py:44), not in a dict lookup (KeyError, base.py:105)
         self._pos_err = None
 
+    def snapshot(self):
+        out = super().snapshot()
+        out['prev_live'], out['updated'] = self._prev_live, self._updated.copy()
+        return out
+
+    def restore(self, state):
+        super().restore(state)
+        self._prev_live, self._updated = state['prev_live'], np.array(state['updated'], dtype=bool)
+
     def _task_tables(self):
         super()._task_tables()
         if not self.new_labels:
@@ -1023,6 +1063,15 @@ class Gdumb(ContinualLearner):
         """The reference's mem_c: label -> count in insertion order."""
         return self.memory.mem_c
 
+    def snapshot(self):
+        out = super().snapshot()
+        out['memory'] = self.memory.snapshot()
+        return out
+
+    def restore(self, state):
+        super().restore(state)
+        self.memory.restore(state['memory'])
+
     def train_mem(self):
         """gdumb.py:52-83."""
         _drain(self._train_mem_steps())
@@ -1116,6 +1165,15 @@ class EWC_pp(ContinualLearner):
                                zip(names, self.engine.table, self.model.parameters())}
         self.running_fisher, self.tmp_fisher = views(st.running), views(st.tmp)
         self.normalized_fisher, self._prev = views(st.normalized), views(st.prev)
+
+    def snapshot(self):
+        out = super().snapshot()
+        out['penalty_live'] = self._penalty_live
+        return out
+
+    def restore(self, state):
+        super().restore(state)
+        self._penalty_live = state['penalty_live']
 
     @property
     def prev_params(self):

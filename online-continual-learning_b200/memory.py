@@ -516,6 +516,25 @@ class GreedyBalancedMemory(object):
         parts = [np.asarray(self.slots[c], dtype=np.int64) for c in self.mem_c]
         return np.concatenate(parts) if parts else np.zeros(0, dtype=np.int64)
 
+    def snapshot(self):
+        """The pool on the host (one device-to-host copy of the images after a synchronise of the current stream) and
+        the decision state: counts and slot lists in their insertion order, the free-slot stack, the label mirror."""
+        if self.images.is_cuda:
+            torch.cuda.current_stream(self.device).synchronize()
+        return {'images': self.images.to('cpu'), 'labels': self._labels_host.copy(), 'mem_c': dict(self.mem_c),
+                'slots': {c: list(v) for c, v in self.slots.items()}, 'free': list(self._free), 'size': self._size}
+
+    def restore(self, state):
+        if tuple(state['images'].shape) != tuple(self.images.shape):
+            raise ValueError('snapshot memory %s does not fit %s' % (tuple(state['images'].shape), tuple(self.images.shape)))
+        self.images.copy_(state['images'])
+        self._labels_host = np.asarray(state['labels'], dtype=np.int64).copy()
+        self.labels = torch.from_numpy(self._labels_host.copy()).to(self.device)
+        self.mem_c = dict(state['mem_c'])
+        self.slots = {c: list(v) for c, v in state['slots'].items()}
+        self._free = list(state['free'])
+        self._size = int(state['size'])
+
 
 # --------------------------------------------------------------------------- buffer
 def random_retrieve(buffer, num_retrieve, excl_indices=None, return_indices=False):
@@ -571,6 +590,33 @@ class Buffer(torch.nn.Module):
 
     def update(self, x, y, **kwargs):
         return self.update_method.update(buffer=self, x=x, y=y, **kwargs)
+
+    def snapshot(self):
+        """The filled slots on the host (rows current_index.. are never written before the rows below them), the
+        counters, the label mirror with this buffer's deferred updates applied, and the update plugin's own state when
+        it keeps one (GSS's scores).  The current stream is synchronised once, then one device-to-host copy per tensor."""
+        flush_pending(self)
+        if self.buffer_img.is_cuda:
+            torch.cuda.current_stream(self.buffer_img.device).synchronize()
+        n = self.current_index
+        out = {'images': self.buffer_img[:n].to('cpu'), 'labels': self.buffer_label[:n].to('cpu'),
+               'labels_host': self._labels_host.copy(), 'current_index': n, 'n_seen_so_far': self.n_seen_so_far}
+        if hasattr(self.update_method, 'snapshot'):
+            out['update'] = self.update_method.snapshot()
+        return out
+
+    def restore(self, state):
+        n = int(state['current_index'])
+        if n > self.buffer_img.shape[0] or tuple(state['images'].shape[1:]) != tuple(self.buffer_img.shape[1:]):
+            raise ValueError('snapshot buffer %s does not fit %s' % (tuple(state['images'].shape),
+                                                                    tuple(self.buffer_img.shape)))
+        flush_pending(self)
+        self.buffer_img[:n].copy_(state['images'])
+        self.buffer_label[:n].copy_(state['labels'])
+        self._labels_host = np.asarray(state['labels_host'], dtype=np.int64).copy()
+        self.current_index, self.n_seen_so_far = n, int(state['n_seen_so_far'])
+        if 'update' in state:
+            self.update_method.restore(state['update'])
 
     def retrieve(self, **kwargs):
         return self.retrieve_method.retrieve(buffer=self, **kwargs)

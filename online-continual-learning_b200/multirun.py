@@ -19,6 +19,9 @@ every run's final training is one entry of run_group, seeded by tune_seed() and 
 With B200OCL_RUN_DEVICES (a list of CUDA ordinals) both drivers hand their trainings to worker processes instead, one per
 list entry (WorkerPool); each worker runs them through run_group, R at a time, on its own device.  A training's seed does
 not depend on where it runs, so its numbers are the same as in one process.
+
+With B200OCL_CHECKPOINT_DIR run_group writes each training's snapshot after every task and its record once it ends, and
+both drivers resume an interrupted experiment from them (checkpoint.py).
 """
 import contextlib
 import io
@@ -165,6 +168,40 @@ class RunRng(object):
         self.cpu = torch.get_rng_state()
         self.cuda = torch.cuda.get_rng_state() if _cuda_rng() else None
 
+    def snapshot(self):
+        """The four states as a picklable tuple (restore() takes it back)."""
+        return (self.py, self.np, self.cpu.clone(), None if self.cuda is None else self.cuda.clone())
+
+    def restore(self, state):
+        self.py, self.np, self.cpu, self.cuda = state
+        if self.cuda is None and _cuda_rng():
+            raise ValueError('a snapshot taken without CUDA cannot resume a run that uses the CUDA generator')
+
+
+class _Tee(object):
+    """A stdout that writes to two streams (a run's per-run line to its output and to its record)."""
+
+    def __init__(self, out, copy):
+        self.out, self.copy = out, copy
+
+    def write(self, s):
+        self.copy.write(s)
+        return self.out.write(s)
+
+    def flush(self):
+        self.out.flush()
+
+
+def _teed(fn, copy):
+    def call(*args):
+        out = sys.stdout
+        sys.stdout = _Tee(out, copy)
+        try:
+            return fn(*args)
+        finally:
+            sys.stdout = out
+    return call
+
 
 class _Run(object):
     """One run of a group: its random state, its host state, its stream, its agent, and where its prints go (None: the
@@ -179,6 +216,29 @@ class _Run(object):
         self.agent = None
         self.steps = None
         self.acc = []
+        self.start = 0          # the first task this run trains (after a restored snapshot: the task after it)
+
+    def snapshot(self, task):
+        """The run's state at the end of `task`, after its evaluation: the deferred host-mirror updates are drained,
+        then its agent's snapshot() is taken under its stream; the random and host states are the ones run.call left."""
+        def take():
+            memory.flush_pending()
+            return self.agent.snapshot()
+        agent = self.call(take)
+        return {'task': task, 'acc': [np.array(a) for a in self.acc], 'rng': self.rng.snapshot(),
+                'sampler': self.host.sampler, 'agent': agent}
+
+    def restore(self, snap):
+        """Continue from a snapshot of this run: its agent (built as usual) takes the snapshot's state, then the
+        random state, the sampler state and the accuracy rows; training restarts at the task after the snapshot's."""
+        if len(snap['acc']) != snap['task'] + 1:
+            raise ValueError('run %d: a snapshot of task %d holds %d accuracy rows'
+                             % (self.index, snap['task'], len(snap['acc'])))
+        self.call(self.agent.restore, snap['agent'])
+        self.rng.restore(snap['rng'])
+        self.host.sampler, self.host.pending = snap['sampler'], []
+        self.acc = [np.array(a) for a in snap['acc']]
+        self.start = snap['task'] + 1
 
     def call(self, fn, *args):
         """fn(*args) with this run's random state, host state, stream and stdout current.  An exception leaves with
@@ -213,7 +273,7 @@ def _next_step(steps):
 
 
 def run_group(tasks_per_run, test_loaders_per_run, make_agent, n_concurrent, seed=0, first_run=0,
-              on_task=None, on_run_end=None, before_run=None, seeds=None, stdout=None):
+              on_task=None, on_run_end=None, before_run=None, seeds=None, stdout=None, checkpoint=None):
     """Train and evaluate len(tasks_per_run) runs, n_concurrent at a time, and return each run's accuracy array
     (np.array of the per-task evaluate() results, [n_tasks, n_test_loaders]).
 
@@ -226,11 +286,21 @@ def run_group(tasks_per_run, test_loaders_per_run, make_agent, n_concurrent, see
     agent is dropped once its last evaluation is done.
     Optional hooks, all called with the run's state current: before_run(r), on_task(r, t, x_train, y_train) before the
     run starts task t, on_run_end(r, acc) after the run's last evaluation.  stdout[i], when given, receives everything
-    run first_run + i prints (its hooks, its agent's construction, steps and evaluations)."""
+    run first_run + i prints (its hooks, its agent's construction, steps and evaluations).
+
+    checkpoint (a checkpoint.Checkpoint, default None: nothing is read or written): run first_run + i is its training
+    first_run + i.  A run with a record is not trained: its array is returned and its text printed in run order, before
+    the next group if that group's runs all follow it, else just before the next run's on_run_end.  The others are cut
+    into groups as above; a run with a snapshot is
+    built as usual, then restored, and trains from the task after the snapshot's.  After its evaluation of every task
+    but its last a run's snapshot is written; after on_run_end its record (what on_run_end printed)."""
     n_concurrent = int(n_concurrent)
     if n_concurrent < 1:
         raise ValueError('n_concurrent must be >= 1, got %d' % n_concurrent)
     check_concurrent(n_concurrent)
+    if checkpoint is not None:
+        from .checkpoint import check_checkpoint
+        check_checkpoint(checkpoint.directory)
     n_runs = len(tasks_per_run)
     if len(test_loaders_per_run) != n_runs:
         raise ValueError('%d task lists for %d sets of test loaders' % (n_runs, len(test_loaders_per_run)))
@@ -240,14 +310,30 @@ def run_group(tasks_per_run, test_loaders_per_run, make_agent, n_concurrent, see
         raise ValueError('%d seeds for %d runs' % (len(seeds), n_runs))
     if stdout is not None and len(stdout) != n_runs:
         raise ValueError('%d outputs for %d runs' % (len(stdout), n_runs))
+    done = {}
+    if checkpoint is not None:
+        for i in range(n_runs):
+            rec = checkpoint.record(first_run + i)
+            if rec is not None:
+                done[i] = rec
+    results = [done[i][0] if i in done else None for i in range(n_runs)]
+    replayed = []
+
+    def replay(upto):
+        """Print the records of the runs before position `upto`, in run order."""
+        for i in sorted(done):
+            if i < upto and i not in replayed:
+                (sys.stdout if stdout is None else stdout[i]).write(done[i][1])
+                replayed.append(i)
     memory.flush_pending()
     outer_rng, outer_host = RunRng.capture(), memory.RunHostState()
     outer_host.leave()
-    results = []
+    todo = [i for i in range(n_runs) if i not in done]
     try:
-        for g0 in range(0, n_runs, n_concurrent):
+        for g0 in range(0, len(todo), n_concurrent):
             group = [_Run(first_run + i, seeds[i], None if stdout is None else stdout[i])
-                     for i in range(g0, min(g0 + n_concurrent, n_runs))]
+                     for i in todo[g0:g0 + n_concurrent]]
+            replay(group[0].index - first_run)
             tasks, loaders = [], []
             for run in group:
                 i = run.index - first_run
@@ -260,27 +346,43 @@ def run_group(tasks_per_run, test_loaders_per_run, make_agent, n_concurrent, see
                 if n_concurrent > 1 and getattr(run.agent, 'grad_sync', None) is not None:
                     raise ValueError('run %d: an agent with data-parallel gradient sync cannot share the GPU with other '
                                      'runs' % run.index)
+                snap = None if checkpoint is None else checkpoint.snapshot(run.index)
+                if snap is not None:
+                    run.restore(snap)
             for t in range(max(len(ts) for ts in tasks)):
                 live = []
                 for run, ts in zip(group, tasks):
-                    if t < len(ts):
+                    if run.start <= t < len(ts):
                         x, y = ts[t][0], ts[t][1]
                         if on_task is not None:
                             run.call(on_task, run.index, t, x, y)
                         run.steps = run.agent._steps(x, y)
                         live.append(run)
+                trained = list(live)
                 while live:                                                 # one step per run, in run order
                     live = [run for run in live if run.call(_next_step, run.steps)]
                 for run, ts, ls in zip(group, tasks, loaders):
-                    if t < len(ts):
+                    if run in trained:
                         run.acc.append(run.call(run.agent.evaluate, ls))
+                if checkpoint is not None:
+                    for run, ts in zip(group, tasks):
+                        if run in trained and t < len(ts) - 1:
+                            checkpoint.save_snapshot(run.index, run.snapshot(t))
             for run in group:
+                replay(run.index - first_run)
                 acc = np.array(run.acc)
-                if on_run_end is not None:
-                    run.call(on_run_end, run.index, acc)
-                results.append(acc)
+                if checkpoint is None:
+                    if on_run_end is not None:
+                        run.call(on_run_end, run.index, acc)
+                else:
+                    text = io.StringIO()
+                    if on_run_end is not None:
+                        run.call(_teed(on_run_end, text), run.index, acc)
+                    checkpoint.save_record(run.index, acc, text.getvalue())
+                results[run.index - first_run] = acc
                 run.agent = run.steps = None                                # its engine arenas and graphs go with it
             del group, tasks, loaders
+        replay(n_runs)
     finally:
         outer_host.enter()
         outer_rng.swap_in()
@@ -466,6 +568,13 @@ class _Recipe(object):
     """What a driver's trainings need, sent to every worker: picklable descriptions (params, seeds, the caller's random
     state) only.  Attributes named in LOCAL (the data continuum, task lists, hook state) are rebuilt where it runs."""
     LOCAL = ()
+    checkpoint_dir = None         # B200OCL_CHECKPOINT_DIR of the driver (None: no checkpoints)
+
+    def _checkpoint(self, stage):
+        if self.checkpoint_dir is None:
+            return None
+        from .checkpoint import Checkpoint
+        return Checkpoint(self.checkpoint_dir, stage)
 
     def __getstate__(self):
         return {k: v for k, v in self.__dict__.items() if k not in self.LOCAL}
@@ -484,6 +593,19 @@ class _Recipe(object):
             return continuum(params.data, params.cl_type, params), RunRng.capture()
         finally:
             keep.swap_in()
+
+
+def _open_checkpoint(checkpoint_dir, params, grid=None):
+    """A driver's checkpoint directory (None: none), with its refusals and fingerprint checked before anything is
+    built."""
+    from . import checkpoint
+    directory = checkpoint.checkpoint_dir() if checkpoint_dir is None else (checkpoint_dir or None)
+    if directory is None:
+        return None
+    checkpoint.check_checkpoint(directory)
+    from . import registry
+    checkpoint.open_dir(directory, checkpoint.fingerprint(params, registry.installed_extra, grid=grid))
+    return directory
 
 
 # --------------------------------------------------------------------------- the reference's multiple_run
@@ -547,10 +669,10 @@ class _Repetitions(_Recipe):
         n = r1 - r0
         return run_group([self.task_list] * n, [self.test_loaders] * n, self.make_agent, R, seed=self.params.seed,
                          first_run=r0, before_run=self.new_run, on_task=self.on_task, on_run_end=self.on_run_end,
-                         stdout=outs)
+                         stdout=outs, checkpoint=self._checkpoint('runs'))
 
 
-def multiple_run(params, store=False, save_path=None, n_concurrent=None, devices=None):
+def multiple_run(params, store=False, save_path=None, n_concurrent=None, devices=None, checkpoint_dir=None):
     """experiment/run.py:multiple_run with up to R = B200OCL_CONCURRENT_RUNS runs at once.  Same stdout lines (the per-run
     line of each run once it ends, then the compute_performance summary), same --store pickle ({'time', 'acc_array'} in
     config/global.yml's result path) and the offline mode (online: False) of the reference.  Each run of a group keeps
@@ -559,7 +681,10 @@ def multiple_run(params, store=False, save_path=None, n_concurrent=None, devices
     With worker devices (B200OCL_RUN_DEVICES, or `devices`) the runs are trained by a WorkerPool, R at a time in each
     worker, and each run's lines are printed in run order once it and every run before it have ended.  This process
     still builds the continuum, so its lines (and the caller's random state after it) are the in-process ones; it
-    drops it before the workers start, and each worker builds its own, silently."""
+    drops it before the workers start, and each worker builds its own, silently.
+
+    With a checkpoint directory (B200OCL_CHECKPOINT_DIR, or `checkpoint_dir`; '' turns it off) the runs resume from it
+    (checkpoint.py): its fingerprint is checked before anything is built."""
     from continuum.continuum import continuum
     from experiment.metrics import compute_performance
     from utils.io import load_yaml
@@ -569,6 +694,7 @@ def multiple_run(params, store=False, save_path=None, n_concurrent=None, devices
     check_concurrent(R, devices=devices)
     if devices:
         check_device_count(devices)
+    directory = _open_checkpoint(checkpoint_dir, params)
     entry_rng = RunRng.capture()
     start = time.time()
     print('Setting up data stream')
@@ -585,6 +711,7 @@ def multiple_run(params, store=False, save_path=None, n_concurrent=None, devices
 
     online = params.online
     recipe = _Repetitions(params, entry_rng, None if devices else data_continuum)
+    recipe.checkpoint_dir = directory
     if devices:
         from . import registry
         del data_continuum
@@ -731,7 +858,8 @@ class _Tuning(_Recipe):
         return run_group([self.data(ri)[0] for ri, _, _ in ents], [self.data(ri)[1] for ri, _, _ in ents],
                          lambda i: self.build(self.point_params[self.entries[i][1]]), R, first_run=i0,
                          seeds=[tune_seed(self.defaults['seed'], self.run_list[ri], g, v) for ri, g, v in ents],
-                         before_run=self.tune_begin, on_task=self.tune_task, on_run_end=self.tune_end, stdout=outs)
+                         before_run=self.tune_begin, on_task=self.tune_task, on_run_end=self.tune_end, stdout=outs,
+                         checkpoint=self._checkpoint('tune'))
 
     # stage 2: each run's final agent, with its chosen point
     def final(self, r0, r1, R, outs=None, params_keep=(), default_params=None):
@@ -764,14 +892,16 @@ class _Tuning(_Recipe):
         self._keep_only(set(ris))
         return run_group([self.data(ri)[2] for ri in ris], [self.data(ri)[3] for ri in ris], make, R,
                          first_run=r0, seeds=[run_seed(self.defaults['seed'], self.run_list[ri]) for ri in ris],
-                         before_run=begin, on_task=task, on_run_end=end, stdout=outs)
+                         before_run=begin, on_task=task, on_run_end=end, stdout=outs,
+                         checkpoint=self._checkpoint('final'))
 
 
 def _concat(tasks):
     return [(np.concatenate([x for x, _ in tasks], axis=0), np.concatenate([y for _, y in tasks], axis=0))]
 
 
-def multiple_run_tune_separate(default_params, tune_params, save_path, n_concurrent=None, devices=None):
+def multiple_run_tune_separate(default_params, tune_params, save_path, n_concurrent=None, devices=None,
+                               checkpoint_dir=None):
     """experiment/run.py:multiple_run_tune_separate (main_tune.py) with up to R = B200OCL_CONCURRENT_RUNS trainings at
     once, for both of its branches (single_tune, and single_tune_train_val with train_val), online and offline.
 
@@ -790,7 +920,10 @@ def multiple_run_tune_separate(default_params, tune_params, save_path, n_concurr
     each worker, and each training's lines are printed in training order.  This process still draws every run's data,
     in run order, printing what the draws print, but keeps no run's lists; each worker replays the chain of draws from
     the caller's random state on entry, silently, and keeps the runs it is given.  default_params gets the last run's
-    point once every final training has ended."""
+    point once every final training has ended.
+
+    With a checkpoint directory (B200OCL_CHECKPOINT_DIR, or `checkpoint_dir`; '' turns it off) both stages resume from
+    it (checkpoint.py): its fingerprint, the grid included, is checked before anything is built."""
     from continuum.continuum import continuum
     from experiment.metrics import compute_performance
     from utils.io import check_ram_usage, load_yaml
@@ -800,6 +933,7 @@ def multiple_run_tune_separate(default_params, tune_params, save_path, n_concurr
     check_concurrent(R, devices=devices)
     if devices:
         check_device_count(devices)
+    directory = _open_checkpoint(checkpoint_dir, default_params, grid=tune_params)
     entry_rng = RunRng.capture()
     start = time.time()
     print('Setting up data stream')
@@ -826,6 +960,7 @@ def multiple_run_tune_separate(default_params, tune_params, save_path, n_concurr
                     else default_params.num_runs)
     grid = param_grid(tune_params)
     recipe = _Tuning(dict(vars(default_params)), grid, run_list, start, entry_rng)
+    recipe.checkpoint_dir = directory
 
     def choose(tune_acc):
         """The chosen points, as tune_hyper chooses them."""
@@ -850,6 +985,8 @@ def multiple_run_tune_separate(default_params, tune_params, save_path, n_concurr
         recipe.data_all(data_continuum)
         params_keep = choose(recipe.tune(0, len(recipe.entries), R))
         accuracy_list = recipe.final(0, len(run_list), R, params_keep=params_keep, default_params=default_params)
+        if directory is not None:
+            vars(default_params).update(params_keep[-1])    # the last run's final agent may come from a record
     end = time.time()
     result = {'seed': default_params.seed, 'time': end - start, 'acc_array': np.array(accuracy_list),
               'ram': check_ram_usage(), 'best_params': params_keep}

@@ -24,6 +24,10 @@ With B200OCL_RUN_DEVICES (a comma-separated list of CUDA ordinals, e.g. 0,1,2,3 
 two drivers whatever R is: their trainings then run in worker processes, one per list entry, R at a time in each.  A
 non-integer, a negative ordinal or an empty entry raises ValueError, as do the refusals of R > 1.  Unset or empty
 changes nothing.
+
+With B200OCL_CHECKPOINT_DIR (a directory) install() replaces the same two drivers whatever R is, so that an
+interrupted experiment resumes from its last finished task (checkpoint.py).  Parity mode and data-parallel gradient sync
+are refused with ValueError before anything is replaced.  Unset or empty changes nothing.
 """
 from .learners import AGEM, EWC_pp, ExperienceReplay, Gdumb, Icarl, Lwf, SupContrastReplay
 from .retrieve import ASER_retrieve, MIR_retrieve, Random_retrieve
@@ -68,10 +72,12 @@ def install(reference_name_match=None, extra=()):
     if unknown:
         raise ValueError('unknown extra agent(s) %s; available: %s' % (', '.join(map(repr, unknown)),
                                                                       ', '.join(sorted(extra_agents))))
-    from . import multirun
+    from . import checkpoint, multirun
     n_concurrent = multirun.concurrent_runs()
     devices = multirun.run_devices()
     multirun.check_concurrent(n_concurrent, devices=devices)
+    directory = checkpoint.checkpoint_dir()
+    checkpoint.check_checkpoint(directory)
     if reference_name_match is None:
         reference_name_match = importlib.import_module('utils.name_match')
     nm = reference_name_match
@@ -96,7 +102,7 @@ def install(reference_name_match=None, extra=()):
             continue
         replaced[(mod_name, attr)] = getattr(mod, attr, None)
         setattr(mod, attr, obj)
-    if n_concurrent > 1 or devices:
+    if n_concurrent > 1 or devices or directory:
         run = importlib.import_module('experiment.run')
         replaced[('experiment.run', 'multiple_run')] = run.multiple_run
         run.multiple_run = multirun.multiple_run

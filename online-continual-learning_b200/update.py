@@ -199,6 +199,13 @@ class GSSGreedyUpdate(object):
         self.last_batch_sim = None        # kept for inspection (tests: near-zero decisions)
         self.last_replaced = None
 
+    def snapshot(self):
+        """The score of every slot, on the host (the buffer's snapshot() synchronised the stream)."""
+        return {'buffer_score': self.buffer_score.to('cpu')}
+
+    def restore(self, state):
+        self.buffer_score.copy_(state['buffer_score'])
+
     # ---- one gradient: model.zero_grad(); F.cross_entropy(model.forward(x), y).backward()  (:80-83, :100-103, :117-119)
     def _gradient(self, eng, x, y):
         from .engine import ce_loss
