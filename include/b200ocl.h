@@ -544,6 +544,37 @@ size_t b200ocl_wgrad_tc_selftest_workspace_bytes(int N, int H, int W, int cin, i
 int b200ocl_wgrad_tc_selftest(const float* x, const float* dz, float* dw_oihw, int N, int H, int W, int cin, int cout,
                               void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- task snapshots (checkpoint.py, B200OCL_CHECKPOINT_ASYNC): one staging arena per run ----
+ * A segment is one device array of a snapshot and its region of the staging arena, which holds `bytes` bytes at
+ * `offset`.  B200OCL_SNAP_COPY regions hold the bytes as they are.  B200OCL_SNAP_U8 segments are fp32 replay-memory
+ * rows (bytes a multiple of 4): each value v is stored as one byte u = rint(v * 255) when v is finite, 0 <= u <= 255
+ * and u / 255 (IEEE division, the stream feeder's, common.cuh:u8_unit) is v bit for bit; the region keeps its fp32
+ * size so that a segment with any other value can be stored as fp32 instead.  The table itself is in device memory. */
+#define B200OCL_SNAP_COPY 0
+#define B200OCL_SNAP_U8 1
+typedef struct b200ocl_snapshot_segment {
+  uint64_t ptr;    /* device address: the source (pack) or the destination (unpack); 16-byte aligned is fastest */
+  uint64_t bytes;  /* bytes at ptr */
+  uint64_t offset; /* byte offset of the segment's region in the staging arena */
+  int32_t kind;    /* pack: B200OCL_SNAP_COPY or B200OCL_SNAP_U8; unpack: the form the region holds */
+  int32_t reserved;
+} b200ocl_snapshot_segment;
+
+/* Workspace of pack and unpack: int32 counters[n_segments + 1].  After a pack, counters[s] is the number of values
+ * of U8 segment s that failed the test (its region then holds the fp32 rows) and counters[n_segments] the number of
+ * segments that were skipped as malformed (a region past staging_bytes, or a U8 size not a multiple of 4); after an
+ * unpack, counters[n_segments] is the latter. */
+size_t b200ocl_snapshot_workspace_bytes(int n_segments);
+/* Copy (or encode) every segment into the staging arena: a memset of the counters, one launch that copies COPY
+ * segments and encodes U8 segments while counting rejections, and one launch that overwrites the region of every U8
+ * segment with a non-zero counter with its fp32 rows.  Nothing is read back. */
+int b200ocl_snapshot_pack(const b200ocl_snapshot_segment* table, int n_segments, void* staging, size_t staging_bytes,
+                          void* workspace, size_t workspace_bytes, void* stream);
+/* The inverse: one launch that copies each COPY region to its ptr and decodes each U8 region (bytes / 4 bytes) into
+ * bytes / 4 fp32 values u / 255 at its ptr. */
+int b200ocl_snapshot_unpack(const b200ocl_snapshot_segment* table, int n_segments, const void* staging,
+                            size_t staging_bytes, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

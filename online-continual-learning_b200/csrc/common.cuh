@@ -100,6 +100,10 @@ __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
 }
 
+// An 8-bit image value in [0, 1]: u / 255 with an IEEE division (torchvision's ToTensor).  The stream feeder and the
+// snapshot encoder / decoder share it, so a stored byte always decodes to the value the stream produced.
+__device__ __forceinline__ float u8_unit(unsigned u) { return __fdiv_rn((float)u, 255.f); }
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL_MASK, v, o);

@@ -166,7 +166,7 @@ __global__ void __launch_bounds__(256) stream_prepare_kernel(const unsigned char
   float* out = dst + (size_t)blockIdx.x * row;
   for (int o = threadIdx.x; o < (int)row; o += blockDim.x) {
     const int c = o / hw, pix = o - c * hw;
-    out[o] = __fdiv_rn((float)s_img[pix * 3 + c], 255.f);
+    out[o] = u8_unit(s_img[pix * 3 + c]);
   }
 }
 

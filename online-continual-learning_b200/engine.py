@@ -145,6 +145,11 @@ def set_graphs(on):
 
 
 _replayed = [0]      # kernel launches issued through graph replays (the library's own counter only sees eager ones)
+# Held while a graph is captured.  A capture fails when another thread of the process makes a CUDA call that may
+# synchronise meanwhile, so a thread that copies from the device beside training (checkpoint.py's writer) takes it
+# around each of its CUDA calls.
+import threading as _threading
+capture_lock = _threading.Lock()
 
 
 def graph_launch_count():
@@ -167,13 +172,14 @@ class _Graphed:
             self.calls += 1
             return
         if not self.graphs:                      # second call: capture all executables, run the first
-            for _ in range(self.N_EXEC):
-                before = _native.launch_count()
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    launch()
-                self.kernels = int(_native.launch_count() - before)
-                self.graphs.append(g)
+            with capture_lock:
+                for _ in range(self.N_EXEC):
+                    before = _native.launch_count()
+                    g = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g):
+                        launch()
+                    self.kernels = int(_native.launch_count() - before)
+                    self.graphs.append(g)
         self.graphs[self.turn].replay()
         self.turn = (self.turn + 1) % self.N_EXEC
         _replayed[0] += self.kernels
@@ -242,25 +248,32 @@ class Engine:
                       'b200ocl_net_pack')
 
     # ------------------------------------------------------------------ snapshot / restore (checkpoint.py)
-    def snapshot(self):
-        """The arenas a resumed run reads, on the host: parameters, BN running statistics and bn_tracked, and when they
+    def snapshot_parts(self):
+        """The arenas a resumed run reads, on the device: parameters, BN running statistics and bn_tracked, and when they
         exist the teacher's (parameters, statistics, bn_tracked), EWC++'s running / tmp / normalized Fisher and previous
-        parameters, and Adam's moments and step count.  The current stream is synchronised once, then each arena is one
-        device-to-host copy.  Packed weights, gradients, workspaces and MIR's virtual copy are rebuilt or overwritten
-        before they are read, so they are not kept."""
-        torch.cuda.current_stream(self.device).synchronize()
-        host = lambda t: t.to('cpu')                                                 # noqa: E731
-        out = {'params': host(self.state.params), 'bn_stats': host(self.state.bn_stats),
-               'bn_tracked': host(self.state.bn_tracked)}
+        parameters, and Adam's moments and step count (a host int).  Packed weights, gradients, workspaces and MIR's
+        virtual copy are rebuilt or overwritten before they are read, so they are not kept."""
+        out = {'params': self.state.params, 'bn_stats': self.state.bn_stats, 'bn_tracked': self.state.bn_tracked}
         if self._teacher is not None:
             t = self._teacher
-            out['teacher'] = {'params': host(t.params), 'bn_stats': host(t.bn_stats), 'bn_tracked': host(t.bn_tracked)}
+            out['teacher'] = {'params': t.params, 'bn_stats': t.bn_stats, 'bn_tracked': t.bn_tracked}
         if getattr(self, '_ewc', None) is not None:
-            out['ewc'] = {k: host(getattr(self._ewc, k)) for k in ('running', 'tmp', 'normalized', 'prev')}
+            out['ewc'] = {k: getattr(self._ewc, k) for k in ('running', 'tmp', 'normalized', 'prev')}
         if getattr(self, '_adam', None) is not None:
-            out['adam'] = {'exp_avg': host(self._adam.exp_avg), 'exp_avg_sq': host(self._adam.exp_avg_sq),
-                           'step': self._adam.step}
+            out['adam'] = {'exp_avg': self._adam.exp_avg, 'exp_avg_sq': self._adam.exp_avg_sq, 'step': self._adam.step}
         return out
+
+    def snapshot(self):
+        """snapshot_parts() on the host: the current stream is synchronised once, then each arena is one device-to-host
+        copy."""
+        from .memory import host_tree
+        return host_tree(self.snapshot_parts())
+
+    def snapshot_capacity(self):
+        """Bytes of the largest snapshot_parts() this engine can give: its arenas plus the teacher, EWC++ and Adam arenas
+        it may allocate later."""
+        arena = self.info.n_params * 4 + self.info.n_bn_stats * 4 + self.info.n_bn * 8
+        return 2 * arena + 6 * self.info.n_params * 4
 
     def restore(self, state):
         """Copy a snapshot() back into the arenas, in place (the Parameters, EWC++ views and optimizer state that alias

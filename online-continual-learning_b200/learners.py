@@ -411,18 +411,29 @@ class ContinualLearner(torch.nn.Module):
     _TABLES = ('old_labels', 'new_labels', 'task_seen', 'lbl_inv_map', 'class_task_map', 'error_list', 'new_class_score',
                'old_class_score', 'fc_norm_new', 'fc_norm_old', 'bias_norm_new', 'bias_norm_old')
 
-    def snapshot(self):
-        """What train_learner and evaluate read next, at a task boundary: the engine's arenas (Engine.snapshot), the
-        buffer's (Buffer.snapshot) when the learner has one, the label bookkeeping, the error-analysis history, whether
-        the teacher is live and whether Adam has started.  restore() on a learner built with the same params takes it
-        back."""
+    def snapshot_parts(self):
+        """What train_learner and evaluate read next, at a task boundary, with the device arrays left on the device:
+        the engine's arenas (Engine.snapshot_parts), the buffer's (Buffer.snapshot_parts) when the learner has one, and
+        copies of the label bookkeeping, the error-analysis history, whether the teacher is live and whether Adam has
+        started."""
         out = {k: pickle.loads(pickle.dumps(getattr(self, k))) for k in self._TABLES}
         out['new_labels_zombie'] = list(getattr(self, 'new_labels_zombie', []))
         out['teacher_live'], out['adam_started'] = self._teacher_live, self._adam_started
-        out['engine'] = self.engine.snapshot()
+        out['engine'] = self.engine.snapshot_parts()
         if isinstance(getattr(self, 'buffer', None), Buffer):
-            out['buffer'] = self.buffer.snapshot()
+            out['buffer'] = self.buffer.snapshot_parts()
         return out
+
+    def snapshot(self):
+        """snapshot_parts() on the host.  restore() on a learner built with the same params takes it back."""
+        return memory.host_tree(self.snapshot_parts())
+
+    def snapshot_capacity(self):
+        """Bytes of the largest snapshot_parts() device tree this learner can give."""
+        n = self.engine.snapshot_capacity()
+        if isinstance(getattr(self, 'buffer', None), Buffer):
+            n += self.buffer.snapshot_capacity()
+        return n
 
     def restore(self, state):
         """The inverse of snapshot(), on a learner built with the same params and not trained yet.  The derived device
@@ -952,8 +963,8 @@ class Icarl(ContinualLearner):
         # the reference fails here in list.index (ValueError, icarl.py:44), not in a dict lookup (KeyError, base.py:105)
         self._pos_err = None
 
-    def snapshot(self):
-        out = super().snapshot()
+    def snapshot_parts(self):
+        out = super().snapshot_parts()
         out['prev_live'], out['updated'] = self._prev_live, self._updated.copy()
         return out
 
@@ -1063,10 +1074,13 @@ class Gdumb(ContinualLearner):
         """The reference's mem_c: label -> count in insertion order."""
         return self.memory.mem_c
 
-    def snapshot(self):
-        out = super().snapshot()
-        out['memory'] = self.memory.snapshot()
+    def snapshot_parts(self):
+        out = super().snapshot_parts()
+        out['memory'] = self.memory.snapshot_parts()
         return out
+
+    def snapshot_capacity(self):
+        return super().snapshot_capacity() + self.memory.snapshot_capacity()
 
     def restore(self, state):
         super().restore(state)
@@ -1166,8 +1180,8 @@ class EWC_pp(ContinualLearner):
         self.running_fisher, self.tmp_fisher = views(st.running), views(st.tmp)
         self.normalized_fisher, self._prev = views(st.normalized), views(st.prev)
 
-    def snapshot(self):
-        out = super().snapshot()
+    def snapshot_parts(self):
+        out = super().snapshot_parts()
         out['penalty_live'] = self._penalty_live
         return out
 

@@ -222,6 +222,39 @@ def flush_pending(owner=None):
     _pending.extend(keep)
 
 
+class Rows8(object):
+    """A replay-memory image tensor in a snapshot_parts() tree: fp32 rows that, for 8-bit streams, all hold u / 255 for
+    a byte u, so a staged snapshot may store them at one byte per value (checkpoint.py)."""
+    __slots__ = ('tensor',)
+
+    def __init__(self, tensor):
+        self.tensor = tensor
+
+
+def host_tree(tree):
+    """A snapshot_parts() tree with every tensor on the host: one synchronise of the current stream when a leaf is on
+    a CUDA device, then one device-to-host copy per tensor (a host tensor is kept as it is, as .to('cpu') does)."""
+    def leaves(t):
+        if isinstance(t, dict):
+            return [x for v in t.values() for x in leaves(v)]
+        if isinstance(t, (list, tuple)):
+            return [x for v in t for x in leaves(v)]
+        return [t.tensor if isinstance(t, Rows8) else t]
+
+    def host(t):
+        if isinstance(t, dict):
+            return {k: host(v) for k, v in t.items()}
+        if isinstance(t, Rows8):
+            return t.tensor.to('cpu')
+        if isinstance(t, torch.Tensor):
+            return t.to('cpu')
+        return t
+    cuda = [t for t in leaves(tree) if isinstance(t, torch.Tensor) and t.is_cuda]
+    if cuda:
+        torch.cuda.current_stream(cuda[0].device).synchronize()
+    return host(tree)
+
+
 class RunHostState(object):
     """The module-level host state of the replay path that belongs to one run when several runs share the process
     (multirun.run_group): the class-level state of ClassBalancedRandomSampling, which the buffers of one run share as
@@ -516,13 +549,20 @@ class GreedyBalancedMemory(object):
         parts = [np.asarray(self.slots[c], dtype=np.int64) for c in self.mem_c]
         return np.concatenate(parts) if parts else np.zeros(0, dtype=np.int64)
 
+    def snapshot_parts(self):
+        """snapshot() with the pool left on the device (marked as 8-bit rows) and the decision state copied: counts and
+        slot lists in their insertion order, the free-slot stack, the label mirror."""
+        return {'images': Rows8(self.images), 'labels': self._labels_host.copy(), 'mem_c': dict(self.mem_c),
+                'slots': {c: list(v) for c, v in self.slots.items()}, 'free': list(self._free), 'size': self._size}
+
     def snapshot(self):
         """The pool on the host (one device-to-host copy of the images after a synchronise of the current stream) and
-        the decision state: counts and slot lists in their insertion order, the free-slot stack, the label mirror."""
-        if self.images.is_cuda:
-            torch.cuda.current_stream(self.device).synchronize()
-        return {'images': self.images.to('cpu'), 'labels': self._labels_host.copy(), 'mem_c': dict(self.mem_c),
-                'slots': {c: list(v) for c, v in self.slots.items()}, 'free': list(self._free), 'size': self._size}
+        the decision state."""
+        return host_tree(self.snapshot_parts())
+
+    def snapshot_capacity(self):
+        """Bytes of the largest snapshot_parts() device tree."""
+        return self.images.numel() * self.images.element_size()
 
     def restore(self, state):
         if tuple(state['images'].shape) != tuple(self.images.shape):
@@ -591,19 +631,32 @@ class Buffer(torch.nn.Module):
     def update(self, x, y, **kwargs):
         return self.update_method.update(buffer=self, x=x, y=y, **kwargs)
 
+    def snapshot_parts(self):
+        """snapshot() with the filled slots left on the device (the images marked as 8-bit rows) and the host values
+        copied.  This buffer's deferred label-mirror updates are applied first.  The update plugin's state is its
+        snapshot_parts(), or its snapshot() when it has only that."""
+        flush_pending(self)
+        n = self.current_index
+        out = {'images': Rows8(self.buffer_img[:n]), 'labels': self.buffer_label[:n],
+               'labels_host': self._labels_host.copy(), 'current_index': n, 'n_seen_so_far': self.n_seen_so_far}
+        if hasattr(self.update_method, 'snapshot_parts'):
+            out['update'] = self.update_method.snapshot_parts()
+        elif hasattr(self.update_method, 'snapshot'):
+            out['update'] = self.update_method.snapshot()
+        return out
+
     def snapshot(self):
         """The filled slots on the host (rows current_index.. are never written before the rows below them), the
         counters, the label mirror with this buffer's deferred updates applied, and the update plugin's own state when
         it keeps one (GSS's scores).  The current stream is synchronised once, then one device-to-host copy per tensor."""
-        flush_pending(self)
-        if self.buffer_img.is_cuda:
-            torch.cuda.current_stream(self.buffer_img.device).synchronize()
-        n = self.current_index
-        out = {'images': self.buffer_img[:n].to('cpu'), 'labels': self.buffer_label[:n].to('cpu'),
-               'labels_host': self._labels_host.copy(), 'current_index': n, 'n_seen_so_far': self.n_seen_so_far}
-        if hasattr(self.update_method, 'snapshot'):
-            out['update'] = self.update_method.snapshot()
-        return out
+        return host_tree(self.snapshot_parts())
+
+    def snapshot_capacity(self):
+        """Bytes of the largest snapshot_parts() device tree (every slot filled)."""
+        n = sum(t.numel() * t.element_size() for t in (self.buffer_img, self.buffer_label))
+        if hasattr(self.update_method, 'snapshot_parts'):
+            n += sum(t.numel() * t.element_size() for t in self.update_method.snapshot_parts().values())
+        return n
 
     def restore(self, state):
         n = int(state['current_index'])

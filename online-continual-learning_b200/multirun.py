@@ -21,7 +21,8 @@ list entry (WorkerPool); each worker runs them through run_group, R at a time, o
 not depend on where it runs, so its numbers are the same as in one process.
 
 With B200OCL_CHECKPOINT_DIR run_group writes each training's snapshot after every task and its record once it ends, and
-both drivers resume an interrupted experiment from them (checkpoint.py).
+both drivers resume an interrupted experiment from them (checkpoint.py).  With B200OCL_CHECKPOINT_ASYNC=1 as well the
+snapshots are staged on the device and written by a background thread while the next task trains.
 """
 import contextlib
 import io
@@ -215,6 +216,7 @@ class _Run(object):
         self.out = out
         self.agent = None
         self.steps = None
+        self.staging = None     # its checkpoint.Staging when snapshots are written behind the run
         self.acc = []
         self.start = 0          # the first task this run trains (after a restored snapshot: the task after it)
 
@@ -227,6 +229,17 @@ class _Run(object):
         agent = self.call(take)
         return {'task': task, 'acc': [np.array(a) for a in self.acc], 'rng': self.rng.snapshot(),
                 'sampler': self.host.sampler, 'agent': agent}
+
+    def stage(self, task):
+        """snapshot(task), staged: the host state is captured as snapshot() captures it, the agent's device arrays
+        (snapshot_parts()) are packed into the run's staging arena under its stream.  Returns (the snapshot with
+        placeholders for those arrays, the job that writes them)."""
+        def take():
+            memory.flush_pending()
+            return self.staging.stage(self.agent.snapshot_parts())
+        agent, job = self.call(take)
+        return {'task': task, 'acc': [np.array(a) for a in self.acc], 'rng': self.rng.snapshot(),
+                'sampler': self.host.sampler, 'agent': agent}, job
 
     def restore(self, snap):
         """Continue from a snapshot of this run: its agent (built as usual) takes the snapshot's state, then the
@@ -293,14 +306,18 @@ def run_group(tasks_per_run, test_loaders_per_run, make_agent, n_concurrent, see
     the next group if that group's runs all follow it, else just before the next run's on_run_end.  The others are cut
     into groups as above; a run with a snapshot is
     built as usual, then restored, and trains from the task after the snapshot's.  After its evaluation of every task
-    but its last a run's snapshot is written; after on_run_end its record (what on_run_end printed)."""
+    but its last a run's snapshot is written; after on_run_end its record (what on_run_end printed).  With
+    checkpoint.async_write each run gets a staging arena when it is built, snapshots are staged and they and the records
+    are written by the writer thread; every write has ended when run_group returns or raises, and a failed write raises
+    CheckpointError there or at the next task boundary."""
     n_concurrent = int(n_concurrent)
     if n_concurrent < 1:
         raise ValueError('n_concurrent must be >= 1, got %d' % n_concurrent)
     check_concurrent(n_concurrent)
+    staged = checkpoint is not None and checkpoint.async_write
     if checkpoint is not None:
-        from .checkpoint import check_checkpoint
-        check_checkpoint(checkpoint.directory)
+        from . import checkpoint as ckpt
+        ckpt.check_checkpoint(checkpoint.directory)
     n_runs = len(tasks_per_run)
     if len(test_loaders_per_run) != n_runs:
         raise ValueError('%d task lists for %d sets of test loaders' % (n_runs, len(test_loaders_per_run)))
@@ -346,7 +363,9 @@ def run_group(tasks_per_run, test_loaders_per_run, make_agent, n_concurrent, see
                 if n_concurrent > 1 and getattr(run.agent, 'grad_sync', None) is not None:
                     raise ValueError('run %d: an agent with data-parallel gradient sync cannot share the GPU with other '
                                      'runs' % run.index)
-                snap = None if checkpoint is None else checkpoint.snapshot(run.index)
+                if staged:
+                    run.staging = run.call(lambda: ckpt.Staging(run.agent.snapshot_capacity(), run.agent.device))
+                snap = None if checkpoint is None else run.call(checkpoint.snapshot, run.index, run.staging)
                 if snap is not None:
                     run.restore(snap)
             for t in range(max(len(ts) for ts in tasks)):
@@ -367,7 +386,10 @@ def run_group(tasks_per_run, test_loaders_per_run, make_agent, n_concurrent, see
                 if checkpoint is not None:
                     for run, ts in zip(group, tasks):
                         if run in trained and t < len(ts) - 1:
-                            checkpoint.save_snapshot(run.index, run.snapshot(t))
+                            if staged:
+                                checkpoint.save_staged(run.index, *run.stage(t))
+                            else:
+                                checkpoint.save_snapshot(run.index, run.snapshot(t))
             for run in group:
                 replay(run.index - first_run)
                 acc = np.array(run.acc)
@@ -380,9 +402,19 @@ def run_group(tasks_per_run, test_loaders_per_run, make_agent, n_concurrent, see
                         run.call(_teed(on_run_end, text), run.index, acc)
                     checkpoint.save_record(run.index, acc, text.getvalue())
                 results[run.index - first_run] = acc
-                run.agent = run.steps = None                                # its engine arenas and graphs go with it
+                if run.staging is not None:
+                    run.staging.release()
+                run.agent = run.steps = run.staging = None                  # its engine arenas and graphs go with it
             del group, tasks, loaders
         replay(n_runs)
+        if staged:
+            ckpt.writer().drain()
+    except BaseException as e:
+        if staged:                     # every write ends; a failed one is told with the exception that is leaving
+            failed = ckpt.writer().drain(check=False)
+            if failed is not None:
+                e.add_note('and a snapshot write failed meanwhile: %s' % failed)
+        raise
     finally:
         outer_host.enter()
         outer_rng.swap_in()
@@ -569,12 +601,13 @@ class _Recipe(object):
     state) only.  Attributes named in LOCAL (the data continuum, task lists, hook state) are rebuilt where it runs."""
     LOCAL = ()
     checkpoint_dir = None         # B200OCL_CHECKPOINT_DIR of the driver (None: no checkpoints)
+    checkpoint_async = False      # B200OCL_CHECKPOINT_ASYNC of the driver
 
     def _checkpoint(self, stage):
         if self.checkpoint_dir is None:
             return None
         from .checkpoint import Checkpoint
-        return Checkpoint(self.checkpoint_dir, stage)
+        return Checkpoint(self.checkpoint_dir, stage, self.checkpoint_async)
 
     def __getstate__(self):
         return {k: v for k, v in self.__dict__.items() if k not in self.LOCAL}
@@ -596,16 +629,18 @@ class _Recipe(object):
 
 
 def _open_checkpoint(checkpoint_dir, params, grid=None):
-    """A driver's checkpoint directory (None: none), with its refusals and fingerprint checked before anything is
-    built."""
+    """A driver's checkpoint directory (None: none) and whether its snapshots are written behind the runs
+    (B200OCL_CHECKPOINT_ASYNC), with the refusals and the fingerprint checked before anything is built.  The switch is
+    not part of the fingerprint: both forms of snapshot resume either way."""
     from . import checkpoint
     directory = checkpoint.checkpoint_dir() if checkpoint_dir is None else (checkpoint_dir or None)
     if directory is None:
-        return None
+        return None, False
+    async_write = checkpoint.checkpoint_async(directory=directory)
     checkpoint.check_checkpoint(directory)
     from . import registry
     checkpoint.open_dir(directory, checkpoint.fingerprint(params, registry.installed_extra, grid=grid))
-    return directory
+    return directory, async_write
 
 
 # --------------------------------------------------------------------------- the reference's multiple_run
@@ -694,7 +729,7 @@ def multiple_run(params, store=False, save_path=None, n_concurrent=None, devices
     check_concurrent(R, devices=devices)
     if devices:
         check_device_count(devices)
-    directory = _open_checkpoint(checkpoint_dir, params)
+    directory, async_write = _open_checkpoint(checkpoint_dir, params)
     entry_rng = RunRng.capture()
     start = time.time()
     print('Setting up data stream')
@@ -711,7 +746,7 @@ def multiple_run(params, store=False, save_path=None, n_concurrent=None, devices
 
     online = params.online
     recipe = _Repetitions(params, entry_rng, None if devices else data_continuum)
-    recipe.checkpoint_dir = directory
+    recipe.checkpoint_dir, recipe.checkpoint_async = directory, async_write
     if devices:
         from . import registry
         del data_continuum
@@ -933,7 +968,7 @@ def multiple_run_tune_separate(default_params, tune_params, save_path, n_concurr
     check_concurrent(R, devices=devices)
     if devices:
         check_device_count(devices)
-    directory = _open_checkpoint(checkpoint_dir, default_params, grid=tune_params)
+    directory, async_write = _open_checkpoint(checkpoint_dir, default_params, grid=tune_params)
     entry_rng = RunRng.capture()
     start = time.time()
     print('Setting up data stream')
@@ -960,7 +995,7 @@ def multiple_run_tune_separate(default_params, tune_params, save_path, n_concurr
                     else default_params.num_runs)
     grid = param_grid(tune_params)
     recipe = _Tuning(dict(vars(default_params)), grid, run_list, start, entry_rng)
-    recipe.checkpoint_dir = directory
+    recipe.checkpoint_dir, recipe.checkpoint_async = directory, async_write
 
     def choose(tune_acc):
         """The chosen points, as tune_hyper chooses them."""

@@ -6,6 +6,7 @@ streams only.  Non-CUDA inputs raise: there is no CPU path.
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _native
@@ -478,3 +479,35 @@ def adam_step(param, grad, exp_avg, exp_avg_sq, step, lr, betas=(0.9, 0.999), ep
                                          ctypes.byref(s), flags, _stream())
     _native.check(rc, 'b200ocl_adam_step')
     return param
+
+
+# --------------------------------------------------------------------------- task snapshots (checkpoint.py)
+SNAP_COPY, SNAP_U8 = 0, 1           # B200OCL_SNAP_* (include/b200ocl.h)
+SNAP_SEGMENT = np.dtype([('ptr', '<u8'), ('bytes', '<u8'), ('offset', '<u8'), ('kind', '<i4'), ('reserved', '<i4')])
+
+
+def snapshot_workspace(n_segments, device):
+    """Workspace of snapshot_pack / snapshot_unpack over n_segments segments: its first n_segments + 1 int32 are the
+    counters (include/b200ocl.h)."""
+    return _workspace(_native.lib().b200ocl_snapshot_workspace_bytes(int(n_segments)), device)
+
+
+def _snapshot_call(name, table, n, staging, workspace):
+    _need_cuda(table, staging, workspace)
+    if table.dtype != torch.uint8 or table.numel() != n * SNAP_SEGMENT.itemsize:
+        raise ValueError('the segment table must be %d uint8 records of %d bytes' % (n, SNAP_SEGMENT.itemsize))
+    rc = getattr(_native.lib(), name)(_ptr(table), int(n), _ptr(staging), staging.numel() * staging.element_size(),
+                                      _ptr(workspace), workspace.numel(), _stream())
+    _native.check(rc, name)
+
+
+def snapshot_pack(table, n, staging, workspace):
+    """Copy (B200OCL_SNAP_COPY) or encode (B200OCL_SNAP_U8) the n segments of `table` (a device uint8 tensor of
+    SNAP_SEGMENT records) into `staging`, on the current stream; workspace[:4 * (n + 1)] gets the counters.  Nothing
+    is read back."""
+    _snapshot_call('b200ocl_snapshot_pack', table, n, staging, workspace)
+
+
+def snapshot_unpack(table, n, staging, workspace):
+    """The inverse of snapshot_pack: each segment's region of `staging`, in the form its kind names, to its ptr."""
+    _snapshot_call('b200ocl_snapshot_unpack', table, n, staging, workspace)

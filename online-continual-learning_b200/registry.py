@@ -28,6 +28,10 @@ changes nothing.
 With B200OCL_CHECKPOINT_DIR (a directory) install() replaces the same two drivers whatever R is, so that an
 interrupted experiment resumes from its last finished task (checkpoint.py).  Parity mode and data-parallel gradient sync
 are refused with ValueError before anything is replaced.  Unset or empty changes nothing.
+
+With B200OCL_CHECKPOINT_ASYNC=1 as well, the snapshots are staged on the device and written behind the runs
+(checkpoint.py).  Unset, empty or 0 changes nothing; any other value, or 1 without a checkpoint directory, raises
+ValueError in install() before anything is replaced.
 """
 from .learners import AGEM, EWC_pp, ExperienceReplay, Gdumb, Icarl, Lwf, SupContrastReplay
 from .retrieve import ASER_retrieve, MIR_retrieve, Random_retrieve
@@ -78,6 +82,7 @@ def install(reference_name_match=None, extra=()):
     multirun.check_concurrent(n_concurrent, devices=devices)
     directory = checkpoint.checkpoint_dir()
     checkpoint.check_checkpoint(directory)
+    checkpoint.checkpoint_async()
     if reference_name_match is None:
         reference_name_match = importlib.import_module('utils.name_match')
     nm = reference_name_match

@@ -199,9 +199,13 @@ class GSSGreedyUpdate(object):
         self.last_batch_sim = None        # kept for inspection (tests: near-zero decisions)
         self.last_replaced = None
 
+    def snapshot_parts(self):
+        """The score of every slot, on the device."""
+        return {'buffer_score': self.buffer_score}
+
     def snapshot(self):
-        """The score of every slot, on the host (the buffer's snapshot() synchronised the stream)."""
-        return {'buffer_score': self.buffer_score.to('cpu')}
+        """The score of every slot, on the host."""
+        return memory.host_tree(self.snapshot_parts())
 
     def restore(self, state):
         self.buffer_score.copy_(state['buffer_score'])
