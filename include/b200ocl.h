@@ -495,6 +495,17 @@ int b200ocl_icarl_loss(const float* logits, const float* teacher, const int64_t*
                        int pos_len, int N, int n_stream, int C, int K, int n_old, float* loss, float* dlogits,
                        int* err_flag, void* stream);
 
+/* DER++'s logit-matching term (Buzzega et al., NeurIPS 2020) over the logits z [n,C] of a memory batch and the logit
+ * memory mem [mem_rows,C], read in place through the int64 slot indices idx [n] (repeats allowed):
+ *   loss[1] = alpha * sum (z - mem[idx])^2 / (n*C)      (alpha * F.mse_loss(z, mem[idx]), reduction 'mean'),
+ *   dz [n,C] = alpha * 2 (z - mem[idx]) / (n*C).
+ * Each difference and gradient element is formed in double and rounded once; the squares are summed in double in a
+ * fixed order, with no atomics, so repeated launches are bit-identical.  One launch (one CTA) for every n >= 1, C >= 1.
+ * A slot outside [0, mem_rows) sets *err_flag = 1 (nullable, never cleared): its row gets a zero gradient and adds
+ * nothing to the loss (which still divides by n*C).  B200OCL_EINVAL for a null z, mem, idx, loss or dz, or a size < 1. */
+int b200ocl_logit_mse(const float* z, const float* mem, int mem_rows, const int64_t* idx, int n, int C, double alpha,
+                      float* loss, float* dz, int* err_flag, void* stream);
+
 /* ---------------------------------------------------------------- SCR augmentation
  * The second view of agents/scr.py:18-24,54 (kornia RandomResizedCrop -> RandomHorizontalFlip ->
  * ColorJitter -> RandomGrayscale) in one kernel over NCHW fp32 images in [0,1].

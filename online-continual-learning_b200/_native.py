@@ -2,7 +2,7 @@
 is missing -- there is no fallback path."""
 import ctypes
 import os
-from ctypes import c_char_p, c_float, c_int, c_int64, c_size_t, c_uint64, c_void_p
+from ctypes import c_char_p, c_double, c_float, c_int, c_int64, c_size_t, c_uint64, c_void_p
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, 'libb200ocl.so')
@@ -67,6 +67,7 @@ SIGNATURES = {
     'b200ocl_cls_loss': (c_int, [P, P, c_int, c_int, c_int, P, c_int, c_int, P, c_int, P, c_float, c_float, P, P, P, P,
                                  P]),
     'b200ocl_icarl_loss': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, P, P, P, P]),
+    'b200ocl_logit_mse': (c_int, [P, P, c_int, P, c_int, c_int, c_double, P, P, P, P]),
     'b200ocl_scr_augment': (c_int, [P, P, P, c_int, c_int, c_int, P]),
     'b200ocl_aser_replace': (c_int, [P, c_int, c_int, P, P, P, c_int, c_size_t, P, P, P, P]),
     'b200ocl_conv_selftest_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int, c_int]),

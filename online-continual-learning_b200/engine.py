@@ -605,6 +605,27 @@ def ce_loss(logits, labels, want_grad=True, want_per_sample=False, want_correct=
     return out
 
 
+def logit_mse(logits, memory, idx, alpha, err=None):
+    """DER++'s logit term (b200ocl_logit_mse): alpha * F.mse_loss(logits, memory[idx]) for logits [n,C], the logit
+    memory [mem,C] and int64 slot indices idx [n] (read in place, no gather); returns dict(loss[1], dlogits).  err: int32
+    device flag [1] set to 1 by a slot outside the memory; such a row has zero dlogits and adds nothing to loss."""
+    _need_cuda(logits, memory, idx, err)
+    logits = logits.detach().to(torch.float32).contiguous()
+    idx = idx.detach().to(torch.int64).contiguous().reshape(-1)
+    n, c = logits.shape
+    if memory.dtype != torch.float32 or not memory.is_contiguous() or memory.dim() != 2 or memory.shape[1] != c:
+        raise ValueError('the logit memory must be a contiguous fp32 [mem, %d] tensor, got %s %s'
+                         % (c, memory.dtype, tuple(memory.shape)))
+    if idx.numel() != n:
+        raise ValueError('idx must hold one slot per logits row: got %d for %d rows' % (idx.numel(), n))
+    out = {'loss': torch.empty(1, dtype=torch.float32, device=logits.device), 'dlogits': torch.empty_like(logits)}
+    rc = _lib().b200ocl_logit_mse(logits.data_ptr(), memory.data_ptr(), memory.shape[0], idx.data_ptr(), n, c,
+                                  float(alpha), out['loss'].data_ptr(), out['dlogits'].data_ptr(),
+                                  0 if err is None else err.data_ptr(), _stream())
+    _native.check(rc, 'b200ocl_logit_mse')
+    return out
+
+
 CLS_MODES = {'ce': 0, 'labels_trick': 1, 'separated_softmax': 2}
 
 

@@ -1,9 +1,10 @@
 """Agents of the replay path with the reference surface `cls(model, opt, params)`,
 `.train_learner(x_train, y_train)`, `.evaluate(test_loaders)`:
 ExperienceReplay (agents/exp_replay.py:10-104: ER / MIR / ASER), SupContrastReplay (agents/scr.py:11-69), AGEM
-(agents/agem.py), Lwf (agents/lwf.py), Icarl (agents/icarl.py), Gdumb (agents/gdumb.py) and EWC_pp (agents/ewc_pp.py, registered
-only on request: registry.extra_agents), over ContinualLearner (agents/base.py:14-113) with its training tricks (labels
-trick, separated softmax, kd_trick / kd_trick_star, review trick).
+(agents/agem.py), Lwf (agents/lwf.py), Icarl (agents/icarl.py), Gdumb (agents/gdumb.py), and EWC_pp (agents/ewc_pp.py)
+and DERPP (DER++, which the reference lacks), both registered only on request (registry.extra_agents), over
+ContinualLearner (agents/base.py:14-113) with its training tricks (labels trick, separated softmax, kd_trick /
+kd_trick_star, review trick).
 
 The loop structure, the order of train-mode forwards (they move BN running statistics) and the
 order of buffer operations follow the reference step exactly; what changes is who does the
@@ -20,7 +21,7 @@ import torch
 
 from . import memory, nets, ops
 from .augment import SCRTransform
-from .engine import ce_loss, cls_loss, icarl_loss
+from .engine import ce_loss, cls_loss, icarl_loss, logit_mse
 from .memory import Buffer, input_size_match
 from .nets import adopt, engine_of, EngineModel
 
@@ -1129,6 +1130,115 @@ class Gdumb(ContinualLearner):
         yield from self._train_mem_steps()                                                     # :49
         self._raise_label_errors()
         yield from _after_train_steps(self)                                                   # :50
+
+
+def der_weights(params):
+    """(der_alpha, der_beta) of params as floats: each must be present, finite and >= 0 (ValueError otherwise; there is
+    no default)."""
+    out = []
+    for name in ('der_alpha', 'der_beta'):
+        v = getattr(params, name, None)
+        if v is None or isinstance(v, bool):
+            raise ValueError('DER++ needs params.%s (a finite number >= 0), got %r' % (name, v))
+        try:
+            f = float(v)
+        except (TypeError, ValueError):
+            raise ValueError('DER++ needs params.%s (a finite number >= 0), got %r' % (name, v)) from None
+        if not math.isfinite(f) or f < 0:
+            raise ValueError('DER++ needs params.%s (a finite number >= 0), got %r' % (name, v))
+        out.append(f)
+    return tuple(out)
+
+
+class DERPP(ContinualLearner):
+    """DER++ (Buzzega et al., NeurIPS 2020, online and without augmentation) on the engine; DER when der_beta = 0.  Each
+    slot of the reservoir memory (memory.LogitBuffer) also keeps the logits the network gave the sample when it was
+    stored.  Per stream batch (x, y), mem_iters times:
+      1. the stream forward z_s, mean CE at y, backward into the gradient arena (ER's stream half);
+      2. when der_alpha != 0: a uniform draw idx1 of eps_mem_batch filled slots (memory.random_retrieve, ER's numpy
+         draw), their forward z1, der_alpha * mean((z1 - L[idx1])^2) (b200ocl_logit_mse, targets read in place), an
+         accumulating backward;
+      3. when der_beta != 0: a second, independent draw idx2, its forward, der_beta * CE at the stored labels, an
+         accumulating backward;
+      4. one optimizer step (SGD or Adam).
+    An empty draw skips its term's passes.  The BN running statistics move in the order stream, mem1, mem2.  Then one
+    reservoir update of (x, y) writes, for every slot it fills, the fp32 row of the last iteration's z_s.  With
+    der_alpha = 0 and der_beta = 1 every draw and every result bit is ER's (random retrieval, reservoir update).
+    Evaluation is the inherited arg-max path."""
+
+    def __init__(self, model, opt, params):
+        if params.update != 'random' or params.retrieve != 'random':
+            raise NotImplementedError('DER++ keeps each slot\'s logits beside it through the reservoir update and the '
+                                      'random retrieval (update=random, retrieve=random), not update=%r, retrieve=%r'
+                                      % (params.update, params.retrieve))
+        trick = getattr(params, 'trick', None) or {}
+        on = [k for k in ('labels_trick', 'separated_softmax', 'kd_trick', 'kd_trick_star') if trick.get(k)]
+        if on:
+            raise NotImplementedError('DER++ runs with plain cross-entropy; %s not implemented' % ', '.join(on))
+        alpha, beta = der_weights(params)
+        super().__init__(model, opt, params)
+        self.der_alpha, self.der_beta = alpha, beta
+        self.buffer = memory.LogitBuffer(model, params, self.engine.out_dim)
+        self.mem_size = params.mem_size
+        self.eps_mem_batch = params.eps_mem_batch
+        self.mem_iters = params.mem_iters
+
+    def replay_step(self, batch_x, batch_y, batch_y_host, meters=None):
+        if self.grad_sync is not None:
+            raise NotImplementedError('data-parallel DER++: the logit memory is not kept consistent across ranks')
+        eng = self.engine
+        spec = self._optimizer()
+        for _ in range(self.mem_iters):
+            logits, ws = eng.forward_train(batch_x, slot=0)                          # 1. stream (BN stats move)
+            ce = self.criterion(logits, batch_y, want_correct=meters is not None)
+            if meters is not None:
+                meters['acc_batch'].update(ce['n_correct'] / batch_y.size(0), batch_y.size(0))
+                meters['losses_batch'].update(ce['loss'], batch_y.size(0))
+            eng.backward(batch_x, ce['dlogits'], ws)
+            self.last_loss_logit = self.last_loss_mem = None
+            if self.der_alpha != 0.0:                                                # 2. logit term
+                mem_x, _, idx = memory.random_retrieve(self.buffer, self.eps_mem_batch, return_indices=True)
+                if mem_x.size(0) > 0:
+                    z1, ws1 = eng.forward_train(mem_x, slot=1)
+                    lm = logit_mse(z1, self.buffer.buffer_logits, idx, self.der_alpha)
+                    eng.backward(mem_x, lm['dlogits'], ws1, accumulate=True)
+                    self.last_loss_logit = lm['loss']
+                    if meters is not None:
+                        meters['losses_logit'].update(lm['loss'], mem_x.size(0))
+            if self.der_beta != 0.0:                                                 # 3. memory CE term
+                mem_x, mem_y, _ = memory.random_retrieve(self.buffer, self.eps_mem_batch, return_indices=True)
+                if mem_x.size(0) > 0:
+                    z2, ws2 = eng.forward_train(mem_x, slot=1)
+                    ce_m = self.criterion(z2, mem_y, w_ce=self.der_beta, want_correct=meters is not None)
+                    eng.backward(mem_x, ce_m['dlogits'], ws2, accumulate=True)
+                    self.last_loss_mem = ce_m['loss']
+                    if meters is not None:
+                        meters['losses_mem'].update(ce_m['loss'], mem_y.size(0))
+                        meters['acc_mem'].update(ce_m['n_correct'] / mem_y.size(0), mem_y.size(0))
+            self.last_loss = ce['loss']
+            self._optimizer_step(spec)                                               # 4.
+        self.buffer.update(batch_x, batch_y, logits=logits, y_host=batch_y_host)     # z_s of the last iteration
+        self._throttle()
+
+    def _steps(self, x_train, y_train):
+        self._begin_call()
+        self.before_train(x_train, y_train)
+        self.engine.pack()          # the caller may have written the Parameters (load_state_dict, weight surgery)
+        self.model = self.model.train()
+        meters = {k: AverageMeter() for k in ('losses_batch', 'losses_logit', 'losses_mem', 'acc_batch', 'acc_mem')}
+        for ep in range(self.epoch):
+            stream = StreamFeeder(x_train, y_train, self.batch, self.device)   # DataLoader(shuffle=True): new order per epoch
+            for i, (batch_x, batch_y, y_host) in enumerate(stream):
+                self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
+                yield
+                if i % 100 == 1 and self.verbose:
+                    print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
+                          .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
+                    print('==>>> it: {}, mem logit loss: {:.6f}, mem avg. loss: {:.6f}, running mem acc: {:.3f}'
+                          .format(i, meters['losses_logit'].avg(), meters['losses_mem'].avg(), meters['acc_mem'].avg()))
+        self._raise_label_errors()
+        yield from _after_train_steps(self)
+        self._end_call()
 
 
 def ewc_ema_schedule(n_batches, epochs, fisher_update_after):

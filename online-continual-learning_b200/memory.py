@@ -695,3 +695,70 @@ class Buffer(torch.nn.Module):
             self.buffer_img[idx_t] = x_rows
             self.buffer_label[idx_t] = y_rows
         self.labels_host[slots_host] = np.asarray(y_host, dtype=np.int64)
+
+
+class LogitBuffer(Buffer):
+    """DER++'s memory: a Buffer whose slots also keep buffer_logits [mem_size, out_dim] fp32, the logits the network gave
+    each stored sample.  update(x, y, logits=...) is the reservoir update of Reservoir_update, with the same
+    update.reservoir_draws / reservoir_plan calls, and writes each chosen stream row's logits beside its image and label.
+    Retrieval is the inherited random one; the learner reads the logits of the slots it drew."""
+
+    def __init__(self, model, params, out_dim, update_methods=None, retrieve_methods=None):
+        super().__init__(model, params, update_methods, retrieve_methods)
+        self.register_buffer('buffer_logits', torch.zeros((params.mem_size, int(out_dim)), dtype=torch.float32,
+                                                          device=self.buffer_img.device))
+
+    def update(self, x, y, logits=None, **kwargs):
+        """The reservoir update of (x, y) (Reservoir_update.update) with buffer_logits[slot] = logits[row] for every row
+        it stores.  Returns the slots written by the reservoir draws, as Reservoir_update does."""
+        from . import update as _update
+        if logits is None or logits.shape != (x.size(0), self.buffer_logits.shape[1]):
+            raise ValueError('LogitBuffer.update needs the [%d, %d] logits of the stream rows'
+                             % (x.size(0), self.buffer_logits.shape[1]))
+        y_host = _update._host_labels(y, kwargs)
+        batch_size = x.size(0)
+        mem = self.buffer_img.size(0)
+        place_left = max(0, mem - self.current_index)
+        if place_left:
+            offset = min(place_left, batch_size)
+            s, e = self.current_index, self.current_index + offset
+            self.buffer_img[s:e].copy_(x[:offset])
+            self.buffer_label[s:e].copy_(y[:offset])
+            self.buffer_logits[s:e].copy_(logits[:offset])
+            self.labels_host[s:e] = y_host[:offset]
+            self.current_index += offset
+            self.n_seen_so_far += offset
+            if offset == batch_size:
+                return list(range(s, e))
+        x, y, y_host, logits = x[place_left:], y[place_left:], y_host[place_left:], logits[place_left:]
+        draws = _update.reservoir_draws(x.size(0), self.n_seen_so_far, x.device)
+        self.last_draws = draws
+        self.n_seen_so_far += x.size(0)
+        slots, src = _update.reservoir_plan(draws, mem)
+        if not slots:
+            return []
+        src_t = to_device_i64(src, x.device)
+        if x.is_cuda:
+            self.write(slots, ops.gather_rows(x, src_t), ops.gather_rows(y, src_t), y_host[src])
+            ops.scatter_rows(self.buffer_logits, to_device_i64(slots, x.device), ops.gather_rows(logits, src_t))
+        else:
+            self.write(slots, x[src_t], y[src_t], y_host[src])
+            self.buffer_logits[torch.as_tensor(slots)] = logits[src_t]
+        return slots
+
+    def snapshot_parts(self):
+        """Buffer.snapshot_parts() plus the filled logit rows, on the device, kept as fp32."""
+        out = super().snapshot_parts()
+        out['logits'] = self.buffer_logits[:self.current_index]
+        return out
+
+    def snapshot_capacity(self):
+        return super().snapshot_capacity() + self.buffer_logits.numel() * self.buffer_logits.element_size()
+
+    def restore(self, state):
+        super().restore(state)
+        n = int(state['current_index'])
+        if tuple(state['logits'].shape) != (n, self.buffer_logits.shape[1]):
+            raise ValueError('snapshot logits %s do not fit %s' % (tuple(state['logits'].shape),
+                                                                    tuple(self.buffer_logits.shape)))
+        self.buffer_logits[:n].copy_(state['logits'])
