@@ -540,6 +540,14 @@ int b200ocl_conv_selftest_geom(int N, int H, int W, int cin, int cout, int ks, i
 int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N, int H, int W, int cin, int cout,
                           int ks, int stride, int dgrad, int path, int mode, float* stats_out, void* workspace,
                           size_t workspace_bytes, void* stream);
+/* The eval forward of one 3x3 stride-1 C -> C convolution through a chosen path (as b200ocl_conv_selftest: 0 automatic,
+ * 1 CUDA-core kernels, 2 conv_tc.cu, 3 conv_tcp.cu) with the epilogue's inputs given separately, as the network's
+ * eval pass gives them: out = (conv - mean) * gamma / sqrt(var + eps) + beta with bn[4*C] = mean, var, gamma, beta;
+ * plus residual[N,H,W,C] when residual is not null (a buffer other than x, like a block's input); then ReLU when
+ * relu != 0.  The workspace is b200ocl_conv_selftest_workspace_bytes(N, C, C, H, W, 3, 1). */
+int b200ocl_conv_selftest_eval(const float* x, const float* w_oihw, const float* bn, const float* residual, int relu,
+                               float* out, int N, int H, int W, int C, int path, void* workspace, size_t workspace_bytes,
+                               void* stream);
 
 /* Window variant: A is read in place from a larger swizzled buffer P[rows][32] of 128-byte rows (tile row
  * 8g + r = P row start_row + g * sbo_rows + r), start address unaligned to the swizzle repeat when
@@ -552,6 +560,22 @@ int b200ocl_selftest_umma_window(const float* P, const float* B, float* D, int r
  * dw in OIHW: the cuDNN weight-gradient call behind loss.backward() for nn.Conv2d (models/resnet.py:11-12).  Exists so
  * that tests can pin the kernel against a reference; B200OCL_EUNSUPPORTED when the geometry is not covered. */
 size_t b200ocl_wgrad_tc_selftest_workspace_bytes(int N, int H, int W, int cin, int cout);
+typedef struct {
+  int eligible;         /* the kernel covers the geometry; the fields below are 0 otherwise */
+  int slices;           /* CTA columns: 20-channel slices of the activation */
+  int cout_blocks;      /* CTA layers: blocks of at most 40 output channels */
+  int bn;               /* MMA N of a block */
+  int tiles;            /* 128-position tiles of the zero-padded strip */
+  int tpc;              /* tiles per tensor-core accumulation chain */
+  int chains;           /* partials per (slice, block) */
+  int chains_per_cta;   /* chains one CTA walks: ceil(chains / CTAs), made even when above 1 */
+  int ctas_x;           /* CTAs per (slice, block) */
+  int sm_share;         /* sms / (slices * cout_blocks): the CTAs per (slice, block) the SM count allows */
+  int sms;
+} b200ocl_wgrad_tc_geom;
+/* Host only: the launch b200ocl_wgrad_tc_selftest makes for these arguments on a GPU with sms SMs (0: the current
+ * device). */
+int b200ocl_wgrad_tc_selftest_geom(int N, int H, int W, int cin, int cout, int sms, b200ocl_wgrad_tc_geom* out);
 int b200ocl_wgrad_tc_selftest(const float* x, const float* dz, float* dw_oihw, int N, int H, int W, int cin, int cout,
                               void* workspace, size_t workspace_bytes, void* stream);
 

@@ -74,9 +74,11 @@ SIGNATURES = {
     'b200ocl_conv_selftest_geom': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                            P]),
     'b200ocl_conv_selftest': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P, P, c_size_t, P]),
+    'b200ocl_conv_selftest_eval': (c_int, [P, P, P, P, c_int, P, c_int, c_int, c_int, c_int, c_int, P, c_size_t, P]),
     'b200ocl_selftest_umma_tf32': (c_int, [P, P, P, c_int, c_int, c_int, P, P]),
     'b200ocl_selftest_umma_window': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, P, P]),
     'b200ocl_wgrad_tc_selftest_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    'b200ocl_wgrad_tc_selftest_geom': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, P]),
     'b200ocl_wgrad_tc_selftest': (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, P, c_size_t, P]),
     'b200ocl_snapshot_workspace_bytes': (c_size_t, [c_int]),
     'b200ocl_snapshot_pack': (c_int, [P, c_int, P, c_size_t, P, c_size_t, P]),

@@ -885,19 +885,12 @@ int b200ocl_conv_selftest_geom(int N, int H, int W, int cin, int cout, int ks, i
   return B200OCL_OK;
 }
 
-int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N, int H, int W, int cin, int cout,
-                          int ks, int stride, int dgrad, int path, int mode, float* stats_out, void* workspace,
-                          size_t workspace_bytes, void* stream_) {
+// The self-test's launch once its arguments are checked: pack the weights into the workspace, then one convolution.
+// In eval mode (3, 4) stats holds mean, var, gamma, beta and is only read; residual and relu are the epilogue's.
+static int selftest_run(const float* x, const float* w_oihw, float* out, int N, int H, int W, int cin, int cout, int ks,
+                        int stride, int dgrad, int path, int mode, float* stats_out, const float* residual, int relu,
+                        void* workspace, cudaStream_t stream) {
   using namespace b200ocl;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  B200OCL_CHECK_ARG(x && w_oihw && out && workspace, "null pointer");
-  B200OCL_CHECK_ARG(N > 0 && H > 0 && W > 0 && cin % 20 == 0 && cout % 20 == 0 && cin > 0 && cout > 0, "bad shape");
-  B200OCL_CHECK_ARG(mode >= 0 && mode <= 4 && (mode != 2 || (stats_out && !dgrad)), "mode 2 (train) needs stats_out, forward only");
-  B200OCL_CHECK_ARG(mode < 3 || (stats_out && !dgrad && (mode == 3 || cin == cout)),
-                    "modes 3 / 4 (eval) need stats_out, forward only; mode 4 needs cin == cout");
-  B200OCL_CHECK_ARG((ks == 3 || ks == 1) && (stride == 1 || stride == 2) && (!dgrad || (ks == 3 && stride == 1)),
-                    "3x3 or 1x1, stride 1 or 2; data gradient for 3x3 stride 1 only");
-  B200OCL_CHECK_ARG(workspace_bytes >= b200ocl_conv_selftest_workspace_bytes(N, cin, cout, H, W, ks, stride), "workspace too small");
   NetPlan p;
   memset(&p, 0, sizeof(p));
   p.n_conv = 1;
@@ -930,10 +923,38 @@ int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N
     a.rvar = stats_out + cout;
     a.gamma = stats_out + 2 * cout;
     a.beta = stats_out + 3 * cout;
-    a.residual = mode == 4 ? x : nullptr;
-    a.relu = mode == 4;
+    a.residual = residual;
+    a.relu = relu;
   }
   return launch_conv(a, sms, stream);
+}
+
+int b200ocl_conv_selftest(const float* x, const float* w_oihw, float* out, int N, int H, int W, int cin, int cout,
+                          int ks, int stride, int dgrad, int path, int mode, float* stats_out, void* workspace,
+                          size_t workspace_bytes, void* stream_) {
+  using namespace b200ocl;
+  B200OCL_CHECK_ARG(x && w_oihw && out && workspace, "null pointer");
+  B200OCL_CHECK_ARG(N > 0 && H > 0 && W > 0 && cin % 20 == 0 && cout % 20 == 0 && cin > 0 && cout > 0, "bad shape");
+  B200OCL_CHECK_ARG(mode >= 0 && mode <= 4 && (mode != 2 || (stats_out && !dgrad)), "mode 2 (train) needs stats_out, forward only");
+  B200OCL_CHECK_ARG(mode < 3 || (stats_out && !dgrad && (mode == 3 || cin == cout)),
+                    "modes 3 / 4 (eval) need stats_out, forward only; mode 4 needs cin == cout");
+  B200OCL_CHECK_ARG((ks == 3 || ks == 1) && (stride == 1 || stride == 2) && (!dgrad || (ks == 3 && stride == 1)),
+                    "3x3 or 1x1, stride 1 or 2; data gradient for 3x3 stride 1 only");
+  B200OCL_CHECK_ARG(workspace_bytes >= b200ocl_conv_selftest_workspace_bytes(N, cin, cout, H, W, ks, stride), "workspace too small");
+  return selftest_run(x, w_oihw, out, N, H, W, cin, cout, ks, stride, dgrad, path, mode, stats_out,
+                      mode == 4 ? x : nullptr, mode == 4, workspace, static_cast<cudaStream_t>(stream_));
+}
+
+int b200ocl_conv_selftest_eval(const float* x, const float* w_oihw, const float* bn, const float* residual, int relu,
+                               float* out, int N, int H, int W, int C, int path, void* workspace, size_t workspace_bytes,
+                               void* stream_) {
+  using namespace b200ocl;
+  B200OCL_CHECK_ARG(x && w_oihw && bn && out && workspace, "null pointer");
+  B200OCL_CHECK_ARG(N > 0 && H > 0 && W > 0 && C % 20 == 0 && C > 0, "bad shape");
+  B200OCL_CHECK_ARG(workspace_bytes >= b200ocl_conv_selftest_workspace_bytes(N, C, C, H, W, 3, 1), "workspace too small");
+  // eval mode only reads the BatchNorm block
+  return selftest_run(x, w_oihw, out, N, H, W, C, C, 3, 1, 0, path, 3, const_cast<float*>(bn), residual, relu != 0,
+                      workspace, static_cast<cudaStream_t>(stream_));
 }
 
 size_t b200ocl_net_eval_workspace_bytes(const b200ocl_net_desc* desc, int N) {

@@ -329,6 +329,22 @@ extern "C" size_t b200ocl_wgrad_tc_selftest_workspace_bytes(int N, int H, int W,
   return align_up((size_t)g.chains * 9 * cin * cout * sizeof(float), 256);
 }
 
+extern "C" int b200ocl_wgrad_tc_selftest_geom(int N, int H, int W, int cin, int cout, int sms, b200ocl_wgrad_tc_geom* out) {
+  using namespace b200ocl;
+  B200OCL_CHECK_ARG(out && N >= 1 && H >= 1 && W >= 1 && cin >= 1 && cout >= 1 && sms >= 0, "null pointer / bad shape");
+  if (sms == 0) sms = sm_count();
+  const WgradTcCfg g = wgrad_tc_cfg(N, H, W, 3, 1, 1, cin, cout, sms);
+  *out = b200ocl_wgrad_tc_geom{};
+  out->eligible = g.eligible;
+  out->sms = sms;
+  if (!g.eligible) return B200OCL_OK;
+  out->slices = g.slices; out->cout_blocks = g.cout_blocks; out->bn = g.bn;
+  out->tiles = g.tiles; out->tpc = g.tpc; out->chains = g.chains;
+  out->chains_per_cta = g.chains_per_cta; out->ctas_x = g.ctas_x;
+  out->sm_share = sms / (g.slices * g.cout_blocks);
+  return B200OCL_OK;
+}
+
 extern "C" int b200ocl_wgrad_tc_selftest(const float* x, const float* dz, float* dw_oihw, int N, int H, int W, int cin, int cout,
                                          void* workspace, size_t workspace_bytes, void* stream_) {
   using namespace b200ocl;

@@ -103,6 +103,21 @@ def conv_selftest_geom(n, h, w, cin, cout, ks, stride, dgrad, path, mode, sms=0)
     return out
 
 
+class WgradTcGeom(ctypes.Structure):
+    """b200ocl_wgrad_tc_geom: the grid of the wgmma weight gradient and how it splits the strip's tiles into chains."""
+    _fields_ = [('eligible', c_int), ('slices', c_int), ('cout_blocks', c_int), ('bn', c_int), ('tiles', c_int),
+                ('tpc', c_int), ('chains', c_int), ('chains_per_cta', c_int), ('ctas_x', c_int), ('sm_share', c_int),
+                ('sms', c_int)]
+
+
+def wgrad_tc_selftest_geom(n, h, w, cin, cout, sms=0):
+    """Host-only test hook (b200ocl_wgrad_tc_selftest_geom): the launch b200ocl_wgrad_tc_selftest makes."""
+    out = WgradTcGeom()
+    _native.check(_lib().b200ocl_wgrad_tc_selftest_geom(int(n), int(h), int(w), int(cin), int(cout), int(sms),
+                                                        ctypes.byref(out)), 'b200ocl_wgrad_tc_selftest_geom')
+    return out
+
+
 def describe(in_hw, num_classes, head=None, feat_dim=128, nf=20):
     """Host-only: arena sizes and tensor table for a network description (no GPU needed)."""
     desc = NetDesc(int(in_hw), int(in_hw), int(nf), int(num_classes), HEAD_CODES[head], int(feat_dim))
