@@ -165,6 +165,11 @@ int b200ocl_linear_argmax_ea(const float* feats, int B, int d, const float* weig
                              uint64_t* n_correct, int64_t* pred_task, double* set_sums, uint64_t* counts, void* stream);
 int b200ocl_rows_mean(const float* weight, const float* bias, int C, int d, const int64_t* rows, int n, float* out,
                       void* stream);
+/* PCR's evaluation (Lin et al., CVPR 2023): pred[b] = arg-max_c <f_b / (||f_b|| + eps), w_c / (||w_c|| + eps)>, eps =
+ * 1e-6, over the C rows of weight (the classifier's; no bias); the first maximum wins.  *n_correct += #(pred == truth).
+ * The classify body of b200ocl_linear_argmax, one warp per row; truth, pred and n_correct nullable. */
+int b200ocl_cosine_argmax(const float* feats, int B, int d, const float* weight, int C, const int64_t* truth,
+                          int64_t* pred, uint64_t* n_correct, void* stream);
 
 /* The network's linear layer on its own: y [N,out] = x [N,in] . W[out,in]^T + b (relu != 0: then ReLU), the kernel the
  * classifier and projection heads run.  Each output sums its lane-strided products in a fixed order (no atomics).
@@ -338,6 +343,9 @@ int b200ocl_net_apply_running_stats(const b200ocl_net_desc* desc, const b200ocl_
 /* loss.backward() for the forward kept in `workspace` (same x): dout [N,out_dim] -> st->grads
  * (overwritten, or added to when accumulate != 0 -- exp_replay.py:55,77 accumulate two
  * backward passes before one opt.step()).  accumulate bit 1 (value 2): the forward was b200ocl_net_forward_evalgrad.
+ * accumulate bit 2 (value 4): the pass starts from the encoder features: dout is dL/dfeatures [N,dim_in] (the `feat` the
+ * forward kept, b200ocl_net_train_ws_layout), the head's backward is skipped and the head's gradient entries are left as
+ * they are; bit 0 still selects overwriting or adding for every other entry (PCR's loss writes the classifier's own).
  * The weight-gradient launches run on a helper stream that is forked from / joined into `stream` with events (captured
  * as parallel branches when `stream` is being captured into a CUDA graph); the helper stream and its four events (one set per
  * caller stream, at most four caller streams per device) are the one piece of state the library creates itself, on the first call (B200OCL_WG_ASYNC=0: everything on `stream`). */
@@ -505,6 +513,26 @@ int b200ocl_icarl_loss(const float* logits, const float* teacher, const int64_t*
  * nothing to the loss (which still divides by n*C).  B200OCL_EINVAL for a null z, mem, idx, loss or dz, or a size < 1. */
 int b200ocl_logit_mse(const float* z, const float* mem, int mem_rows, const int64_t* idx, int n, int C, double alpha,
                       float* loss, float* dz, int* err_flag, void* stream);
+
+/* PCR's proxy-contrastive loss (Lin et al., CVPR 2023) over features F [R,d] with labels [R] (int64) and the proxies, the
+ * classifier weight W [C,d]; eps = 1e-6, tau = temperature:
+ *   u_i = F_i / (||F_i|| + eps),  v_c = W_c / (||W_c|| + eps),  g_ic = <u_i, v_c> / tau,
+ *   n_c = #rows labelled c,  m_ic = n_c - [c = y_i],  Z_i = sum_c m_ic exp(g_ic),  l_i = log Z_i - g_{i,y_i},
+ *   loss[1] = (1/R) sum_i l_i.
+ * With p_ic = m_ic exp(g_ic) / Z_i: dL/du_i = (sum_c p_ic v_c - v_{y_i}) / (tau R) and dL/dv_c = sum_i (p_ic - [y_i = c])
+ * u_i / (tau R), each taken through its normalisation (dx = g / (n + eps) - x <x, g> / (n (n + eps)^2), the second term
+ * 0 at n = 0) into dfeats [R,d] and dproxies [C,d]; dbias [C] is zeroed (the bias never enters the loss).  dproxies and
+ * dbias are meant to be the classifier's slices of the gradient arena.  A row of dproxies whose class no row carries is
+ * exactly 0.  An anchor whose class occurs once has no positive pair: the loss is NaN (SupConLoss's 0/0, as in
+ * b200ocl_supcon) and its gradients keep only the log Z_i part.  A label outside [0, C) sets *err_flag = 1 (nullable,
+ * never cleared): its row adds nothing to the loss (which still divides by R), is not counted in n_c and gets a zero
+ * dfeats row.  Two launches, every reduction in a fixed order with no floating-point atomics: repeated calls are
+ * bit-identical on any GPU; no host synchronisation.  B200OCL_EINVAL for a null pointer, R < 2, d or C < 1, or a
+ * temperature that is not finite and positive; B200OCL_EUNSUPPORTED for R > 4096, d > 2560 or C > 1024. */
+size_t b200ocl_pcr_loss_workspace_bytes(int R, int C);
+int b200ocl_pcr_loss(const float* feats, const int64_t* labels, int R, int d, const float* proxies, int C,
+                     float temperature, float* loss, float* dfeats, float* dproxies, float* dbias, int* err_flag,
+                     void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------- SCR augmentation
  * The second view of agents/scr.py:18-24,54 (kornia RandomResizedCrop -> RandomHorizontalFlip ->

@@ -32,6 +32,7 @@ SIGNATURES = {
     'b200ocl_linear_argmax': (c_int, [P, c_int, c_int, P, P, c_int, P, P, P, P]),
     'b200ocl_linear_argmax_ea': (c_int, [P, c_int, c_int, P, P, c_int, P, P, P, P, P, P, P, P, P]),
     'b200ocl_rows_mean': (c_int, [P, P, c_int, c_int, P, c_int, P, P]),
+    'b200ocl_cosine_argmax': (c_int, [P, c_int, c_int, P, c_int, P, P, P, P]),
     'b200ocl_linear_fwd': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, P]),
     'b200ocl_agem_project_workspace_bytes': (c_size_t, []),
     'b200ocl_agem_project': (c_int, [P, P, P, c_size_t, P, P, c_size_t, P]),
@@ -68,6 +69,8 @@ SIGNATURES = {
                                  P]),
     'b200ocl_icarl_loss': (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, P, P, P, P]),
     'b200ocl_logit_mse': (c_int, [P, P, c_int, P, c_int, c_int, c_double, P, P, P, P]),
+    'b200ocl_pcr_loss_workspace_bytes': (c_size_t, [c_int, c_int]),
+    'b200ocl_pcr_loss': (c_int, [P, P, c_int, c_int, P, c_int, c_float, P, P, P, P, P, P, c_size_t, P]),
     'b200ocl_scr_augment': (c_int, [P, P, P, c_int, c_int, c_int, P]),
     'b200ocl_aser_replace': (c_int, [P, c_int, c_int, P, P, P, c_int, c_size_t, P, P, P, P]),
     'b200ocl_conv_selftest_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int, c_int]),

@@ -10,6 +10,7 @@
 //   ncm_classify      one warp per test sample: normalise, squared distance to every class mean with the
 //                     reference's (f - mu)^2 form, first arg-min, label lookup, correct count (integer atomic)
 //   linear_argmax     the non-NCM branch (base.py:172-175): arg-max of the classifier logits
+//   cosine_argmax     PCR's evaluation: arg-max of the cosine between the feature and each classifier row
 //   linear_argmax_ea  the same launch with the error analysis of base.py:144-226 (--error_analysis) riding along:
 //                     predicted task, per-row fp64 logit sums over the new / old class sets, wrong rows bucketed by
 //                     the set they were predicted into; rows_mean the classifier's weight / bias means over a row set
@@ -98,19 +99,21 @@ struct EaArgs {
 
 // NCM: score = squared distance, smaller wins.  LINEAR: score = -(f.w + b), so that one arg-min serves both.
 // EA (LINEAR only) adds the error-analysis outputs; the arg-max and the hit count run the same instructions either way.
-template <bool NCM, bool EA = false>
+// COS (LINEAR only, no bias): score = -<f / (||f|| + eps), w / (||w|| + eps)>, eps = 1e-6.
+template <bool NCM, bool EA = false, bool COS = false>
 __global__ void __launch_bounds__(256) classify_kernel(const float* __restrict__ feats, int B, int d,
                                                        const float* __restrict__ means, const float* __restrict__ bias, int K,
                                                        const long long* __restrict__ class_ids,
                                                        const long long* __restrict__ truth, long long* __restrict__ pred,
                                                        unsigned long long* __restrict__ n_correct, EaArgs ea = EaArgs()) {
   static_assert(!(NCM && EA), "the error analysis reads logits: linear branch only");
+  static_assert(!(COS && (NCM || EA)), "the cosine arg-max is a linear-branch form without the error analysis");
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (b >= B) return;
   const float* f = feats + (size_t)b * d;
   float inv = 1.f;
-  if (NCM) {
+  if (NCM || COS) {
     float ss = 0.f;
     for (int dd = lane; dd < d; dd += 32) ss = fmaf(f[dd], f[dd], ss);
     inv = sqrtf(warp_sum(ss));
@@ -120,17 +123,19 @@ __global__ void __launch_bounds__(256) classify_kernel(const float* __restrict__
   double sum_new = 0.0, sum_old = 0.0;
   for (int k = 0; k < K; ++k) {
     const float* mu = means + (size_t)k * d;
-    float s = 0.f;
+    float s = 0.f, ww = 0.f;
     for (int dd = lane; dd < d; dd += 32) {
       if (NCM) {
         const float df = f[dd] / inv - mu[dd];             // normalised feature (base.py:159-160) minus the mean
         s = fmaf(df, df, s);
       } else {
         s = fmaf(f[dd], mu[dd], s);
+        if (COS) ww = fmaf(mu[dd], mu[dd], ww);
       }
     }
     s = warp_sum(s);
-    if (!NCM) s = -(s + bias[k]);
+    if (COS) s = -((s / (inv + 1e-6f)) / (sqrtf(warp_sum(ww)) + 1e-6f));
+    else if (!NCM) s = -(s + bias[k]);
     if (EA) {                                              // -s is the logit f.w + b exactly
       const unsigned m = ea.sets[k];
       if (m & 1u) sum_new += (double)(-s);
@@ -238,6 +243,22 @@ int b200ocl_linear_argmax(const float* feats, int B, int d, const float* weight,
                                                           reinterpret_cast<const long long*>(truth),
                                                           reinterpret_cast<long long*>(pred),
                                                           reinterpret_cast<unsigned long long*>(n_correct));
+  B200OCL_LAUNCHED();
+  return B200OCL_OK;
+}
+
+int b200ocl_cosine_argmax(const float* feats, int B, int d, const float* weight, int C, const int64_t* truth,
+                          int64_t* pred, uint64_t* n_correct, void* stream_) {
+  using namespace b200ocl;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200OCL_CHECK_ARG(B >= 0 && d >= 1 && C >= 1, "need B >= 0, d >= 1, C >= 1");
+  if (B == 0) return B200OCL_OK;
+  B200OCL_CHECK_ARG(feats && weight, "null pointer");
+  B200OCL_PROF("ncm", 4.0 * B * (double)d + 8.0 * C * (double)d, stream);
+  classify_kernel<false, false, true><<<(B + 7) / 8, 256, 0, stream>>>(feats, B, d, weight, nullptr, C, nullptr,
+                                                                       reinterpret_cast<const long long*>(truth),
+                                                                       reinterpret_cast<long long*>(pred),
+                                                                       reinterpret_cast<unsigned long long*>(n_correct));
   B200OCL_LAUNCHED();
   return B200OCL_OK;
 }

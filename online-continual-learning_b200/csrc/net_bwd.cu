@@ -788,6 +788,7 @@ extern "C" int b200ocl_net_backward(const b200ocl_net_desc* desc, const b200ocl_
   if ((rc = check_workspace("b200ocl_net_backward", workspace, workspace_bytes,
                             b200ocl_net_train_workspace_bytes(desc, N)))) return rc;
   const int eval_stats = (accumulate >> 1) & 1;   // bit 1 of `accumulate`: backward of b200ocl_net_forward_evalgrad
+  const int from_feat = (accumulate >> 2) & 1;    // bit 2: dout is dL/dfeatures [N, dim_in]; the head is skipped
   accumulate &= 1;
   const int sms = sm_count();
   TrainWs w = train_ws(p, N, workspace, sms);
@@ -798,7 +799,10 @@ extern "C" int b200ocl_net_backward(const b200ocl_net_desc* desc, const b200ocl_
   const int C_last = desc->nf * 8;
 
   // ---- heads: dout -> dfeat
-  if (p.head == 0) {
+  const float* dfeat = from_feat ? dout : w.dfeat;
+  if (from_feat) {
+    // the head's gradient entries are left as they are
+  } else if (p.head == 0) {
     if ((rc = linear_backward(p.lin[0], st->params, st->grads, w.feat, dout, nullptr, w.dfeat, N, accumulate, stream))) return rc;
   } else {
     const float* pre = (p.head == 3) ? w.feat : w.proj;
@@ -820,7 +824,7 @@ extern "C" int b200ocl_net_backward(const b200ocl_net_desc* desc, const b200ocl_
     size_t blocks = (total + 255) / 256;
     if (blocks > (size_t)16 * sms) blocks = (size_t)16 * sms;
     B200OCL_PROF("pool", 8.0 * total, stream);
-    pool_bwd_kernel<<<(unsigned)blocks, 256, 0, stream>>>(w.dfeat, g0, N, p.final_h, p.final_w, C_last, p.pooled_h,
+    pool_bwd_kernel<<<(unsigned)blocks, 256, 0, stream>>>(dfeat, g0, N, p.final_h, p.final_w, C_last, p.pooled_h,
                                                           p.pooled_w);
     B200OCL_LAUNCHED();
   }

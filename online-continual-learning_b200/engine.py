@@ -215,6 +215,7 @@ class Engine:
         self._eval_ws = {}
         self._train_ws = {}
         self._graphs = {}
+        self._feat_off = {}
 
     # ------------------------------------------------------------------ state
     def param_views(self, shapes=None):
@@ -403,12 +404,23 @@ class Engine:
                 self._train_ws[key] = ws
         return ws
 
-    def forward_train(self, x, ws=None, state=None, slot=0, eval_stats=False, defer_stats=False, _tag='fwd'):
+    def train_features(self, ws, n):
+        """The encoder features [n, dim_in] the train-mode forward over n images left in its workspace ws
+        (b200ocl_net_train_ws_layout's `feat`): a view, overwritten by the next forward into ws."""
+        off = self._feat_off.get(n)
+        if off is None:
+            off = self._feat_off[n] = train_ws_layout(self.desc, n, 0).feat
+        return ws[off:off + n * self.dim_in * 4].view(torch.float32).view(n, self.dim_in)
+
+    def forward_train(self, x, ws=None, state=None, slot=0, eval_stats=False, defer_stats=False, features=False,
+                      _tag='fwd'):
         """model.train(); model.forward(x).  Returns (out [N,out_dim], workspace kept for backward).
         eval_stats=True: model.eval() forward that can be differentiated (running statistics, nothing updated).
         defer_stats=True: the BN running statistics are left alone; apply_running_stats(ws, N) moves them later (so that
         the train-mode passes of one step can run concurrently on different streams and still update the statistics in
-        the reference's order).  _tag: the graph key of a forward over another persistent state (the teacher's); other
+        the reference's order).  features=True: the same launches, returning the encoder features [N, dim_in] in place of
+        out, as train_features(ws, N) gives them (a view of the workspace; backward(..., features=True) starts from
+        their gradient).  _tag: the graph key of a forward over another persistent state (the teacher's); other
         forwards over a state= run eagerly."""
         x = self._x(x)
         n = x.shape[0]
@@ -434,10 +446,12 @@ class Engine:
                                                  [torch.empty((n, self.out_dim), dtype=torch.float32, device=x.device)])
             e.inputs[0].copy_(x)
             e.run(lambda: launch(e.inputs[0], e.outputs[0]))
+            if features:
+                return self.train_features(ws, n), ws
             return e.outputs[0].clone(), ws      # the static buffer is overwritten by the next call
         out = torch.empty((n, self.out_dim), dtype=torch.float32, device=x.device)
         launch(x, out)
-        return out, ws
+        return (self.train_features(ws, n) if features else out), ws
 
     def apply_running_stats(self, ws, n):
         """The running-statistics update of a forward_train(..., defer_stats=True) over n images kept in ws."""
@@ -461,15 +475,18 @@ class Engine:
         rc = _lib().b200ocl_sgd_step(g.data_ptr(), alt.data_ptr(), g.data_ptr(), g.numel(), -1.0, 0.0, _stream())
         _native.check(rc, 'b200ocl_sgd_step')
 
-    def backward(self, x, dout, ws, accumulate=False, eval_stats=False, alt=False):
+    def backward(self, x, dout, ws, accumulate=False, eval_stats=False, alt=False, features=False):
         """loss.backward() for the forward of the same x kept in ws; fills (or adds to) the grad arena.
-        eval_stats=True: the forward was forward_train(..., eval_stats=True).  alt=True: into the second arena."""
+        eval_stats=True: the forward was forward_train(..., eval_stats=True).  alt=True: into the second arena.
+        features=True: dout is the gradient of the encoder features [N, dim_in]; the head's backward is skipped and its
+        gradient entries (linear.* for the classifier network) are left as they are."""
         _need_cuda(dout)
         x = self._x(x)
         dout = dout.detach().to(torch.float32).contiguous()
         n = dout.shape[0]
-        if x.shape[0] != n or dout.shape[1] != self.out_dim:
-            raise ValueError('dout must be [N, out_dim] for the same N as x')
+        width = self.dim_in if features else self.out_dim
+        if x.shape[0] != n or dout.dim() != 2 or dout.shape[1] != width:
+            raise ValueError('dout must be [N, %s] for the same N as x' % ('dim_in' if features else 'out_dim'))
         if alt:
             self.alt_grads()
         st_c = self._alt[1] if alt else self.state.c
@@ -477,14 +494,15 @@ class Engine:
         def launch(xin, din):
             rc = _lib().b200ocl_net_backward(ctypes.byref(self.desc), ctypes.byref(st_c), xin.data_ptr(),
                                              din.data_ptr(), n, ws.data_ptr(), ws.numel(),
-                                             (1 if accumulate else 0) | (2 if eval_stats else 0), _stream())
+                                             (1 if accumulate else 0) | (2 if eval_stats else 0) |
+                                             (4 if features else 0), _stream())
             _native.check(rc, 'b200ocl_net_backward')
 
         slot = next((k[1] for k, w in self._train_ws.items() if w is ws and k[0] == n), None) if (_GRAPHS and not eval_stats) else None
         fwd = (self._graphs.get(('fwd', n, slot, False)) or self._graphs.get(('fwd', n, slot, True))) if slot is not None else None
         if fwd is not None:
             # the images are the static copy the graphed forward read (same data as x)
-            key = ('bwd', n, slot, bool(accumulate), bool(alt))
+            key = ('bwd_feat' if features else 'bwd', n, slot, bool(accumulate), bool(alt))
             e = self._graphs.get(key)
             if e is None:
                 e = self._graphs[key] = _Graphed([fwd.inputs[0], torch.empty_like(dout)], [])
@@ -638,6 +656,38 @@ def logit_mse(logits, memory, idx, alpha, err=None):
                                   float(alpha), out['loss'].data_ptr(), out['dlogits'].data_ptr(),
                                   0 if err is None else err.data_ptr(), _stream())
     _native.check(rc, 'b200ocl_logit_mse')
+    return out
+
+
+def pcr_loss(feats, labels, proxies, temperature, dproxies=None, dbias=None, err=None):
+    """PCR's proxy-contrastive loss (b200ocl_pcr_loss) of features [R,d] at labels [R] against the proxies, the
+    classifier weight [C,d]; returns dict(loss[1], dfeats [R,d], dproxies [C,d], dbias [C] (zeros)).  dproxies / dbias:
+    where to write those two gradients (the classifier's slices of the gradient arena), fresh tensors when None.  err:
+    int32 device flag [1] set to 1 by a label outside [0, C); such a row adds nothing to the loss and has zero dfeats."""
+    _need_cuda(feats, labels, proxies, dproxies, dbias, err)
+    feats = feats.detach().to(torch.float32).contiguous()
+    labels = labels.detach().to(torch.int64).contiguous()
+    proxies = proxies.detach().to(torch.float32).contiguous()
+    if feats.dim() != 2 or proxies.dim() != 2 or proxies.shape[1] != feats.shape[1]:
+        raise ValueError('feats [R,d] and proxies [C,d] must share d: got %s and %s'
+                         % (tuple(feats.shape), tuple(proxies.shape)))
+    _check_labels(feats, labels)
+    r, d = feats.shape
+    c = proxies.shape[0]
+    dev = feats.device
+    for name, t, shape in (('dproxies', dproxies, (c, d)), ('dbias', dbias, (c,))):
+        if t is not None and (t.dtype != torch.float32 or not t.is_contiguous() or tuple(t.shape) != shape):
+            raise ValueError('%s must be a contiguous fp32 %s tensor' % (name, shape))
+    out = {'loss': torch.empty(1, dtype=torch.float32, device=dev), 'dfeats': torch.empty_like(feats),
+           'dproxies': torch.empty((c, d), dtype=torch.float32, device=dev) if dproxies is None else dproxies,
+           'dbias': torch.empty(c, dtype=torch.float32, device=dev) if dbias is None else dbias}
+    lib = _lib()
+    ws = _workspace(lib.b200ocl_pcr_loss_workspace_bytes(r, c), dev)
+    rc = lib.b200ocl_pcr_loss(feats.data_ptr(), labels.data_ptr(), r, d, proxies.data_ptr(), c, float(temperature),
+                              out['loss'].data_ptr(), out['dfeats'].data_ptr(), out['dproxies'].data_ptr(),
+                              out['dbias'].data_ptr(), 0 if err is None else err.data_ptr(), ws.data_ptr(), ws.numel(),
+                              _stream())
+    _native.check(rc, 'b200ocl_pcr_loss')
     return out
 
 

@@ -1,8 +1,8 @@
 """Agents of the replay path with the reference surface `cls(model, opt, params)`,
 `.train_learner(x_train, y_train)`, `.evaluate(test_loaders)`:
 ExperienceReplay (agents/exp_replay.py:10-104: ER / MIR / ASER), SupContrastReplay (agents/scr.py:11-69), AGEM
-(agents/agem.py), Lwf (agents/lwf.py), Icarl (agents/icarl.py), Gdumb (agents/gdumb.py), and EWC_pp (agents/ewc_pp.py)
-and DERPP (DER++, which the reference lacks), both registered only on request (registry.extra_agents), over
+(agents/agem.py), Lwf (agents/lwf.py), Icarl (agents/icarl.py), Gdumb (agents/gdumb.py), and EWC_pp (agents/ewc_pp.py),
+DERPP (DER++) and PCR, the last two lacking in the reference, all registered only on request (registry.extra_agents), over
 ContinualLearner (agents/base.py:14-113) with its training tricks (labels trick, separated softmax, kd_trick /
 kd_trick_star, review trick).
 
@@ -21,7 +21,7 @@ import torch
 
 from . import memory, nets, ops
 from .augment import SCRTransform
-from .engine import ce_loss, cls_loss, icarl_loss, logit_mse
+from .engine import ce_loss, cls_loss, icarl_loss, logit_mse, pcr_loss
 from .memory import Buffer, input_size_match
 from .nets import adopt, engine_of, EngineModel
 
@@ -558,6 +558,8 @@ class ContinualLearner(torch.nn.Module):
         return self.model.forward(x)
 
     # ------------------------------------------------------------------ evaluate (SURVEY section 8f: next)
+    _eval_cosine = False        # PCR: arg-max of the cosine between feature and classifier row (ops.cosine_argmax)
+
     def _ncm(self):
         return (getattr(self.params, 'trick', None) or {}).get('ncm_trick') or self.params.agent in ['ICARL', 'SCR', 'SCP']
 
@@ -575,6 +577,9 @@ class ContinualLearner(torch.nn.Module):
             raise ErrorAnalysisUnsupported('error_analysis reads classifier logits, which the nearest-class-mean '
                                            'evaluation of %s does not compute (the reference fails with '
                                            'UnboundLocalError there)' % self.params.agent)
+        if ea and self._eval_cosine:
+            raise ErrorAnalysisUnsupported('error_analysis reads classifier logits, which the cosine evaluation of %s '
+                                           'does not compute' % self.params.agent)
         eng = self.engine
         eng.pack()                  # the caller may have written the Parameters since the last step
         self.model.eval()           # base.py:119 (the next train_learner switches back)
@@ -607,6 +612,8 @@ class ContinualLearner(torch.nn.Module):
                 f = eng.features_eval(batch_x)
                 if ncm:
                     ops.ncm_classify(f, means, class_ids, truth=batch_y, n_correct=hits)
+                elif self._eval_cosine:
+                    ops.cosine_argmax(f, W, truth=batch_y, n_correct=hits)
                 elif ea:
                     pred_task, sums = ops.linear_argmax_ea(f, W, b, batch_y, sets_t, task_t, counts[task], n_correct=hits)
                     recs += [pred_task, sums.view(torch.int64).reshape(-1)]
@@ -1236,6 +1243,107 @@ class DERPP(ContinualLearner):
                           .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
                     print('==>>> it: {}, mem logit loss: {:.6f}, mem avg. loss: {:.6f}, running mem acc: {:.3f}'
                           .format(i, meters['losses_logit'].avg(), meters['losses_mem'].avg(), meters['acc_mem'].avg()))
+        self._raise_label_errors()
+        yield from _after_train_steps(self)
+        self._end_call()
+
+
+def pcr_temperature(params):
+    """params.pcr_temp as a float, 0.09 when absent; ValueError unless it is finite and positive."""
+    v = getattr(params, 'pcr_temp', None)
+    if v is None:
+        return 0.09
+    try:
+        t = float(v) if not isinstance(v, bool) else float('nan')
+    except (TypeError, ValueError):
+        t = float('nan')
+    if not (math.isfinite(t) and t > 0):
+        raise ValueError('PCR needs params.pcr_temp to be a finite number > 0, got %r' % (v,))
+    return t
+
+
+class PCR(ContinualLearner):
+    """PCR (Lin et al., "PCR: Proxy-based Contrastive Replay for Online Class-Incremental Continual Learning", CVPR 2023)
+    on the engine.  The proxies are the rows of the classifier weight linear.weight [C, d]; linear.bias never enters the
+    loss and gets a zero gradient.  Per stream batch (x, y), mem_iters times:
+      1. a random retrieval of eps_mem_batch memory rows (m, y_m); an empty draw skips the iteration (no pass, no step);
+      2. x' = T(x), then m' = T(m), T being SCR's augmentation for the dataset's size;
+      3. the train-mode forward of [x; x'], then of [m; m'] (the BN running statistics move in that order), keeping the
+         encoder features;
+      4. the proxy-contrastive loss of F = [F_m; F_m'; F_x; F_x'] at [y_m; y_m; y; y] (engine.pcr_loss: dF, and the
+         proxies' gradient written into the gradient arena), the two backward passes from dF, one optimizer step.
+    Then the reservoir update of the unaugmented (x, y).  Evaluation: the arg-max of the cosine between the eval-mode
+    feature and each proxy (ops.cosine_argmax)."""
+
+    _eval_cosine = True
+
+    def __init__(self, model, opt, params):
+        if params.update != 'random' or params.retrieve != 'random':
+            raise NotImplementedError('PCR runs with the random retrieval and the reservoir update (update=random, '
+                                      'retrieve=random), not update=%r, retrieve=%r' % (params.update, params.retrieve))
+        trick = getattr(params, 'trick', None) or {}
+        on = [k for k in ('labels_trick', 'separated_softmax', 'kd_trick', 'kd_trick_star', 'review_trick', 'ncm_trick')
+              if trick.get(k)]
+        if on:
+            raise NotImplementedError('PCR runs its proxy-contrastive loss alone; %s not implemented' % ', '.join(on))
+        temp = pcr_temperature(params)
+        super().__init__(model, opt, params)
+        self.temp = temp
+        self.buffer = Buffer(model, params)
+        self.mem_size = params.mem_size
+        self.eps_mem_batch = params.eps_mem_batch
+        self.mem_iters = params.mem_iters
+        hw = input_size_match[params.data]
+        self.transform = SCRTransform(size=(hw[1], hw[2]))
+        eng = self.engine
+        (wo, wn, _), (bo, bn, _) = eng.table[-2], eng.table[-1]
+        c = bn
+        self._proxies = eng.state.params[wo:wo + wn].view(c, wn // c)
+        self._dproxies = eng.state.grads[wo:wo + wn].view(c, wn // c)
+        self._dbias = eng.state.grads[bo:bo + bn]
+
+    def replay_step(self, batch_x, batch_y, batch_y_host, meters=None):
+        if self.grad_sync is not None:
+            raise NotImplementedError('data-parallel PCR: the proxies\' gradient is not summed across ranks')
+        eng = self.engine
+        spec = self._optimizer()
+        for _ in range(self.mem_iters):
+            mem_x, mem_y = self.buffer.retrieve(x=batch_x, y=batch_y)                # 1.
+            m = mem_x.size(0)
+            if m == 0:
+                continue
+            x_aug = self.transform(batch_x)                                          # 2. stream first
+            m_aug = self.transform(mem_x)
+            xx = torch.cat((batch_x.to(torch.float32), x_aug))
+            mm = torch.cat((mem_x, m_aug))
+            fx, ws_x = eng.forward_train(xx, slot=0, features=True)                  # 3. BN stats: stream pair first
+            fm, ws_m = eng.forward_train(mm, slot=1, features=True)
+            feats = torch.cat((fm, fx))                                              # 4.
+            labels = torch.cat((mem_y, mem_y, batch_y, batch_y))
+            out = pcr_loss(feats, labels, self._proxies, self.temp, dproxies=self._dproxies, dbias=self._dbias,
+                           err=self._err_flag())
+            eng.backward(mm, out['dfeats'][:2 * m], ws_m, features=True)
+            eng.backward(xx, out['dfeats'][2 * m:], ws_x, accumulate=True, features=True)
+            self._optimizer_step(spec)
+            self.last_loss = out['loss']
+            if meters is not None:
+                meters['losses'].update(out['loss'], labels.size(0))
+        self.buffer.update(batch_x, batch_y, y_host=batch_y_host)
+        self._throttle()
+
+    def _steps(self, x_train, y_train):
+        self._begin_call()
+        self.before_train(x_train, y_train)
+        self.engine.pack()          # the caller may have written the Parameters (load_state_dict, weight surgery)
+        self.model = self.model.train()
+        meters = {'losses': AverageMeter()}
+        for ep in range(self.epoch):
+            stream = StreamFeeder(x_train, y_train, self.batch, self.device)   # DataLoader(shuffle=True): new order per epoch
+            for i, (batch_x, batch_y, y_host) in enumerate(stream):
+                self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
+                yield
+                if i % 100 == 1 and self.verbose:
+                    print('==>>> it: {}, avg. loss: {:.6f}, '.format(i, meters['losses'].avg()))
         self._raise_label_errors()
         yield from _after_train_steps(self)
         self._end_call()

@@ -276,6 +276,23 @@ def linear_argmax(feats, weight, bias, truth=None, n_correct=None):
     return pred
 
 
+def cosine_argmax(feats, weight, truth=None, n_correct=None):
+    """PCR's evaluation (b200ocl_cosine_argmax): arg-max over the rows w_c of weight [C,d] of the cosine
+    <f / (||f|| + 1e-6), w_c / (||w_c|| + 1e-6)>, the first maximum on ties.  Returns pred [B]; n_correct (int64 [1])
+    gains the rows whose prediction equals truth."""
+    _need_cuda(feats, weight, truth, n_correct)
+    feats, weight = _f32(feats), _f32(weight)
+    B, d = feats.shape
+    if weight.dim() != 2 or weight.shape[1] != d:
+        raise ValueError('weight [C,d] must have the features\' width d=%d' % d)
+    truth = _check_truth(truth, B)
+    pred = torch.empty(B, dtype=torch.int64, device=feats.device)
+    rc = _native.lib().b200ocl_cosine_argmax(_ptr(feats), B, d, _ptr(weight), weight.shape[0], _ptr(truth), _ptr(pred),
+                                             _ptr(n_correct), _stream())
+    _native.check(rc, 'b200ocl_cosine_argmax')
+    return pred
+
+
 def linear_argmax_ea(feats, weight, bias, truth, class_sets, class_task, counts, n_correct=None, pred=None):
     """linear_argmax with the error analysis of agents/base.py:177-205 in the same launch (b200ocl_linear_argmax_ea):
     the prediction written to pred and the hits added to n_correct are linear_argmax's, bit for bit.  class_sets

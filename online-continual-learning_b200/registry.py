@@ -8,8 +8,8 @@ already hold), so `general_main.py` runs unchanged:
     import b200ocl; b200ocl.install()          # before main(args); or:  python -m b200ocl.launch general_main.py ...
 
 The agents registered here are ER, SCR, AGEM, LWF, ICARL and GDUMB.  `extra_agents` holds agents that are only
-registered on request, `install(extra=('EWC',))` (or `B200OCL_EXTRA_AGENTS=EWC` with b200ocl.launch): EWC (EWC++) and
-DERPP (DER++, an agent the reference does not register).
+registered on request, `install(extra=('EWC',))` (or `B200OCL_EXTRA_AGENTS=EWC` with b200ocl.launch): EWC (EWC++),
+DERPP (DER++) and PCR (proxy-based contrastive replay), the last two agents the reference does not register.
 Every other agent / plugin of the reference (EWC unless requested, CNDPM, the match retrievals) stays registered and
 untouched.
 
@@ -34,7 +34,7 @@ With B200OCL_CHECKPOINT_ASYNC=1 as well, the snapshots are staged on the device 
 (checkpoint.py).  Unset, empty or 0 changes nothing; any other value, or 1 without a checkpoint directory, raises
 ValueError in install() before anything is replaced.
 """
-from .learners import AGEM, DERPP, EWC_pp, ExperienceReplay, Gdumb, Icarl, Lwf, SupContrastReplay
+from .learners import AGEM, DERPP, EWC_pp, ExperienceReplay, Gdumb, Icarl, Lwf, PCR, SupContrastReplay
 from .retrieve import ASER_retrieve, MIR_retrieve, Random_retrieve
 from .update import ASER_update, GSSGreedyUpdate, Reservoir_update
 
@@ -51,6 +51,7 @@ agents = {
 extra_agents = {
     'EWC': EWC_pp,
     'DERPP': DERPP,
+    'PCR': PCR,
 }
 
 retrieve_methods = {
