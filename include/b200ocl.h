@@ -42,6 +42,9 @@ const char* b200ocl_last_error(void);
 int b200ocl_version(void);
 /* Number of kernel launches issued through this library since load (bench.py reports it). */
 uint64_t b200ocl_launch_count(void);
+/* The SM count the current device's launches are planned for: its multiprocessor count, or B200OCL_SM_COUNT when
+ * that is set to a smaller positive value (read once per device per process). */
+int b200ocl_sm_count(void);
 /* Optional per-launch device timing for bench.py's roofline: between begin and end every launch of
  * this library is bracketed by CUDA events on its launch stream and accumulated per kernel class
  * together with its algorithmic work (FLOPs for conv/wgrad classes, bytes otherwise).

@@ -13,6 +13,7 @@ SIGNATURES = {
     'b200ocl_last_error': (c_char_p, []),
     'b200ocl_version': (c_int, []),
     'b200ocl_launch_count': (c_uint64, []),
+    'b200ocl_sm_count': (c_int, []),
     'b200ocl_profile_begin': (None, []),
     'b200ocl_profile_end': (c_int, []),
     'b200ocl_profile_get': (c_int, [c_int, P, c_int, P, P, P]),
@@ -90,14 +91,42 @@ SIGNATURES = {
 
 _lib = None
 
+# The library is built for sm_90a only; no such part has more SMs than the H100 SXM's 132.
+MAX_SMS = 132
+
 
 class NativeError(RuntimeError):
     pass
 
 
+def parse_sm_count(text, device_sms):
+    """The SM count B200OCL_SM_COUNT asks the library to plan for, or None when it is unset (text None).  Refuses
+    anything but an integer in [1, device_sms]: a grid planned for more SMs than the device has could leave part of a
+    grid-synchronised kernel (fused BN backward, fused SupCon) waiting for CTAs that never get an SM."""
+    if text is None:
+        return None
+    try:
+        n = int(text.strip())
+    except ValueError:
+        raise ValueError('B200OCL_SM_COUNT=%r is not an integer' % text) from None
+    if not 1 <= n <= device_sms:
+        raise ValueError('B200OCL_SM_COUNT=%d is outside [1, %d], the SM counts this device can run' % (n, device_sms))
+    return n
+
+
+def _device_sms():
+    """The fewest SMs of any visible device; MAX_SMS where there is none."""
+    import torch
+    if not torch.cuda.is_available():
+        return MAX_SMS
+    return min(torch.cuda.get_device_properties(i).multi_processor_count for i in range(torch.cuda.device_count()))
+
+
 def lib():
     global _lib
     if _lib is None:
+        if os.environ.get('B200OCL_SM_COUNT') is not None:
+            parse_sm_count(os.environ['B200OCL_SM_COUNT'], _device_sms())
         if not os.path.exists(LIB_PATH):
             raise NativeError('%s is missing: build it with `python __graft_entry__.py` (nvcc, sm_90a). '
                               'b200ocl has no CPU or library fallback.' % LIB_PATH)

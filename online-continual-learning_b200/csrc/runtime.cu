@@ -58,14 +58,28 @@ void prof_end() {
   g_recs.back().open = false;
 }
 
+// The SM count every launch geometry, plan and workspace size is derived from.  B200OCL_SM_COUNT=n plans for n SMs
+// instead of the device's count (an H100 PCIe's 114, a MIG slice's 16 or 60), read once per device so a process never
+// mixes two counts.  It only goes down: bn_bwd_fused_kernel and supcon_fused_kernel wait on each other across their
+// CTAs, one per SM, and a grid planned for more SMs than the device has need not be resident at once.  _native.lib()
+// refuses a value outside [1, device count] before anything launches; the clamp here is the last line of defence.
+static int planned_sms(int device_sms) {
+  if (const char* e = getenv("B200OCL_SM_COUNT")) {
+    const long v = strtol(e, nullptr, 10);
+    if (v >= 1 && v < device_sms) return (int)v;
+  }
+  return device_sms;
+}
+
 int sm_count() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  // no device (host-only plan queries): plan for 148 SMs, or fewer when asked
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return planned_sms(148);
   if (cached[dev] == 0) {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
-    cached[dev] = n;
+    cached[dev] = planned_sms(n);
   }
   return cached[dev];
 }
@@ -76,6 +90,7 @@ extern "C" {
 const char* b200ocl_last_error(void) { return b200ocl::g_err; }
 int b200ocl_version(void) { return 100; }
 uint64_t b200ocl_launch_count(void) { return b200ocl::g_launches.load(std::memory_order_relaxed); }
+int b200ocl_sm_count(void) { return b200ocl::sm_count(); }
 
 void b200ocl_profile_begin(void) {
   using namespace b200ocl;
