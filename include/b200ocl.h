@@ -194,6 +194,38 @@ size_t b200ocl_grad_cosine_workspace_bytes(int K);
 int b200ocl_grad_cosine(const float* mem_grads, const float* g, int K, size_t n, float* cos_out, float* max_out, void* workspace,
                         size_t workspace_bytes, void* stream);
 
+/* GEM's projection (Lopez-Paz & Ranzato, NeurIPS 2017; the authors' project2cone2 with margin = memory_strength) on
+ * flat gradient arenas: the t task gradients G [t,n] (row k at G + k * pitch, pitch >= n elements) and the stream
+ * gradient g [n].  P = G G^T and q = G g in fp64 (every product of two floats exact, fp64 sums in a fixed order);
+ * *flag_out = (min_k q_k < 0).  When the flag is set, v [t] (fp64, v_out) minimises 1/2 v^T (P + eps I) v + q^T v subject
+ * to v_k >= margin, solved exactly by an active-set method with a Cholesky solve of the free block per iteration, and
+ * out[i] = fl32((double)g[i] + sum_k v_k (double)G[k,i]) summed in k order (out may alias g).  When it is clear, v_out
+ * is 0 and out is neither read nor written.  A QP that exhausts the kernel's iteration bound sets *err_flag = 1
+ * (nullable, never cleared) and leaves its last feasible iterate in v_out.  kkt_out (nullable, [4] fp64): the primal,
+ * dual and complementarity residuals of w = v - margin and the number of Cholesky solves.  Three launches (Gram, QP,
+ * projection), no host synchronisation, no floating-point atomics: bit-identical on repeat at a given SM count.
+ * B200OCL_EINVAL for a null pointer, t or n < 1, pitch < n, a margin that is negative or not finite or an eps that is
+ * not finite and positive; B200OCL_EUNSUPPORTED for t > 64. */
+size_t b200ocl_gem_project_workspace_bytes(int t, size_t n);
+int b200ocl_gem_project(const float* G, size_t pitch, int t, const float* g, float* out, size_t n, double margin,
+                        double eps, double* v_out, int* flag_out, int* err_flag, double* kkt_out, void* workspace,
+                        size_t workspace_bytes, void* stream);
+
+/* The launches b200ocl_gem_project makes for t task gradients of length n on a GPU with sms SMs (0: the current
+ * device).  rows = t + 1 (the Gram is taken of [G; g]), padded to rows_padded = 4 * row_blocks; each of the
+ * block_pairs = row_blocks (row_blocks + 1) / 2 upper-triangle 4 x 4 blocks of pairs is formed by `lanes` threads over
+ * interleaved columns of each staged tile of tile_cols columns (row stride tile_stride floats, two stages; smem_bytes of
+ * dynamic shared memory).  grid CTAs, each owning chunk consecutive columns (tiles_per_cta tiles; the last CTA fewer,
+ * none without columns), write pairs = rows (rows + 1) / 2 fp64 partials each: part_bytes, inside workspace_bytes.  The
+ * projection runs proj_grid CTAs of 256 threads.  Host only, launches nothing; exists so that tests can check every
+ * plan on any SM count.  B200OCL_EINVAL unless 1 <= t <= 64 and n >= 1. */
+typedef struct {
+  int rows, rows_padded, row_blocks, block_pairs, lanes, tile_cols, tile_stride, pairs;
+  int grid, tiles_per_cta, proj_grid, sms;
+  size_t chunk, smem_bytes, part_bytes, workspace_bytes;
+} b200ocl_gem_launch;
+int b200ocl_gem_plan(int t, size_t n, int sms, b200ocl_gem_launch* out);
+
 /* Stream feeder (continuum/data_utils.py:38-54: ToTensor on every sample + DataLoader shuffle): dst[i] = image
  * src[perm[i]] converted uint8 HWC -> fp32 CHW in [0,1] with an IEEE division by 255 (bit-identical to the
  * reference's CPU ToTensor).  perm may be NULL (identity).  h*w*3 % 4 == 0. */

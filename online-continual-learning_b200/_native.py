@@ -39,6 +39,10 @@ SIGNATURES = {
     'b200ocl_agem_project': (c_int, [P, P, P, c_size_t, P, P, c_size_t, P]),
     'b200ocl_grad_cosine_workspace_bytes': (c_size_t, [c_int]),
     'b200ocl_grad_cosine': (c_int, [P, P, c_int, c_size_t, P, P, P, c_size_t, P]),
+    'b200ocl_gem_project_workspace_bytes': (c_size_t, [c_int, c_size_t]),
+    'b200ocl_gem_project': (c_int, [P, c_size_t, c_int, P, P, c_size_t, c_double, c_double, P, P, P, P, P, c_size_t,
+                                    P]),
+    'b200ocl_gem_plan': (c_int, [c_int, c_size_t, c_int, P]),
     'b200ocl_sgd_step': (c_int, [P, P, P, c_size_t, c_float, c_float, P]),
     # ResNet engine: descriptor / state / info structs are passed by pointer (see engine.py)
     'b200ocl_net_query': (c_int, [P, P]),

@@ -5,7 +5,7 @@
 The reference tree is put first on sys.path, its registries are patched in place
 (b200ocl.registry.install) and general_main.py is executed with runpy, byte-identical.  Any entry point of the reference
 runs the same way, main_tune.py included.
-B200OCL_EXTRA_AGENTS (comma-separated, e.g. EWC or EWC,DERPP,PCR) also registers those opt-in agents (registry.extra_agents)."""
+B200OCL_EXTRA_AGENTS (comma-separated, e.g. EWC or EWC,DERPP,PCR,GEM) also registers those opt-in agents (registry.extra_agents)."""
 import os
 import runpy
 import sys

@@ -2,7 +2,8 @@
 `.train_learner(x_train, y_train)`, `.evaluate(test_loaders)`:
 ExperienceReplay (agents/exp_replay.py:10-104: ER / MIR / ASER), SupContrastReplay (agents/scr.py:11-69), AGEM
 (agents/agem.py), Lwf (agents/lwf.py), Icarl (agents/icarl.py), Gdumb (agents/gdumb.py), and EWC_pp (agents/ewc_pp.py),
-DERPP (DER++) and PCR, the last two lacking in the reference, all registered only on request (registry.extra_agents), over
+DERPP (DER++), PCR and GEM, the last three lacking in the reference, all registered only on request
+(registry.extra_agents), over
 ContinualLearner (agents/base.py:14-113) with its training tricks (labels trick, separated softmax, kd_trick /
 kd_trick_star, review trick).
 
@@ -1345,6 +1346,140 @@ class PCR(ContinualLearner):
                 if i % 100 == 1 and self.verbose:
                     print('==>>> it: {}, avg. loss: {:.6f}, '.format(i, meters['losses'].avg()))
         self._raise_label_errors()
+        yield from _after_train_steps(self)
+        self._end_call()
+
+
+def gem_margin(params):
+    """params.gem_margin as a float, 0.5 when absent; ValueError unless it is finite and >= 0."""
+    v = getattr(params, 'gem_margin', None)
+    if v is None:
+        return 0.5
+    try:
+        m = float(v) if not isinstance(v, bool) else float('nan')
+    except (TypeError, ValueError):
+        m = float('nan')
+    if not (math.isfinite(m) and m >= 0):
+        raise ValueError('GEM needs params.gem_margin to be a finite number >= 0, got %r' % (v,))
+    return m
+
+
+class GEM(ContinualLearner):
+    """GEM (Lopez-Paz & Ranzato, "Gradient Episodic Memory for Continual Learning", NeurIPS 2017) on the engine, in the
+    single-head form.  Each task keeps its own ring of M = mem_size // num_tasks rows (memory.TaskRingMemory).  Per
+    stream batch (x, y), mem_iters times:
+      1. for every earlier task whose ring is not empty, in task order: a train-mode forward over its filled rows, mean
+         CE and backward; the gradient arena is copied into row k of G [t, n] (these BN statistics move first);
+      2. the stream batch's train-mode forward, mean CE and backward: g in the arena;
+      3. when t >= 1, ops.gem_project: P = G G^T, q = G g in fp64 and, when min q < 0, g <- g + G^T v with v the
+         solution of min 1/2 v^T (P + 1e-3 I) v + q^T v subject to v >= gem_margin (the authors' project2cone2, their
+         memory_strength); otherwise g is left bit for bit;
+      4. one optimizer step (SGD or Adam).
+    Then the batch is written into the current task's ring.  Evaluation is the inherited arg-max path."""
+
+    MEM_SLOT = 2          # the memory passes' workspace (and graph) slot: one capture per row count
+    EPS = 1e-3
+
+    def __init__(self, model, opt, params):
+        if params.update != 'random' or params.retrieve != 'random':
+            raise NotImplementedError('GEM keeps its own per-task memory (update=random, retrieve=random), not '
+                                      'update=%r, retrieve=%r' % (params.update, params.retrieve))
+        trick = getattr(params, 'trick', None) or {}
+        on = [k for k in ('labels_trick', 'separated_softmax', 'kd_trick', 'kd_trick_star', 'review_trick', 'ncm_trick')
+              if trick.get(k)]
+        if on:
+            raise NotImplementedError('GEM runs with plain cross-entropy and arg-max evaluation; %s not implemented'
+                                      % ', '.join(on))
+        margin = gem_margin(params)
+        M = int(params.mem_size) // int(params.num_tasks)
+        if M < 1:
+            raise ValueError('GEM splits mem_size=%d over num_tasks=%d: no row per task' % (params.mem_size,
+                                                                                         params.num_tasks))
+        super().__init__(model, opt, params)
+        self.margin = margin
+        self.mem_iters = params.mem_iters
+        # not named `memory` or `buffer`: those names carry GDumb's and the replay buffer's layouts elsewhere
+        self.rings = memory.TaskRingMemory(M, input_size_match[params.data][1], self.device)
+        self._task = 0
+        self._G = None                                   # [t, n] task gradients, grown when t grows
+        self._v = torch.zeros(ops.GEM_MAX_T, dtype=torch.float64, device=self.device)
+        self._flag = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self._qp_err = torch.zeros(1, dtype=torch.int32, device=self.device)
+
+    def snapshot_parts(self):
+        out = super().snapshot_parts()
+        out['rings'] = self.rings.snapshot_parts()
+        return out
+
+    def snapshot_capacity(self):
+        # num_tasks rings, or 12, the most tasks of the OpenLORIS and CORe50 (ni, nc) streams, which set their own count
+        return super().snapshot_capacity() + self.rings.snapshot_capacity(max(int(self.params.num_tasks), 12))
+
+    def restore(self, state):
+        super().restore(state)
+        self.rings.restore(state['rings'])
+
+    def _task_grads(self, t):
+        n = self.engine.info.n_params
+        if self._G is None or self._G.shape[0] < t:
+            self._G = torch.empty((t, n), dtype=torch.float32, device=self.device)
+        return self._G
+
+    def replay_step(self, batch_x, batch_y, batch_y_host, meters=None):
+        if self.grad_sync is not None:
+            raise NotImplementedError('data-parallel GEM: the task gradients and the QP are not reduced across ranks')
+        eng = self.engine
+        spec = self._optimizer()
+        past = [k for k in range(self._task) if self.rings.filled[k]]
+        t = len(past)
+        G = self._task_grads(t) if t else None
+        for _ in range(self.mem_iters):
+            for j, k in enumerate(past):                                              # 1.
+                mx, my = self.rings.rows(k)
+                logits_k, ws_k = eng.forward_train(mx, slot=self.MEM_SLOT)
+                ce_k = self.criterion(logits_k, my)
+                eng.backward(mx, ce_k['dlogits'], ws_k)
+                G[j].copy_(eng.state.grads)
+            logits, ws = eng.forward_train(batch_x, slot=0)                           # 2.
+            ce = self.criterion(logits, batch_y, want_correct=meters is not None)
+            eng.backward(batch_x, ce['dlogits'], ws)
+            if meters is not None:
+                meters['acc_batch'].update(ce['n_correct'] / batch_y.size(0), batch_y.size(0))
+                meters['losses_batch'].update(ce['loss'], batch_y.size(0))
+            if t:                                                                     # 3.
+                ops.gem_project(G, t, eng.state.grads, out=eng.state.grads, margin=self.margin, eps=self.EPS,
+                                v=self._v, flag=self._flag, err=self._qp_err)
+            self.last_loss = ce['loss']
+            self._optimizer_step(spec)                                                # 4.
+        self.rings.write(self._task, batch_x, batch_y, batch_y_host)
+        self._throttle()
+
+    def _raise_qp_errors(self):
+        if int(self._qp_err.item()):
+            self._qp_err.zero_()
+            raise RuntimeError('GEM: the projection QP ran out of iterations (b200ocl_gem_project set its error flag)')
+
+    def _steps(self, x_train, y_train):
+        if self.task_seen > ops.GEM_MAX_T:
+            raise ValueError('GEM projects against at most %d earlier tasks; this task has %d'
+                             % (ops.GEM_MAX_T, self.task_seen))
+        self._begin_call()
+        self.before_train(x_train, y_train)
+        self._task = self.task_seen
+        self.rings.begin_task(self._task)
+        self.engine.pack()          # the caller may have written the Parameters (load_state_dict, weight surgery)
+        self.model = self.model.train()
+        meters = {k: AverageMeter() for k in ('losses_batch', 'acc_batch')}
+        for ep in range(self.epoch):
+            stream = StreamFeeder(x_train, y_train, self.batch, self.device)   # DataLoader(shuffle=True): new order per epoch
+            for i, (batch_x, batch_y, y_host) in enumerate(stream):
+                self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
+                yield
+                if i % 100 == 1 and self.verbose:
+                    print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
+                          .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
+        self._raise_label_errors()
+        self._raise_qp_errors()
         yield from _after_train_steps(self)
         self._end_call()
 

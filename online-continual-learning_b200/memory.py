@@ -576,6 +576,82 @@ class GreedyBalancedMemory(object):
         self._size = int(state['size'])
 
 
+class TaskRingMemory(object):
+    """GEM's episodic memory: one ring of M rows per task (images fp32 [M,3,H,W] and labels int64 [M] on the device, a
+    host mirror of the labels), allocated when its task begins, so the memory grows one task at a time.  write() follows
+    the authors' release: rows [cnt, endcnt) take the batch's first endcnt - cnt rows with endcnt = min(cnt + bsz, M)
+    (truncated at the ring's end, not wrapped) and the counter returns to 0 when it reaches M; begin_task() restarts the
+    counter of its task at 0.  A task's filled row count is min(rows written, M)."""
+
+    def __init__(self, M, in_hw, device):
+        if int(M) < 1:
+            raise ValueError('GEM needs at least one memory row per task (mem_size // num_tasks >= 1), got %d' % int(M))
+        self.M = int(M)
+        self.in_hw = int(in_hw)
+        self.device = torch.device(device)
+        self.images, self.labels, self.labels_host = [], [], []
+        self.filled, self.cnt = [], []
+
+    def __len__(self):
+        return len(self.images)
+
+    def begin_task(self, task):
+        """Rings up to task `task` exist (a task never written keeps an empty one); its counter restarts at 0."""
+        while len(self.images) <= task:
+            self.images.append(torch.zeros((self.M, 3, self.in_hw, self.in_hw), dtype=torch.float32, device=self.device))
+            self.labels.append(torch.zeros(self.M, dtype=torch.int64, device=self.device))
+            self.labels_host.append(np.zeros(self.M, dtype=np.int64))
+            self.filled.append(0)
+            self.cnt.append(0)
+        self.cnt[task] = 0
+
+    def write(self, task, x, y, y_host):
+        """The ring write of one batch into task `task`'s ring; returns (start, rows written)."""
+        cnt = self.cnt[task]
+        end = min(cnt + x.size(0), self.M)
+        k = end - cnt
+        self.images[task][cnt:end].copy_(x[:k])
+        self.labels[task][cnt:end].copy_(y[:k])
+        self.labels_host[task][cnt:end] = np.asarray(y_host, dtype=np.int64)[:k]
+        self.filled[task] = max(self.filled[task], end)
+        self.cnt[task] = 0 if end == self.M else end
+        return cnt, k
+
+    def rows(self, task):
+        """(images, labels) of task `task`'s filled rows: views of its ring."""
+        n = self.filled[task]
+        return self.images[task][:n], self.labels[task][:n]
+
+    def snapshot_parts(self):
+        """The filled rows of every ring on the device (images marked as 8-bit rows, one array per task), the label
+        mirrors, counters and filled counts on the host."""
+        return {'M': self.M, 'filled': list(self.filled), 'cnt': list(self.cnt),
+                'labels': [lab[:n].copy() for lab, n in zip(self.labels_host, self.filled)],
+                'images': {k: Rows8(img[:n]) for k, (img, n) in enumerate(zip(self.images, self.filled)) if n}}
+
+    def snapshot(self):
+        return host_tree(self.snapshot_parts())
+
+    def snapshot_capacity(self, n_tasks):
+        """Bytes of the snapshot_parts() device tree of n_tasks full rings."""
+        return int(n_tasks) * self.M * 3 * self.in_hw * self.in_hw * 4
+
+    def restore(self, state):
+        if int(state['M']) != self.M:
+            raise ValueError('snapshot memory of %d rows per task does not fit %d' % (int(state['M']), self.M))
+        filled = [int(n) for n in state['filled']]
+        self.images, self.labels, self.labels_host, self.filled, self.cnt = [], [], [], [], []
+        if filled:
+            self.begin_task(len(filled) - 1)
+        for k, n in enumerate(filled):
+            if n:
+                self.images[k][:n].copy_(state['images'][k])
+                self.labels_host[k][:n] = np.asarray(state['labels'][k], dtype=np.int64)
+                self.labels[k].copy_(torch.from_numpy(self.labels_host[k]))
+        self.filled = filled
+        self.cnt = [int(c) for c in state['cnt']]
+
+
 # --------------------------------------------------------------------------- buffer
 def random_retrieve(buffer, num_retrieve, excl_indices=None, return_indices=False):
     """buffer_utils.py:9-26."""

@@ -375,6 +375,56 @@ def agem_project(g, g_ref, out=None, want_dots=False):
     return (out, dots) if want_dots else out
 
 
+GEM_MAX_T = 64          # task gradients b200ocl_gem_project's QP takes
+
+
+class GemLaunch(ctypes.Structure):
+    """b200ocl_gem_launch: the launches one b200ocl_gem_project call makes."""
+    _fields_ = [(k, ctypes.c_int) for k in ('rows', 'rows_padded', 'row_blocks', 'block_pairs', 'lanes', 'tile_cols',
+                                            'tile_stride', 'pairs', 'grid', 'tiles_per_cta', 'proj_grid', 'sms')] + \
+               [(k, ctypes.c_size_t) for k in ('chunk', 'smem_bytes', 'part_bytes', 'workspace_bytes')]
+
+
+def gem_plan(t, n, sms=0):
+    """Host-only test hook (b200ocl_gem_plan): the launches gem_project() makes for t task gradients of length n on a
+    GPU with sms SMs (0: the current device)."""
+    out = GemLaunch()
+    _native.check(_native.lib().b200ocl_gem_plan(int(t), int(n), int(sms), ctypes.byref(out)), 'b200ocl_gem_plan')
+    return out
+
+
+def gem_project(G, t, g, out=None, margin=0.5, eps=1e-3, v=None, flag=None, err=None, kkt=None):
+    """GEM's projection (b200ocl_gem_project) of the flat gradient g [n] against the first t rows of G [rows, pitch]
+    (fp32, row-major, read in place): when min(G g) < 0, out = g + G^T v with v the solution of the dual QP
+    (v >= margin), else out is left alone.  out may be g.  v (fp64 [t]), flag (int32 [1]), err (int32 [1], set on a QP
+    that runs out of iterations) and kkt (fp64 [4]) are device tensors written by the call; v and flag are made when
+    None.  Returns (out, v, flag)."""
+    _need_cuda(G, g, out, v, flag, err, kkt)
+    if G.dtype != torch.float32 or G.dim() != 2 or G.stride(1) != 1:
+        raise ValueError('G must be an fp32 [rows, pitch] matrix with unit column stride')
+    if g.dtype != torch.float32 or not g.is_contiguous():
+        raise ValueError('g must be a contiguous fp32 vector')
+    n = g.numel()
+    if not 1 <= t <= G.shape[0] or G.shape[1] < n:
+        raise ValueError('need 1 <= t <= %d rows of at least n=%d columns' % (G.shape[0], n))
+    if out is None:
+        out = g.clone()
+    elif out.dtype != torch.float32 or not out.is_contiguous() or out.numel() != n:
+        raise ValueError('out must be a contiguous fp32 tensor of n elements')
+    dev = g.device
+    v = torch.empty(t, dtype=torch.float64, device=dev) if v is None else v
+    flag = torch.empty(1, dtype=torch.int32, device=dev) if flag is None else flag
+    if v.dtype != torch.float64 or v.numel() < t or flag.dtype != torch.int32 or \
+            (kkt is not None and (kkt.dtype != torch.float64 or kkt.numel() < 4)):
+        raise ValueError('v must be fp64 [t], flag int32 [1], kkt fp64 [4]')
+    lib = _native.lib()
+    ws = _workspace(lib.b200ocl_gem_project_workspace_bytes(int(t), n), dev)
+    rc = lib.b200ocl_gem_project(_ptr(G), G.stride(0), int(t), _ptr(g), _ptr(out), n, float(margin), float(eps),
+                                 _ptr(v), _ptr(flag), _ptr(err), _ptr(kkt), _ptr(ws), ws.numel(), _stream())
+    _native.check(rc, 'b200ocl_gem_project')
+    return out, v, flag
+
+
 GRAD_COSINE_MAX_K = 64
 
 

@@ -9,7 +9,8 @@ already hold), so `general_main.py` runs unchanged:
 
 The agents registered here are ER, SCR, AGEM, LWF, ICARL and GDUMB.  `extra_agents` holds agents that are only
 registered on request, `install(extra=('EWC',))` (or `B200OCL_EXTRA_AGENTS=EWC` with b200ocl.launch): EWC (EWC++),
-DERPP (DER++) and PCR (proxy-based contrastive replay), the last two agents the reference does not register.
+DERPP (DER++), PCR (proxy-based contrastive replay) and GEM (gradient episodic memory), the last three agents the
+reference does not register.
 Every other agent / plugin of the reference (EWC unless requested, CNDPM, the match retrievals) stays registered and
 untouched.
 
@@ -34,7 +35,7 @@ With B200OCL_CHECKPOINT_ASYNC=1 as well, the snapshots are staged on the device 
 (checkpoint.py).  Unset, empty or 0 changes nothing; any other value, or 1 without a checkpoint directory, raises
 ValueError in install() before anything is replaced.
 """
-from .learners import AGEM, DERPP, EWC_pp, ExperienceReplay, Gdumb, Icarl, Lwf, PCR, SupContrastReplay
+from .learners import AGEM, DERPP, EWC_pp, ExperienceReplay, Gdumb, GEM, Icarl, Lwf, PCR, SupContrastReplay
 from .retrieve import ASER_retrieve, MIR_retrieve, Random_retrieve
 from .update import ASER_update, GSSGreedyUpdate, Reservoir_update
 
@@ -52,6 +53,7 @@ extra_agents = {
     'EWC': EWC_pp,
     'DERPP': DERPP,
     'PCR': PCR,
+    'GEM': GEM,
 }
 
 retrieve_methods = {
