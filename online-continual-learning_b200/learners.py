@@ -61,6 +61,13 @@ class AverageMeter(object):
         return float(self.sum) / self.count
 
 
+def _update_meters(meters, key, out, n, loss=None):
+    """meters['acc_' + key] and meters['losses_' + key] take a batch of n rows: out's hit rate and out's loss (or
+    `loss`)."""
+    meters['acc_' + key].update(out['n_correct'] / n, n)
+    meters['losses_' + key].update(out['loss'] if loss is None else loss, n)
+
+
 class StreamFeeder(object):
     """One task's stream: uint8 NHWC images -> fp32 NCHW in [0,1] on the device (ToTensor,
     continuum/data_utils.py:38-54), shuffled, batches of `batch`, last partial batch dropped
@@ -206,6 +213,38 @@ def kd_mix(task_seen, kd_trick=False, kd_trick_star=False, lwf=False):
     return w_ce, w_kd
 
 
+_CE_TRICKS = ('labels_trick', 'separated_softmax', 'kd_trick', 'kd_trick_star')
+
+
+def _refuse_options(params, why, tricks, random_memory=None):
+    """NotImplementedError for options an agent does not run, raised before it builds anything.  random_memory, when
+    given, says why the agent runs only with update=random, retrieve=random; `tricks` are the params.trick flags it
+    does not implement, and `why` says why."""
+    if random_memory is not None and (params.update != 'random' or params.retrieve != 'random'):
+        raise NotImplementedError('%s (update=random, retrieve=random), not update=%r, retrieve=%r'
+                                  % (random_memory, params.update, params.retrieve))
+    trick = getattr(params, 'trick', None) or {}
+    on = [k for k in tricks if trick.get(k)]
+    if on:
+        raise NotImplementedError('%s; %s not implemented' % (why, ', '.join(on)))
+
+
+def _finite_param(params, name, agent, positive=False, default=None):
+    """params.<name> as a float (a string such as '1.5' converts, a bool does not), `default` when it is absent and
+    there is one; ValueError unless it is finite and > 0 (positive) or >= 0."""
+    v = getattr(params, name, None)
+    if v is None and default is not None:
+        return default
+    try:
+        f = float(v) if not isinstance(v, bool) else math.nan
+    except (TypeError, ValueError):
+        f = math.nan
+    if not (math.isfinite(f) and (f > 0 if positive else f >= 0)):
+        raise ValueError('%s needs params.%s to be a finite number %s, got %r'
+                         % (agent, name, '> 0' if positive else '>= 0', v))
+    return f
+
+
 class OptimizerSpec(collections.namedtuple('OptimizerSpec', 'kind lr weight_decay betas eps foreach')):
     """What one opt.step() runs: kind 'sgd' (lr, weight_decay) or 'adam' (also betas, eps and foreach: torch's
     multi-tensor path, else its single-tensor one; the two round sqrt(v) / bc2_sqrt differently)."""
@@ -241,7 +280,7 @@ class ContinualLearner(torch.nn.Module):
         self.bias_norm_new = []
         self.bias_norm_old = []
         trick = getattr(params, 'trick', None) or {}
-        self._trick = {k: bool(trick.get(k)) for k in ('labels_trick', 'separated_softmax', 'kd_trick', 'kd_trick_star')}
+        self._trick = {k: bool(trick.get(k)) for k in _CE_TRICKS}
         contrastive = params.agent in ('SCR', 'SCP')
         if contrastive and (self._trick['labels_trick'] or self._trick['separated_softmax']):
             # base.py:95-107 would feed [B,2,128] projections to a CE branch
@@ -505,9 +544,6 @@ class ContinualLearner(torch.nn.Module):
         return self.criterion(logits, labels, t, w_ce, w_kd if t is not None else 0.0, want_grad=want_grad,
                               want_correct=want_correct)
 
-    def _review(self):
-        _drain(self._review_steps())
-
     def _review_steps(self):
         """Review trick (agents/base.py:62-88, the published SCR setting config_CVPR/agent/scr/scr_5k.yml:10): one
         pass over the filled memory in shuffled batches of eps_mem_batch (drop_last), gradients divided by 10.
@@ -546,6 +582,12 @@ class ContinualLearner(torch.nn.Module):
             self._throttle()
             yield
 
+    # ------------------------------------------------------------------ the task loop (train_learner)
+    # The verbose progress lines, printed after batches i = 1, 101, 201, ... of every epoch: (format, meter keys), the
+    # format filled with i and those meters' averages.  replay_step fills the meters these lines name; an agent
+    # without lines gets meters=None and prints nothing.
+    _progress = ()
+
     def train_learner(self, x_train, y_train):
         _drain(self._steps(x_train, y_train))
 
@@ -553,7 +595,41 @@ class ContinualLearner(torch.nn.Module):
         """train_learner as a generator that yields after every replay step (and every step of the review trick), so
         that a driver can interleave the steps of several learners (multirun.run_group).  Draining it is
         train_learner: the same launches in the same order."""
-        raise NotImplementedError
+        self._begin_call()
+        self.before_train(x_train, y_train)
+        self._begin_task(len(y_train) // self.batch)
+        self.engine.pack()          # the caller may have written the Parameters (load_state_dict, weight surgery)
+        self.model = self.model.train()
+        meters = None
+        if self.verbose and self._progress:
+            meters = {k: AverageMeter() for _, keys in self._progress for k in keys}
+        for ep in range(self.epoch):
+            stream = StreamFeeder(x_train, y_train, self.batch, self.device)   # DataLoader(shuffle=True): new order per epoch
+            for i, (batch_x, batch_y, y_host) in enumerate(stream):
+                self.replay_step(batch_x, batch_y, y_host, meters=meters, **self._step_extras(ep * len(stream) + i))
+                yield
+                if meters is not None and i % 100 == 1:
+                    for fmt, keys in self._progress:
+                        print(fmt.format(i, *[meters[k].avg() for k in keys]))
+        self._end_task()
+        self._raise_errors()
+        yield from _after_train_steps(self)
+        self._end_call()
+
+    def _begin_task(self, n_batches):
+        """After before_train, before anything launches; n_batches: the stream's batches per epoch."""
+
+    def _step_extras(self, step):
+        """Keyword arguments of replay_step beyond the batch and the meters, at step `step` of the call (counted over
+        its epochs)."""
+        return {}
+
+    def _end_task(self):
+        """After the last replay step, before the error checks."""
+
+    def _raise_errors(self):
+        """The device error flags the task's steps may have set, read once per task."""
+        self._raise_label_errors()
 
     def forward(self, x):
         return self.model.forward(x)
@@ -692,7 +768,15 @@ def _set_mean(row_sums, n):
         return float(np.float32(np.float64(math.fsum(row_sums.tolist())) / np.float64(n)))
 
 
+# the progress lines (ContinualLearner._progress) most agents share
+_BATCH_LINE = ('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}', ('losses_batch', 'acc_batch'))
+_LOSS_LINE = ('==>>> it: {}, avg. loss: {:.6f}, ', ('losses',))
+
+
 class ExperienceReplay(ContinualLearner):
+    _progress = (_BATCH_LINE,
+                 ('==>>> it: {}, mem avg. loss: {:.6f}, running mem acc: {:.3f}', ('losses_mem', 'acc_mem')))
+
     def __init__(self, model, opt, params):
         super().__init__(model, opt, params)
         self.buffer = Buffer(model, params)
@@ -716,8 +800,7 @@ class ExperienceReplay(ContinualLearner):
                 if (kd or self._needs_batch_grad) else \
                 self.criterion(logits, batch_y, want_grad=self._needs_batch_grad, want_correct=meters is not None)   # :41-47
             if meters is not None:
-                meters['acc_batch'].update(ce['n_correct'] / batch_y.size(0), batch_y.size(0))
-                meters['losses_batch'].update(ce['loss'], batch_y.size(0))
+                _update_meters(meters, 'batch', ce, batch_y.size(0))
             if self._needs_batch_grad:
                 eng.backward(batch_x, ce['dlogits'], ws)                            # :54-55
             mem_x, mem_y = self.buffer.retrieve(x=batch_x, y=batch_y)               # :58
@@ -736,8 +819,7 @@ class ExperienceReplay(ContinualLearner):
                         else self.criterion(mem_logits, mem_y, want_grad=False))    # :63-70
             if mem_x.size(0) > 0 and not both:
                 if meters is not None:
-                    meters['losses_mem'].update(ce_m['loss'], mem_y.size(0))
-                    meters['acc_mem'].update(ce_m['n_correct'] / mem_y.size(0), mem_y.size(0))
+                    _update_meters(meters, 'mem', ce_m, mem_y.size(0))
                 if not aser:
                     eng.backward(mem_x, ce_m['dlogits'], ws_m, accumulate=True)     # :77 (gradients accumulate)
             if aser:
@@ -749,8 +831,7 @@ class ExperienceReplay(ContinualLearner):
                     eng.apply_running_stats(ws_m, mem_x.size(0))
                     eng.apply_running_stats(ws_c, combined.size(0))
                     if meters is not None:
-                        meters['losses_mem'].update(ce_m['loss'], mem_y.size(0))
-                        meters['acc_mem'].update(ce_m['n_correct'] / mem_y.size(0), mem_y.size(0))
+                        _update_meters(meters, 'mem', ce_m, mem_y.size(0))
                 ce_c = self.criterion(logits_c, labels)                             # :85 (no distillation term)
                 eng.backward(combined, ce_c['dlogits'], ws_c)                       # :86
                 self.last_loss = ce_c['loss']
@@ -763,28 +844,10 @@ class ExperienceReplay(ContinualLearner):
         self.buffer.update(batch_x, batch_y, y_host=batch_y_host)                   # :92
         self._throttle()
 
-    def _steps(self, x_train, y_train):
-        self._begin_call()
-        self.before_train(x_train, y_train)
-        self.engine.pack()          # the caller may have written the Parameters (load_state_dict, weight surgery)
-        self.model = self.model.train()
-        meters = {k: AverageMeter() for k in ('losses_batch', 'losses_mem', 'acc_batch', 'acc_mem')}
-        for ep in range(self.epoch):
-            stream = StreamFeeder(x_train, y_train, self.batch, self.device)   # DataLoader(shuffle=True): new order per epoch
-            for i, (batch_x, batch_y, y_host) in enumerate(stream):
-                self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
-                yield
-                if i % 100 == 1 and self.verbose:
-                    print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
-                          .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
-                    print('==>>> it: {}, mem avg. loss: {:.6f}, running mem acc: {:.3f}'
-                          .format(i, meters['losses_mem'].avg(), meters['acc_mem'].avg()))
-        self._raise_label_errors()
-        yield from _after_train_steps(self)
-        self._end_call()
-
 
 class SupContrastReplay(ContinualLearner):
+    _progress = (_LOSS_LINE,)
+
     def __init__(self, model, opt, params):
         nets.check_supcon(input_size_match[params.data][1], getattr(params, 'head', 'mlp'))   # before adopt() allocates
         super().__init__(model, opt, params)
@@ -837,27 +900,13 @@ class SupContrastReplay(ContinualLearner):
         self.buffer.update(batch_x, batch_y, y_host=batch_y_host)                   # :63
         self._throttle()
 
-    def _steps(self, x_train, y_train):
-        self._begin_call()
-        self.before_train(x_train, y_train)
-        self.engine.pack()          # the caller may have written the Parameters (load_state_dict, weight surgery)
-        self.model = self.model.train()
-        meters = {'losses': AverageMeter()}
-        for ep in range(self.epoch):
-            stream = StreamFeeder(x_train, y_train, self.batch, self.device)   # DataLoader(shuffle=True): new order per epoch
-            for i, (batch_x, batch_y, y_host) in enumerate(stream):
-                self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
-                yield
-                if i % 100 == 1 and self.verbose:
-                    print('==>>> it: {}, avg. loss: {:.6f}, '.format(i, meters['losses'].avg()))
-        yield from _after_train_steps(self)
-        self._end_call()
-
 
 class AGEM(ContinualLearner):
     """Averaged GEM (agents/agem.py:11-90) on the engine: the gradient of the stream batch is projected against the
     gradient of a memory batch of earlier tasks when their inner product is negative -- two train-mode
     forward / backward passes over the flat gradient arena and one projection kernel (no per-parameter Python loops)."""
+
+    _progress = (_BATCH_LINE,)
 
     def __init__(self, model, opt, params):
         super().__init__(model, opt, params)
@@ -875,8 +924,7 @@ class AGEM(ContinualLearner):
             logits, ws = eng.forward_train(batch_x, slot=0)                          # :39
             ce = self._kd_loss(logits, batch_y, batch_x, want_grad=True, want_correct=meters is not None)   # :40-46
             if meters is not None:
-                meters['acc_batch'].update(ce['n_correct'] / batch_y.size(0), batch_y.size(0))
-                meters['losses_batch'].update(ce['loss'], batch_y.size(0))
+                _update_meters(meters, 'batch', ce, batch_y.size(0))
             eng.backward(batch_x, ce['dlogits'], ws)                                 # :53-54
             self.last_loss = ce['loss']
             if self.task_seen > 0:
@@ -891,29 +939,13 @@ class AGEM(ContinualLearner):
         self.buffer.update(batch_x, batch_y, y_host=batch_y_host)                    # :83
         self._throttle()
 
-    def _steps(self, x_train, y_train):
-        self._begin_call()
-        self.before_train(x_train, y_train)
-        self.engine.pack()
-        self.model = self.model.train()
-        meters = {k: AverageMeter() for k in ('losses_batch', 'acc_batch')}
-        for ep in range(self.epoch):
-            stream = StreamFeeder(x_train, y_train, self.batch, self.device)
-            for i, (batch_x, batch_y, y_host) in enumerate(stream):
-                self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
-                yield
-                if i % 100 == 1 and self.verbose:
-                    print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
-                          .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
-        self._raise_label_errors()
-        yield from _after_train_steps(self)
-        self._end_call()
-
 
 class Lwf(ContinualLearner):
     """Learning without Forgetting (agents/lwf.py:10-56) on the engine: no memory; per batch one train-mode forward,
     loss = a * criterion + (1 - a) * distillation against the teacher taken after the previous task, a = 1/(task_seen+1),
     one backward pass and one SGD step.  Evaluation is the classifier's arg-max."""
+
+    _progress = (_BATCH_LINE,)
 
     def replay_step(self, batch_x, batch_y, batch_y_host, meters=None):
         """One iteration of lwf.py:30-46."""
@@ -922,30 +954,11 @@ class Lwf(ContinualLearner):
         logits, ws = eng.forward_train(batch_x, slot=0)                              # :35
         out = self._kd_loss(logits, batch_y, batch_x, want_grad=True, want_correct=meters is not None)   # :36-38
         if meters is not None:
-            meters['acc_batch'].update(out['n_correct'] / batch_y.size(0), batch_y.size(0))
-            meters['losses_batch'].update(out['loss'], batch_y.size(0))
+            _update_meters(meters, 'batch', out, batch_y.size(0))
         eng.backward(batch_x, out['dlogits'], ws)                                    # :45-46
         self._optimizer_step(spec)                                                 # :47
         self.last_loss = out['loss']
         self._throttle()
-
-    def _steps(self, x_train, y_train):
-        self._begin_call()
-        self.before_train(x_train, y_train)
-        self.engine.pack()
-        self.model = self.model.train()
-        meters = {k: AverageMeter() for k in ('losses_batch', 'acc_batch')}
-        for ep in range(self.epoch):
-            stream = StreamFeeder(x_train, y_train, self.batch, self.device)
-            for i, (batch_x, batch_y, y_host) in enumerate(stream):
-                self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
-                yield
-                if i % 100 == 1 and self.verbose:
-                    print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
-                          .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
-        self._raise_label_errors()
-        yield from _after_train_steps(self)
-        self._end_call()
 
 
 class Icarl(ContinualLearner):
@@ -1032,30 +1045,20 @@ class Icarl(ContinualLearner):
         self._updated[np.asarray(slots, dtype=np.int64)] = True
         self._throttle()
 
-    def _steps(self, x_train, y_train):
-        self._begin_call()
-        self.before_train(x_train, y_train)
+    def _begin_task(self, n_batches):
         K = self._pos[2] if self._pos is not None else 0
         if K > self.engine.out_dim:
             # replay_step's refusal, raised before this call launches anything (new-instance streams reach it at
             # their second task: every label recurs)
             raise ValueError('iCaRL: %d label positions exceed the %d logits' % (K, self.engine.out_dim))
-        self.engine.pack()
-        self.model = self.model.train()
         self._updated[:] = False                                                     # icarl.py:35, once per call
-        for ep in range(self.epoch):
-            stream = StreamFeeder(x_train, y_train, self.batch, self.device)
-            for batch_x, batch_y, y_host in stream:
-                self.replay_step(batch_x, batch_y, y_host)
-                yield
+
+    def _end_task(self):
         if self._pos_err is not None and int(self._pos_err.item()):
             self._pos_err.zero_()
             raise ValueError("iCaRL trained on a label outside the task's labels (icarl.py:44 raises there)")
         self.engine.update_teacher()                                                 # icarl.py:31, before after_train
         self._prev_live = True
-        self._raise_label_errors()
-        yield from _after_train_steps(self)
-        self._end_call()
 
 
 class Gdumb(ContinualLearner):
@@ -1070,9 +1073,7 @@ class Gdumb(ContinualLearner):
         if params.optimizer != 'SGD':
             # train_mem builds its own optimizer with setup_opt(params.optimizer, ...) (gdumb.py:63); the engine steps SGD
             raise NotImplementedError('GDumb on the b200ocl engine trains with SGD, not %r' % params.optimizer)
-        if (getattr(params, 'trick', None) or {}).get('ncm_trick'):
-            # the reference's nearest-class-mean evaluation reads self.buffer, which GDumb does not have
-            raise NotImplementedError('ncm_trick reads a buffer GDumb does not keep')
+        _refuse_options(params, 'the nearest-class-mean evaluation reads a buffer GDumb does not keep', ('ncm_trick',))
         super().__init__(model, opt, params)
         self._takes_teacher = False      # GDumb never reads a teacher
         # not named `buffer`: after_train runs the review trick when the learner has one, and for GDumb the reference does not
@@ -1141,21 +1142,8 @@ class Gdumb(ContinualLearner):
 
 
 def der_weights(params):
-    """(der_alpha, der_beta) of params as floats: each must be present, finite and >= 0 (ValueError otherwise; there is
-    no default)."""
-    out = []
-    for name in ('der_alpha', 'der_beta'):
-        v = getattr(params, name, None)
-        if v is None or isinstance(v, bool):
-            raise ValueError('DER++ needs params.%s (a finite number >= 0), got %r' % (name, v))
-        try:
-            f = float(v)
-        except (TypeError, ValueError):
-            raise ValueError('DER++ needs params.%s (a finite number >= 0), got %r' % (name, v)) from None
-        if not math.isfinite(f) or f < 0:
-            raise ValueError('DER++ needs params.%s (a finite number >= 0), got %r' % (name, v))
-        out.append(f)
-    return tuple(out)
+    """(der_alpha, der_beta) of params as floats, each finite and >= 0; there is no default."""
+    return tuple(_finite_param(params, name, 'DER++') for name in ('der_alpha', 'der_beta'))
 
 
 class DERPP(ContinualLearner):
@@ -1174,15 +1162,13 @@ class DERPP(ContinualLearner):
     der_alpha = 0 and der_beta = 1 every draw and every result bit is ER's (random retrieval, reservoir update).
     Evaluation is the inherited arg-max path."""
 
+    _progress = (_BATCH_LINE, ('==>>> it: {}, mem logit loss: {:.6f}, mem avg. loss: {:.6f}, running mem acc: {:.3f}',
+                               ('losses_logit', 'losses_mem', 'acc_mem')))
+
     def __init__(self, model, opt, params):
-        if params.update != 'random' or params.retrieve != 'random':
-            raise NotImplementedError('DER++ keeps each slot\'s logits beside it through the reservoir update and the '
-                                      'random retrieval (update=random, retrieve=random), not update=%r, retrieve=%r'
-                                      % (params.update, params.retrieve))
-        trick = getattr(params, 'trick', None) or {}
-        on = [k for k in ('labels_trick', 'separated_softmax', 'kd_trick', 'kd_trick_star') if trick.get(k)]
-        if on:
-            raise NotImplementedError('DER++ runs with plain cross-entropy; %s not implemented' % ', '.join(on))
+        _refuse_options(params, 'DER++ runs with plain cross-entropy', _CE_TRICKS,
+                        random_memory="DER++ keeps each slot's logits beside it through the reservoir update and the "
+                                      "random retrieval")
         alpha, beta = der_weights(params)
         super().__init__(model, opt, params)
         self.der_alpha, self.der_beta = alpha, beta
@@ -1200,8 +1186,7 @@ class DERPP(ContinualLearner):
             logits, ws = eng.forward_train(batch_x, slot=0)                          # 1. stream (BN stats move)
             ce = self.criterion(logits, batch_y, want_correct=meters is not None)
             if meters is not None:
-                meters['acc_batch'].update(ce['n_correct'] / batch_y.size(0), batch_y.size(0))
-                meters['losses_batch'].update(ce['loss'], batch_y.size(0))
+                _update_meters(meters, 'batch', ce, batch_y.size(0))
             eng.backward(batch_x, ce['dlogits'], ws)
             self.last_loss_logit = self.last_loss_mem = None
             if self.der_alpha != 0.0:                                                # 2. logit term
@@ -1221,46 +1206,16 @@ class DERPP(ContinualLearner):
                     eng.backward(mem_x, ce_m['dlogits'], ws2, accumulate=True)
                     self.last_loss_mem = ce_m['loss']
                     if meters is not None:
-                        meters['losses_mem'].update(ce_m['loss'], mem_y.size(0))
-                        meters['acc_mem'].update(ce_m['n_correct'] / mem_y.size(0), mem_y.size(0))
+                        _update_meters(meters, 'mem', ce_m, mem_y.size(0))
             self.last_loss = ce['loss']
             self._optimizer_step(spec)                                               # 4.
         self.buffer.update(batch_x, batch_y, logits=logits, y_host=batch_y_host)     # z_s of the last iteration
         self._throttle()
 
-    def _steps(self, x_train, y_train):
-        self._begin_call()
-        self.before_train(x_train, y_train)
-        self.engine.pack()          # the caller may have written the Parameters (load_state_dict, weight surgery)
-        self.model = self.model.train()
-        meters = {k: AverageMeter() for k in ('losses_batch', 'losses_logit', 'losses_mem', 'acc_batch', 'acc_mem')}
-        for ep in range(self.epoch):
-            stream = StreamFeeder(x_train, y_train, self.batch, self.device)   # DataLoader(shuffle=True): new order per epoch
-            for i, (batch_x, batch_y, y_host) in enumerate(stream):
-                self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
-                yield
-                if i % 100 == 1 and self.verbose:
-                    print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
-                          .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
-                    print('==>>> it: {}, mem logit loss: {:.6f}, mem avg. loss: {:.6f}, running mem acc: {:.3f}'
-                          .format(i, meters['losses_logit'].avg(), meters['losses_mem'].avg(), meters['acc_mem'].avg()))
-        self._raise_label_errors()
-        yield from _after_train_steps(self)
-        self._end_call()
-
 
 def pcr_temperature(params):
     """params.pcr_temp as a float, 0.09 when absent; ValueError unless it is finite and positive."""
-    v = getattr(params, 'pcr_temp', None)
-    if v is None:
-        return 0.09
-    try:
-        t = float(v) if not isinstance(v, bool) else float('nan')
-    except (TypeError, ValueError):
-        t = float('nan')
-    if not (math.isfinite(t) and t > 0):
-        raise ValueError('PCR needs params.pcr_temp to be a finite number > 0, got %r' % (v,))
-    return t
+    return _finite_param(params, 'pcr_temp', 'PCR', positive=True, default=0.09)
 
 
 class PCR(ContinualLearner):
@@ -1277,16 +1232,11 @@ class PCR(ContinualLearner):
     feature and each proxy (ops.cosine_argmax)."""
 
     _eval_cosine = True
+    _progress = (_LOSS_LINE,)
 
     def __init__(self, model, opt, params):
-        if params.update != 'random' or params.retrieve != 'random':
-            raise NotImplementedError('PCR runs with the random retrieval and the reservoir update (update=random, '
-                                      'retrieve=random), not update=%r, retrieve=%r' % (params.update, params.retrieve))
-        trick = getattr(params, 'trick', None) or {}
-        on = [k for k in ('labels_trick', 'separated_softmax', 'kd_trick', 'kd_trick_star', 'review_trick', 'ncm_trick')
-              if trick.get(k)]
-        if on:
-            raise NotImplementedError('PCR runs its proxy-contrastive loss alone; %s not implemented' % ', '.join(on))
+        _refuse_options(params, 'PCR runs its proxy-contrastive loss alone', _CE_TRICKS + ('review_trick', 'ncm_trick'),
+                        random_memory='PCR runs with the random retrieval and the reservoir update')
         temp = pcr_temperature(params)
         super().__init__(model, opt, params)
         self.temp = temp
@@ -1332,36 +1282,10 @@ class PCR(ContinualLearner):
         self.buffer.update(batch_x, batch_y, y_host=batch_y_host)
         self._throttle()
 
-    def _steps(self, x_train, y_train):
-        self._begin_call()
-        self.before_train(x_train, y_train)
-        self.engine.pack()          # the caller may have written the Parameters (load_state_dict, weight surgery)
-        self.model = self.model.train()
-        meters = {'losses': AverageMeter()}
-        for ep in range(self.epoch):
-            stream = StreamFeeder(x_train, y_train, self.batch, self.device)   # DataLoader(shuffle=True): new order per epoch
-            for i, (batch_x, batch_y, y_host) in enumerate(stream):
-                self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
-                yield
-                if i % 100 == 1 and self.verbose:
-                    print('==>>> it: {}, avg. loss: {:.6f}, '.format(i, meters['losses'].avg()))
-        self._raise_label_errors()
-        yield from _after_train_steps(self)
-        self._end_call()
-
 
 def gem_margin(params):
     """params.gem_margin as a float, 0.5 when absent; ValueError unless it is finite and >= 0."""
-    v = getattr(params, 'gem_margin', None)
-    if v is None:
-        return 0.5
-    try:
-        m = float(v) if not isinstance(v, bool) else float('nan')
-    except (TypeError, ValueError):
-        m = float('nan')
-    if not (math.isfinite(m) and m >= 0):
-        raise ValueError('GEM needs params.gem_margin to be a finite number >= 0, got %r' % (v,))
-    return m
+    return _finite_param(params, 'gem_margin', 'GEM', default=0.5)
 
 
 class GEM(ContinualLearner):
@@ -1380,16 +1304,11 @@ class GEM(ContinualLearner):
     MEM_SLOT = 2          # the memory passes' workspace (and graph) slot: one capture per row count
     EPS = 1e-3
 
+    _progress = (_BATCH_LINE,)
+
     def __init__(self, model, opt, params):
-        if params.update != 'random' or params.retrieve != 'random':
-            raise NotImplementedError('GEM keeps its own per-task memory (update=random, retrieve=random), not '
-                                      'update=%r, retrieve=%r' % (params.update, params.retrieve))
-        trick = getattr(params, 'trick', None) or {}
-        on = [k for k in ('labels_trick', 'separated_softmax', 'kd_trick', 'kd_trick_star', 'review_trick', 'ncm_trick')
-              if trick.get(k)]
-        if on:
-            raise NotImplementedError('GEM runs with plain cross-entropy and arg-max evaluation; %s not implemented'
-                                      % ', '.join(on))
+        _refuse_options(params, 'GEM runs with plain cross-entropy and arg-max evaluation',
+                        _CE_TRICKS + ('review_trick', 'ncm_trick'), random_memory='GEM keeps its own per-task memory')
         margin = gem_margin(params)
         M = int(params.mem_size) // int(params.num_tasks)
         if M < 1:
@@ -1444,8 +1363,7 @@ class GEM(ContinualLearner):
             ce = self.criterion(logits, batch_y, want_correct=meters is not None)
             eng.backward(batch_x, ce['dlogits'], ws)
             if meters is not None:
-                meters['acc_batch'].update(ce['n_correct'] / batch_y.size(0), batch_y.size(0))
-                meters['losses_batch'].update(ce['loss'], batch_y.size(0))
+                _update_meters(meters, 'batch', ce, batch_y.size(0))
             if t:                                                                     # 3.
                 ops.gem_project(G, t, eng.state.grads, out=eng.state.grads, margin=self.margin, eps=self.EPS,
                                 v=self._v, flag=self._flag, err=self._qp_err)
@@ -1454,34 +1372,22 @@ class GEM(ContinualLearner):
         self.rings.write(self._task, batch_x, batch_y, batch_y_host)
         self._throttle()
 
-    def _raise_qp_errors(self):
-        if int(self._qp_err.item()):
-            self._qp_err.zero_()
-            raise RuntimeError('GEM: the projection QP ran out of iterations (b200ocl_gem_project set its error flag)')
-
     def _steps(self, x_train, y_train):
+        # refused before anything else runs, the optimizer check included
         if self.task_seen > ops.GEM_MAX_T:
             raise ValueError('GEM projects against at most %d earlier tasks; this task has %d'
                              % (ops.GEM_MAX_T, self.task_seen))
-        self._begin_call()
-        self.before_train(x_train, y_train)
+        yield from super()._steps(x_train, y_train)
+
+    def _begin_task(self, n_batches):
         self._task = self.task_seen
         self.rings.begin_task(self._task)
-        self.engine.pack()          # the caller may have written the Parameters (load_state_dict, weight surgery)
-        self.model = self.model.train()
-        meters = {k: AverageMeter() for k in ('losses_batch', 'acc_batch')}
-        for ep in range(self.epoch):
-            stream = StreamFeeder(x_train, y_train, self.batch, self.device)   # DataLoader(shuffle=True): new order per epoch
-            for i, (batch_x, batch_y, y_host) in enumerate(stream):
-                self.replay_step(batch_x, batch_y, y_host, meters if self.verbose else None)
-                yield
-                if i % 100 == 1 and self.verbose:
-                    print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
-                          .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
-        self._raise_label_errors()
-        self._raise_qp_errors()
-        yield from _after_train_steps(self)
-        self._end_call()
+
+    def _raise_errors(self):
+        super()._raise_errors()
+        if int(self._qp_err.item()):
+            self._qp_err.zero_()
+            raise RuntimeError('GEM: the projection QP ran out of iterations (b200ocl_gem_project set its error flag)')
 
 
 def ewc_ema_schedule(n_batches, epochs, fisher_update_after):
@@ -1517,10 +1423,10 @@ class EWC_pp(ContinualLearner):
     Fisher.  running_fisher, tmp_fisher, normalized_fisher and prev_params are name -> view dicts over the EWC arenas,
     as the reference's dicts are.  There is no memory; evaluation is the inherited arg-max path."""
 
+    _progress = (_BATCH_LINE,)
+
     def __init__(self, model, opt, params):
-        if (getattr(params, 'trick', None) or {}).get('ncm_trick'):
-            # the reference's nearest-class-mean evaluation reads self.buffer, which EWC++ does not have
-            raise NotImplementedError('ncm_trick reads a buffer EWC++ does not keep')
+        _refuse_options(params, 'the nearest-class-mean evaluation reads a buffer EWC++ does not keep', ('ncm_trick',))
         super().__init__(model, opt, params)
         self.lambda_ = params.lambda_
         self.alpha = params.alpha
@@ -1568,31 +1474,16 @@ class EWC_pp(ContinualLearner):
                                    want_penalty=want)
         self.last_loss = out['loss']
         if meters is not None:
-            loss = out['loss'] if pen is None else out['loss'] + up * pen
-            meters['acc_batch'].update(out['n_correct'] / batch_y.size(0), batch_y.size(0))
-            meters['losses_batch'].update(loss, batch_y.size(0))
+            _update_meters(meters, 'batch', out, batch_y.size(0),
+                           loss=out['loss'] if pen is None else out['loss'] + up * pen)
         self._throttle()
 
-    def _steps(self, x_train, y_train):
-        self._begin_call()
-        self.before_train(x_train, y_train)
-        self.engine.pack()
-        self.model = self.model.train()
-        meters = {k: AverageMeter() for k in ('losses_batch', 'acc_batch')}
-        schedule = None
-        for ep in range(self.epoch):
-            stream = StreamFeeder(x_train, y_train, self.batch, self.device)
-            if schedule is None:
-                schedule = ewc_ema_schedule(len(stream), self.epoch, self.fisher_update_after)
-            for i, (batch_x, batch_y, y_host) in enumerate(stream):
-                self.replay_step(batch_x, batch_y, y_host, schedule[ep * len(stream) + i],
-                                 meters if self.verbose else None)
-                yield
-                if i % 100 == 1 and self.verbose:
-                    print('==>>> it: {}, avg. loss: {:.6f}, running train acc: {:.3f}'
-                          .format(i, meters['losses_batch'].avg(), meters['acc_batch'].avg()))
+    def _begin_task(self, n_batches):
+        self._ema = ewc_ema_schedule(n_batches, self.epoch, self.fisher_update_after)
+
+    def _step_extras(self, step):
+        return {'ema': self._ema[step]}
+
+    def _end_task(self):
         self.engine.ewc_consolidate()                                                # :71-78
         self._penalty_live = True
-        self._raise_label_errors()
-        yield from _after_train_steps(self)                                         # :79
-        self._end_call()
