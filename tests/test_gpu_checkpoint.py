@@ -1,11 +1,12 @@
 """GPU: an experiment interrupted by a Python exception and started again on the same checkpoint directory
 (B200OCL_CHECKPOINT_DIR) ends with what an uninterrupted one gives, bit for bit: the --store acc_array, the summary line,
-and every run's final parameters, BN statistics, memory, Adam moments and step and EWC++ arenas.  Three runs of three
-synthetic CIFAR-shaped tasks (test_gpu_multidevice.py's stub reference tree, written to tmp_path), at R = 1 and R = 3,
-interrupted from the on_task hook at (run 1, task 2) or from inside step 2 of task 1 of run 2 (which resumes from the
-end of task 0), for ER (random, ASER, MIR, GSS update), SCR, A-GEM, LwF with kd_trick, ER with the review trick and
-separated softmax, iCaRL, GDumb, EWC++ and ER with torch.optim.Adam.  main_tune.py's loop interrupted in its tuning
-stage chooses the same points, and runs on workers 0,0 resume like runs in process."""
+and every run's final state (agent_cases.final_state: parameters, BN statistics, the memory with DER++'s logits and
+GEM's rings, Adam moments and step, EWC++ arenas).  Three runs of three synthetic CIFAR-shaped tasks
+(test_gpu_multidevice.py's stub reference tree, written to tmp_path), at R = 1 and R = 3, interrupted from the on_task
+hook at (run 1, task 2) or from inside step 2 of task 1 of run 2 (which resumes from the end of task 0), for
+RESUME_CASES of agent_cases.CASES: ER (random, ASER, MIR, GSS update), SCR, A-GEM, LwF with kd_trick, ER with the review
+trick and separated softmax, iCaRL, GDumb, EWC++, ER with torch.optim.Adam, DER++, PCR and GEM.  main_tune.py's loop
+interrupted in its tuning stage chooses the same points, and runs on workers 0,0 resume like runs in process."""
 import multiprocessing
 import os
 import pickle
@@ -18,25 +19,14 @@ import torch
 
 from b200ocl import multirun
 
+import agent_cases
 import test_gpu_multidevice as md
 
 pytestmark = pytest.mark.gpu
 
 N_RUNS = 3
-CASES = {
-    'er_random': dict(),
-    'er_aser': dict(update='ASER', retrieve='ASER'),
-    'er_mir': dict(retrieve='MIR'),
-    'er_gss': dict(update='GSS'),
-    'scr': dict(agent='SCR'),
-    'agem': dict(agent='AGEM'),
-    'lwf_kd': dict(agent='LWF', trick_on=('kd_trick',)),
-    'er_review_sep': dict(trick_on=('review_trick', 'separated_softmax')),
-    'icarl': dict(agent='ICARL', mem_size=100),
-    'gdumb': dict(agent='GDUMB'),
-    'ewc': dict(agent='EWC'),
-    'er_adam': dict(optimizer='Adam', learning_rate=1e-3),
-}
+RESUME_CASES = ('er_random', 'er_aser', 'er_mir', 'er_gss', 'scr', 'agem', 'lwf_kd', 'er_review_sep', 'icarl', 'gdumb',
+                'ewc', 'er_adam', 'derpp', 'pcr', 'gem')
 
 TREE = dict(md.STUB_TREE)
 TREE['utils/setup_elements.py'] = '''
@@ -53,25 +43,10 @@ TREE['utils/name_match.py'] = '''
     import os
 
     import torch
+    from agent_cases import final_state
     from b200ocl import registry
 
     from continuum.continuum import LAST_RUN
-
-
-    def final_state(agent):
-        """What must match: the arenas (parameters, BN statistics and counters, Adam, EWC++) and the memory."""
-        eng = agent.engine
-        out = [eng.state.params, eng.state.bn_stats, eng.state.bn_tracked]
-        adam, ewc = getattr(eng, '_adam', None), getattr(eng, '_ewc', None)
-        if adam is not None:
-            out += [adam.exp_avg, adam.exp_avg_sq, torch.tensor(adam.step)]
-        if ewc is not None:
-            out += [ewc.running, ewc.tmp, ewc.normalized, ewc.prev]
-        if hasattr(agent, 'buffer'):
-            out += [agent.buffer.buffer_img, agent.buffer.buffer_label]
-        if hasattr(agent, 'memory'):
-            out += [agent.memory.images, agent.memory.labels]
-        return [t.detach().cpu().clone() for t in out]
 
 
     _recording = {}
@@ -144,12 +119,8 @@ def stub_tree(monkeypatch, tmp_path):
 
 
 def _params(case):
-    p = md._params('er_random')
-    over = dict(CASES[case])
-    trick_on = over.pop('trick_on', ())
-    p.trick = {k: k in trick_on for k in p.trick}
-    vars(p).update(num_runs=N_RUNS, gss_mem_strength=10, gss_batch_size=10, lambda_=100.0, alpha=0.9,
-                   fisher_update_after=2, **over)
+    p = md._params(case)
+    p.num_runs = N_RUNS
     return p
 
 
@@ -183,13 +154,13 @@ _PLAIN = {}
 def _install(case):
     from b200ocl import registry
     import utils.name_match as nm
-    registry.install(nm, extra=('EWC',) if case == 'ewc' else ())
+    registry.install(nm, extra=agent_cases.extra(case))
     return lambda: registry.uninstall(nm)
 
 
 @pytest.mark.parametrize('how', ['on_task', 'step'])
 @pytest.mark.parametrize('R', [1, 3])
-@pytest.mark.parametrize('case', sorted(CASES))
+@pytest.mark.parametrize('case', sorted(RESUME_CASES))
 def test_a_resumed_experiment_matches_an_uninterrupted_one(case, R, how, stub_tree, monkeypatch, capsys):
     uninstall = _install(case)
     try:

@@ -9,17 +9,17 @@
   * Whole DER++ and DER steps against oracle/derpp.py (fp64) at CIFAR-100, CORe50 and OpenLORIS shapes, with
     test_gpu_replay.py::test_er_random_steps's tolerances; after every update each written slot's logit row is the
     matching row of the last stream forward's logits, bit for bit.  Two-task CORe50 and OpenLORIS runs evaluate.
-  * Adam's state in opt.state; an experiment interrupted after its first task resumes bit for bit, with and without
-    B200OCL_CHECKPOINT_ASYNC=1; multirun at R = 2 gives R = 1's bits."""
-import os
-import sys
-import textwrap
+  * Adam's state in opt.state.
+Checkpoint resume, staged snapshots, concurrent runs and graphs against eager launches are checked with the other
+agents, as agent_cases.CASES['derpp'] (test_gpu_checkpoint.py, test_gpu_checkpoint_async.py, test_gpu_multirun.py,
+test_gpu_graphs.py)."""
 from types import SimpleNamespace
 
 import numpy as np
 import pytest
 import torch
 
+from agent_cases import HW, NCLS, _learner, _load
 from oracle import derpp as oder
 from oracle import resnet as oresnet
 
@@ -96,24 +96,6 @@ def make_params(**kw):
     return SimpleNamespace(**base)
 
 
-HW = {'cifar100': 32, 'core50': 128, 'openloris': 50}
-NCLS = {'cifar100': 100, 'core50': 50, 'openloris': 69}
-
-
-def _load(agent, p, bn, spec):
-    agent.engine.load(list(p.values()), [(bn[n + '.running_mean'], bn[n + '.running_var']) for n in oresnet.bn_names(spec)])
-
-
-def _learner(b, params, seed, opt=None):
-    spec = oresnet.Spec(HW[params.data], 20, NCLS[params.data])
-    p0, bn0 = oresnet.seeded_state(spec, seed)
-    model = b.nets.setup_architecture(params)
-    cls = b.registry.agents.get(params.agent) or b.registry.extra_agents[params.agent]
-    agent = cls(model, opt(model) if opt else None, params)
-    _load(agent, p0, bn0, spec)
-    return agent, spec
-
-
 def _task(rs, n, labels, hw):
     x = rs.randint(0, 256, (n, hw, hw, 3)).astype(np.uint8)
     return x, rs.choice(np.asarray(list(labels)), n)
@@ -131,7 +113,7 @@ def test_alpha_0_beta_1_is_er_bit_for_bit(b):
     results = []
     for agent_name in ('ER', 'DERPP'):
         params = make_params(agent=agent_name, der_alpha=0.0, der_beta=1.0, mem_size=50)
-        agent, _ = _learner(b, params, 31)
+        agent, _ = _learner(params, 31)
         rs = np.random.RandomState(5)
         tasks = [_task(rs, 73, range(4 * t, 4 * t + 4), 32) for t in range(3)]
         loaders = _loaders(rs, 32, [range(4 * t, 4 * t + 4) for t in range(3)])
@@ -177,7 +159,7 @@ def _written_rows(b, buf, s0, n, mem):
 
 def _steps_against_oracle(b, data, alpha, beta, n_steps, seed):
     params = make_params(data=data, der_alpha=alpha, der_beta=beta, mem_size=30)
-    agent, spec = _learner(b, params, seed)
+    agent, spec = _learner(params, seed)
     hw, ncls = HW[data], NCLS[data]
     p64, bn64 = oresnet.seeded_state(spec, seed, dtype=torch.float64)
     st = oder.DerState(spec, p64, bn64, params.mem_size, (3, hw, hw), ncls, lr=params.learning_rate)
@@ -232,7 +214,7 @@ def test_steps_against_oracle_core50_openloris(b, data):
 @pytest.mark.parametrize('data', ['core50', 'openloris'])
 def test_two_task_run_evaluates(b, data):
     params = make_params(data=data, mem_size=40)
-    agent, _ = _learner(b, params, 9)
+    agent, _ = _learner(params, 9)
     hw = HW[data]
     rs = np.random.RandomState(3)
     # CORe50: new classes per task; OpenLORIS: new instances of the same classes
@@ -249,7 +231,7 @@ def test_two_task_run_evaluates(b, data):
 
 def test_adam_state_is_the_engines(b):
     params = make_params(optimizer='Adam', learning_rate=1e-3)
-    agent, _ = _learner(b, params, 11, opt=lambda m: torch.optim.Adam(m.parameters(), lr=1e-3))
+    agent, _ = _learner(params, 11, opt=lambda m: torch.optim.Adam(m.parameters(), lr=1e-3))
     rs = np.random.RandomState(4)
     agent.train_learner(*_task(rs, 33, range(5), 32))
     opt, st = agent.opt, agent.engine.adam_state()
@@ -261,85 +243,3 @@ def test_adam_state_is_the_engines(b):
         assert s['exp_avg'].data_ptr() == st.exp_avg[o:o + k].data_ptr()
         assert s['exp_avg_sq'].data_ptr() == st.exp_avg_sq[o:o + k].data_ptr()
     assert float(st.exp_avg_sq.abs().max()) > 0
-
-
-# ----------------------------------------------------------------------------- experiments (checkpoints, multirun)
-import test_gpu_checkpoint as ck                                                   # noqa: E402
-import test_gpu_multidevice as md                                                  # noqa: E402
-
-TREE = dict(ck.TREE)
-TREE['utils/name_match.py'] = ck.TREE['utils/name_match.py'].replace(
-    "out += [agent.buffer.buffer_img, agent.buffer.buffer_label]",
-    "out += [agent.buffer.buffer_img, agent.buffer.buffer_label, agent.buffer.buffer_logits]")
-assert TREE['utils/name_match.py'] != ck.TREE['utils/name_match.py']
-
-
-@pytest.fixture
-def stub_tree(monkeypatch, tmp_path):
-    if not torch.cuda.is_available():
-        pytest.skip('no CUDA device')
-    from b200ocl import checkpoint, multirun
-    ref = tmp_path / 'reference'
-    for rel, src in TREE.items():
-        (ref / rel).parent.mkdir(parents=True, exist_ok=True)
-        (ref / rel).write_text(textwrap.dedent(src))
-    saved = {k: v for k, v in sys.modules.items() if k.split('.')[0] in md.PACKAGES}
-    for k in saved:
-        del sys.modules[k]
-    monkeypatch.syspath_prepend(str(ref))
-    monkeypatch.chdir(tmp_path)
-    for k in (multirun.ENV, multirun.DEVICES_ENV, checkpoint.ENV, checkpoint.ASYNC_ENV, 'CHECKPOINT_FAIL_STEP'):
-        monkeypatch.delenv(k, raising=False)
-    from b200ocl import registry
-    import utils.name_match as nm
-    registry.install(nm, extra=('DERPP',))
-    yield tmp_path
-    registry.uninstall(nm)
-    for k in [k for k in sys.modules if k.split('.')[0] in md.PACKAGES]:
-        del sys.modules[k]
-    sys.modules.update(saved)
-
-
-def _experiment(R, name, d, monkeypatch, capsys):
-    from b200ocl import multirun
-    params = ck._params('er_random')
-    vars(params).update(agent='DERPP', der_alpha=0.3, der_beta=0.5)
-    out = os.path.join(os.getcwd(), 'states_' + name)
-    os.makedirs(out, exist_ok=True)
-    monkeypatch.setenv('CHECKPOINT_OUT', out)
-    multirun.multiple_run(params, store=True, save_path=name + '.pkl', n_concurrent=R, checkpoint_dir=d)
-    torch.cuda.synchronize()
-    lines = capsys.readouterr().out.splitlines()
-    import pickle
-    with open('result/cifar10/%s.pkl' % name, 'rb') as f:
-        acc = pickle.load(f)['acc_array']
-    return acc, lines[-1], [torch.load(os.path.join(out, 'run%d.pt' % r)) for r in range(ck.N_RUNS)]
-
-
-@pytest.mark.parametrize('asynchronous', [False, True], ids=['sync', 'async'])
-def test_a_resumed_experiment_matches_an_uninterrupted_one(stub_tree, monkeypatch, capsys, asynchronous):
-    from b200ocl import checkpoint, multirun
-    want = _experiment(1, 'plain', '', monkeypatch, capsys)
-    d = str(stub_tree / 'ck')
-    if asynchronous:
-        monkeypatch.setenv(checkpoint.ASYNC_ENV, '1')
-    on_task = multirun._Repetitions.on_task
-
-    def failing(self, r, t, x, y):
-        if (r, t) == (0, 1):
-            raise ck.Interrupt('run 0, task 1')
-        return on_task(self, r, t, x, y)
-    monkeypatch.setattr(multirun._Repetitions, 'on_task', failing)
-    with pytest.raises(ck.Interrupt):
-        _experiment(1, 'resumed', d, monkeypatch, capsys)
-    monkeypatch.setattr(multirun._Repetitions, 'on_task', on_task)
-    assert sorted(os.listdir(os.path.join(d, 'runs'))) == ['run0.snapshot']
-    got = _experiment(1, 'resumed', d, monkeypatch, capsys)
-    assert sorted(os.listdir(os.path.join(d, 'runs'))) == ['run%d.record' % r for r in range(ck.N_RUNS)]
-    ck._same(got, want, ('DERPP', asynchronous))
-
-
-def test_two_runs_at_once_give_one_at_a_times_bits(stub_tree, monkeypatch, capsys):
-    want = _experiment(1, 'one', '', monkeypatch, capsys)
-    got = _experiment(2, 'two', '', monkeypatch, capsys)
-    ck._same(got, want, 'R = 2')

@@ -18,10 +18,12 @@
     2e-4 and BN statistics 1e-4 of their largest element (looser for mem_iters = 2 and Adam, below); the rings bit for
     bit.
   * Three-task runs of registry.extra_agents['GEM'] on CIFAR-100-shaped data: the rings bit-equal to a restatement of
-    the ring rule over the stream's order; B200OCL_GRAPHS=0 against graphs, checkpoint resume (synchronous and
-    asynchronous) and R = 2 against R = 1, bit for bit.
+    the ring rule over the stream's order.
   * The Gram, QP and projection checks again at 114, 60 and 16 SMs (B200OCL_SM_COUNT, one child process per count,
     tests/gem_sm_counts_child.py), whose lengths reach every geometry the plan takes at that count.
+Checkpoint resume, staged snapshots, concurrent runs and graphs against eager launches, the rings included, are checked
+with the other agents, as agent_cases.CASES['gem'] (test_gpu_checkpoint.py, test_gpu_checkpoint_async.py,
+test_gpu_multirun.py, test_gpu_graphs.py).
 
 Worst values per check, measured on an H100 80GB HBM3 (SXM, 132 SMs, 700 W power limit), the same at 114, 60 and 16
 SMs where the check runs there: Gram |kernel - fp64| 0.054 of its bar; QP objective 7.2e-16 relative, dual KKT
@@ -33,13 +35,13 @@ import json
 import os
 import subprocess
 import sys
-import textwrap
 from types import SimpleNamespace
 
 import numpy as np
 import pytest
 import torch
 
+from agent_cases import HW, NCLS, _learner, _load
 from oracle import agem as oagem
 from oracle import gem as ogem
 from oracle import resnet as oresnet
@@ -288,10 +290,6 @@ def test_refusals(b):
 
 
 # ----------------------------------------------------------------------------- the learner against the oracle
-HW = {'cifar100': 32, 'mini_imagenet': 84, 'core50': 128, 'openloris': 50}
-NCLS = {'cifar100': 100, 'mini_imagenet': 100, 'core50': 50, 'openloris': 69}
-
-
 def make_params(**kw):
     base = dict(data='cifar100', cuda=True, epoch=1, batch=10, verbose=False, mem_size=20, eps_mem_batch=10,
                 mem_iters=1, update='random', retrieve='random', agent='GEM', num_tasks=5, buffer_tracker=False,
@@ -300,19 +298,6 @@ def make_params(**kw):
                        'ncm_trick': False, 'kd_trick_star': False})
     base.update(kw)
     return SimpleNamespace(**base)
-
-
-def _load(agent, p, bn, spec):
-    agent.engine.load(list(p.values()), [(bn[n + '.running_mean'], bn[n + '.running_var']) for n in oresnet.bn_names(spec)])
-
-
-def _learner(b, params, seed, opt=None):
-    spec = oresnet.Spec(HW[params.data], 20, NCLS[params.data])
-    p0, bn0 = oresnet.seeded_state(spec, seed)
-    model = b.nets.setup_architecture(params)
-    agent = b.registry.extra_agents['GEM'](model, opt(model) if opt else None, params)
-    _load(agent, p0, bn0, spec)
-    return agent, spec
 
 
 # mem_iters = 2: the second iteration of a step runs from the first one's fp32 weights against the oracle's fp64 ones,
@@ -334,7 +319,7 @@ def _steps_against_oracle(b, data, seed, tasks=4, steps_per_task=3, adam=False, 
     params = make_params(data=data, **kw)
     opt = (lambda m: torch.optim.Adam(m.parameters(), lr=params.learning_rate,
                                       weight_decay=params.weight_decay)) if adam else None
-    agent, spec = _learner(b, params, seed, opt=opt)
+    agent, spec = _learner(params, seed, opt=opt)
     hw, ncls = HW[data], NCLS[data]
     p64, bn64 = oresnet.seeded_state(spec, seed, dtype=torch.float64)
     st = ogem.ors.ReplayState(spec, p64, bn64, 1, (3, hw, hw), ncls, lr=params.learning_rate,
@@ -420,7 +405,7 @@ def _task(rs, n, labels, hw):
 
 def test_three_task_run_keeps_the_rings_of_the_restatement(b):
     params = make_params(mem_size=75, num_tasks=3)
-    agent, _ = _learner(b, params, 9)
+    agent, _ = _learner(params, 9)
     rs = np.random.RandomState(3)
     M = 25
     loaders = []
@@ -447,102 +432,6 @@ def test_three_task_run_keeps_the_rings_of_the_restatement(b):
         assert torch.equal(agent.rings.images[t].cpu(), want_x)
         assert np.array_equal(agent.rings.labels[t].cpu().numpy(), want_y)
     assert agent.task_seen == 3 and len(agent.rings) == 3
-
-
-def _run_task_bits(b, graphs):
-    b.engine.set_graphs(graphs)
-    try:
-        params = make_params(mem_size=60, num_tasks=3)
-        agent, _ = _learner(b, params, 12)
-        rs = np.random.RandomState(6)
-        for t in range(3):
-            np.random.seed(t); torch.manual_seed(t)
-            agent.train_learner(*_task(rs, 60, range(5 * t, 5 * t + 5), 32))
-        torch.cuda.synchronize()
-        eng = agent.engine
-        return [eng.state.params.cpu(), eng.state.bn_stats.cpu()] + [im.cpu() for im in agent.rings.images]
-    finally:
-        b.engine.set_graphs(True)
-
-
-def test_graphs_off_gives_the_graphed_bits(b):
-    on, off = _run_task_bits(b, True), _run_task_bits(b, False)
-    for i, (x, y) in enumerate(zip(on, off)):
-        assert torch.equal(x, y), i
-
-
-import test_gpu_checkpoint as ck                                                   # noqa: E402
-import test_gpu_multidevice as md                                                  # noqa: E402
-
-
-@pytest.fixture
-def stub_tree(monkeypatch, tmp_path):
-    if not torch.cuda.is_available():
-        pytest.skip('no CUDA device')
-    from b200ocl import checkpoint, multirun
-    ref = tmp_path / 'reference'
-    for rel, src in ck.TREE.items():
-        (ref / rel).parent.mkdir(parents=True, exist_ok=True)
-        (ref / rel).write_text(textwrap.dedent(src))
-    saved = {k: v for k, v in sys.modules.items() if k.split('.')[0] in md.PACKAGES}
-    for k in saved:
-        del sys.modules[k]
-    monkeypatch.syspath_prepend(str(ref))
-    monkeypatch.chdir(tmp_path)
-    for k in (multirun.ENV, multirun.DEVICES_ENV, checkpoint.ENV, checkpoint.ASYNC_ENV, 'CHECKPOINT_FAIL_STEP'):
-        monkeypatch.delenv(k, raising=False)
-    from b200ocl import registry
-    import utils.name_match as nm
-    registry.install(nm, extra=('GEM',))
-    yield tmp_path
-    registry.uninstall(nm)
-    for k in [k for k in sys.modules if k.split('.')[0] in md.PACKAGES]:
-        del sys.modules[k]
-    sys.modules.update(saved)
-
-
-def _experiment(R, name, d, monkeypatch, capsys):
-    from b200ocl import multirun
-    params = ck._params('er_random')
-    vars(params).update(agent='GEM', gem_margin=0.5)
-    out = os.path.join(os.getcwd(), 'states_' + name)
-    os.makedirs(out, exist_ok=True)
-    monkeypatch.setenv('CHECKPOINT_OUT', out)
-    multirun.multiple_run(params, store=True, save_path=name + '.pkl', n_concurrent=R, checkpoint_dir=d)
-    torch.cuda.synchronize()
-    lines = capsys.readouterr().out.splitlines()
-    import pickle
-    with open('result/cifar10/%s.pkl' % name, 'rb') as f:
-        acc = pickle.load(f)['acc_array']
-    return acc, lines[-1], [torch.load(os.path.join(out, 'run%d.pt' % r)) for r in range(ck.N_RUNS)]
-
-
-@pytest.mark.parametrize('asynchronous', [False, True], ids=['sync', 'async'])
-def test_a_resumed_experiment_matches_an_uninterrupted_one(stub_tree, monkeypatch, capsys, asynchronous):
-    from b200ocl import checkpoint, multirun
-    want = _experiment(1, 'plain', '', monkeypatch, capsys)
-    d = str(stub_tree / 'ck')
-    if asynchronous:
-        monkeypatch.setenv(checkpoint.ASYNC_ENV, '1')
-    on_task = multirun._Repetitions.on_task
-
-    def failing(self, r, t, x, y):
-        if (r, t) == (0, 2):
-            raise ck.Interrupt('run 0, task 2')
-        return on_task(self, r, t, x, y)
-    monkeypatch.setattr(multirun._Repetitions, 'on_task', failing)
-    with pytest.raises(ck.Interrupt):
-        _experiment(1, 'resumed', d, monkeypatch, capsys)
-    monkeypatch.setattr(multirun._Repetitions, 'on_task', on_task)
-    assert sorted(os.listdir(os.path.join(d, 'runs'))) == ['run0.snapshot']
-    got = _experiment(1, 'resumed', d, monkeypatch, capsys)
-    ck._same(got, want, ('GEM', asynchronous))
-
-
-def test_two_runs_at_once_give_one_at_a_times_bits(stub_tree, monkeypatch, capsys):
-    want = _experiment(1, 'one', '', monkeypatch, capsys)
-    got = _experiment(2, 'two', '', monkeypatch, capsys)
-    ck._same(got, want, 'R = 2')
 
 
 # ----------------------------------------------------------------------------- other SM counts

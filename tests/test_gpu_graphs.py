@@ -16,7 +16,8 @@ less than equality is expected.
   * launch accounting: a replay stands for exactly the launches of the eager call (graph_launch_count, bench.py);
   * the backward's weight gradients on the side stream, serially (B200OCL_WG_ASYNC=0), under the per-launch profiler
     and from a fifth caller stream that gets no side-stream slot, each in a fresh process, bit for bit;
-  * whole agents (test_gpu_multirun.CASES and GSS) over a short seeded stream with graphs on and off."""
+  * whole agents (test_gpu_multirun.RUN_CASES and ER with the GSS update) over a short seeded stream with graphs on and
+    off."""
 import json
 import os
 import subprocess
@@ -27,6 +28,7 @@ import numpy as np
 import pytest
 import torch
 
+import agent_cases
 import test_gpu_backward_fp64 as bwd
 import test_gpu_core50 as core50
 import test_gpu_forward_fp64 as fwd
@@ -483,16 +485,8 @@ def test_weight_gradients_serial_and_side_stream_are_the_same_bits(engine, tmp_p
 
 
 # ----------------------------------------------------------------------------- whole agents
-AGENT_CASES = sorted(mr.CASES) + ['gss']
+AGENT_CASES = sorted(mr.RUN_CASES + ('er_gss',))
 AGENT_KEYS = set()
-
-
-def _agent_params(case):
-    if case == 'gss':
-        p = mr._params('er_random')
-        p.update, p.gss_mem_strength, p.gss_batch_size = 'GSS', 10, 10
-        return p
-    return mr._params(case)
 
 
 def _agent_run(engine, case, graphs, r=2):
@@ -501,7 +495,7 @@ def _agent_run(engine, case, graphs, r=2):
     memory.flush_pending()
     memory.ClassBalancedRandomSampling.reset()
     multirun.RunRng(multirun.run_seed(mr.SEED, r)).swap_in()
-    agent = mr._maker(_agent_params(case), {})(r)
+    agent = mr._maker(agent_cases.params(case), {})(r)
     tasks, loaders = mr._data(r)
     acc = []
     for x, y in tasks:
@@ -509,13 +503,13 @@ def _agent_run(engine, case, graphs, r=2):
         acc.append(agent.evaluate(loaders))
     torch.cuda.synchronize()
     memory.flush_pending()
-    return np.array(acc), mr._final(agent), agent.engine._graphs
+    return np.array(acc), agent_cases.final_state(agent), agent.engine._graphs
 
 
 @pytest.mark.parametrize('case', AGENT_CASES)
 def test_agents_with_and_without_graphs(engine, case):
-    """A short seeded stream (three tasks of three calls) with graphs on and off: accuracies, parameter arena, BN
-    statistics and counters and the memory, bit for bit."""
+    """A short seeded stream (three tasks of three calls) with graphs on and off: accuracies and final state
+    (agent_cases.final_state), bit for bit."""
     acc_g, final_g, graphs = _agent_run(engine, case, True)
     acc_e, final_e, eager = _agent_run(engine, case, False)
     assert not eager
@@ -523,7 +517,7 @@ def test_agents_with_and_without_graphs(engine, case):
     AGENT_KEYS.update(graphs)
     assert np.array_equal(acc_g, acc_e), (case, acc_g, acc_e)
     assert len(final_g) == len(final_e)
-    for i, (a, b) in enumerate(zip(final_g, final_e)):     # params, bn_stats, bn_tracked, then the memory's tensors
+    for i, (a, b) in enumerate(zip(final_g, final_e)):     # params, bn_stats, bn_tracked, then the rest of final_state
         assert _same_bits(a, b), (case, i, _diff(a, b))
     RAN.add(('agent', case))
 

@@ -1,15 +1,15 @@
 """GPU: the experiment drivers on worker processes (B200OCL_RUN_DEVICES) against the in-process wrapper, on real engine
-agents behind a stub reference tree written to tmp_path (spawned workers import it from sys.path).  Six runs of ER
-(random), ER + ASER, SCR with the review trick and GDumb on workers 0,0 at R = 1 and R = 2 per worker: every run's
-accuracy arrays, final parameter arena, BN statistics and memory contents are bit-identical to the in-process run_group
-at R = 1 with the same (seed, r).  main_tune.py's loop on the same 2 x 2 grid and data as test_gpu_multirun_tune.py
-gives the same chosen points and arrays on workers as in process.  Workers 0,1 run only with two devices."""
+agents behind a stub reference tree written to tmp_path (spawned workers import it, and agent_cases.py, from the
+sys.path they inherit).  Six runs of ER (random), ER + ASER, SCR with the review trick and GDumb (WORKER_CASES of
+agent_cases.CASES) on workers 0,0 at R = 1 and R = 2 per worker: every run's accuracy arrays and final state
+(agent_cases.final_state) are bit-identical to the in-process run_group at R = 1 with the same (seed, r).
+main_tune.py's loop on the same 2 x 2 grid and data as test_gpu_multirun_tune.py gives the same chosen points and arrays
+on workers as in process.  Workers 0,1 run only with two devices."""
 import multiprocessing
 import os
 import pickle
 import sys
 import textwrap
-from types import SimpleNamespace
 
 import numpy as np
 import pytest
@@ -17,15 +17,12 @@ import torch
 
 from b200ocl import multirun
 
+import agent_cases
+
 pytestmark = pytest.mark.gpu
 
 SEED, N_RUNS = 11, 6
-CASES = {
-    'er_random': dict(),
-    'er_aser': dict(update='ASER', retrieve='ASER'),
-    'scr': dict(agent='SCR', trick_on=('review_trick',)),
-    'gdumb': dict(agent='GDUMB'),
-}
+WORKER_CASES = ('er_random', 'er_aser', 'scr_review', 'gdumb')
 TUNE_GRID = {'learning_rate': [0.05, 0.1], 'weight_decay': [0.0, 1e-3]}
 
 STUB_TREE = {
@@ -130,20 +127,10 @@ STUB_TREE = {
         import os
 
         import torch
+        from agent_cases import final_state
         from b200ocl import registry
 
         from continuum.continuum import LAST_RUN
-
-
-        def final_state(agent):
-            """What must match: the parameter arena, the BN statistics (and counters), the memory."""
-            eng = agent.engine
-            out = [eng.state.params, eng.state.bn_stats, eng.state.bn_tracked]
-            if hasattr(agent, 'buffer'):
-                out += [agent.buffer.buffer_img, agent.buffer.buffer_label]
-            if hasattr(agent, 'memory'):
-                out += [agent.memory.images, agent.memory.labels]
-            return [t.detach().cpu().clone() for t in out]
 
 
         _recording = {}
@@ -204,16 +191,11 @@ def stub_tree(monkeypatch, tmp_path):
 
 
 def _params(case):
-    over = dict(CASES[case])
-    trick = {k: k in over.pop('trick_on', ()) for k in ('labels_trick', 'kd_trick', 'separated_softmax', 'review_trick',
-                                                         'ncm_trick', 'kd_trick_star')}
-    base = dict(data='cifar10', cl_type='nc', cuda=True, epoch=1, batch=10, verbose=False, mem_size=20,
-                eps_mem_batch=10, mem_iters=1, update='random', retrieve='random', agent='ER', k=3, aser_type='asvm',
-                n_smp_cls=1.5, num_tasks=3, buffer_tracker=False, optimizer='SGD', learning_rate=0.1, weight_decay=0,
-                temp=0.07, head='mlp', subsample=20, error_analysis=False, mem_epoch=2, clip=10.0, test_batch=128,
-                trick=trick, num_runs=N_RUNS, seed=SEED, online=True, model_name='M', data_name='D', stub_data='runs')
-    base.update(over)
-    return SimpleNamespace(**base)
+    """agent_cases.params(case) with the fields of a multiple_run experiment on the stub tree."""
+    p = agent_cases.params(case)
+    vars(p).update(cl_type='nc', num_runs=N_RUNS, seed=SEED, online=True, model_name='M', data_name='D',
+                   stub_data='runs')
+    return p
 
 
 def _experiment(case, devices, R, out, monkeypatch):
@@ -233,7 +215,7 @@ _SOLO = {}
 def _check(case, devices, R, tmp_path, monkeypatch):
     from b200ocl import registry
     import utils.name_match as nm
-    registry.install(nm)
+    registry.install(nm, extra=agent_cases.extra(case))
     try:
         if case not in _SOLO:
             _SOLO[case] = _experiment(case, (), 1, tmp_path / 'solo', monkeypatch)
@@ -251,7 +233,7 @@ def _check(case, devices, R, tmp_path, monkeypatch):
 
 
 @pytest.mark.parametrize('R', [1, 2])
-@pytest.mark.parametrize('case', sorted(CASES))
+@pytest.mark.parametrize('case', sorted(WORKER_CASES))
 def test_runs_on_two_workers_match_in_process_runs_bit_for_bit(case, R, stub_tree, monkeypatch, capsys):
     _check(case, (0, 0), R, stub_tree, monkeypatch)
 

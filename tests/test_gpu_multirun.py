@@ -1,45 +1,24 @@
 """GPU: runs trained side by side (multirun.run_group, R = 3, three groups) give every run, bit for bit, what it gives
-alone (R = 1, the same (seed, r)): accuracy arrays, final parameter arena, BN statistics and buffer contents, for ER
-(random, ASER, MIR, Adam), SCR with the review trick, A-GEM, LwF, iCaRL, GDumb and EWC++.  A solo run through the driver
-also matches a direct train_learner / evaluate loop from the same random state, so the step generators kept the
-learners' behaviour.  Built with nets.setup_architecture on seeded synthetic uint8 tasks."""
+alone (R = 1, the same (seed, r)): accuracy arrays and final state (agent_cases.final_state: parameters, BN statistics,
+Adam and EWC++ arenas, the memory with DER++'s logits and GEM's rings), for RUN_CASES of agent_cases.CASES: ER (random,
+ASER, MIR, Adam), SCR with the review trick, A-GEM, LwF, iCaRL, GDumb, EWC++, DER++, PCR and GEM.  A solo run through
+the driver also matches a direct train_learner / evaluate loop from the same random state, so the step generators kept
+the learners' behaviour.  Built with nets.setup_architecture on seeded synthetic uint8 tasks."""
 import random
-from types import SimpleNamespace
 
 import numpy as np
 import pytest
 import torch
+
+import agent_cases
 
 pytestmark = pytest.mark.gpu
 
 N_RUNS, R, SEED = 9, 3, 11
 N_TASKS, PER_TASK, N_TEST = 3, 30, 40
 
-CASES = {
-    'er_random': dict(),
-    'er_aser': dict(update='ASER', retrieve='ASER'),
-    'er_mir': dict(retrieve='MIR'),
-    'scr': dict(agent='SCR', trick_on=('review_trick',)),
-    'agem': dict(agent='AGEM'),
-    'lwf': dict(agent='LWF'),
-    'icarl': dict(agent='ICARL', mem_size=100),
-    'gdumb': dict(agent='GDUMB'),
-    'ewc': dict(agent='EWC'),
-    'er_adam': dict(optimizer='Adam', learning_rate=1e-3),
-}
-
-
-def _params(case):
-    over = dict(CASES[case])
-    trick = {k: k in over.pop('trick_on', ()) for k in ('labels_trick', 'kd_trick', 'separated_softmax', 'review_trick',
-                                                         'ncm_trick', 'kd_trick_star')}
-    base = dict(data='cifar10', cuda=True, epoch=1, batch=10, verbose=False, mem_size=20, eps_mem_batch=10,
-                mem_iters=1, update='random', retrieve='random', agent='ER', k=3, aser_type='asvm', n_smp_cls=1.5,
-                num_tasks=N_TASKS, buffer_tracker=False, optimizer='SGD', learning_rate=0.1, weight_decay=0,
-                temp=0.07, head='mlp', subsample=20, error_analysis=False, mem_epoch=2, clip=10.0, lambda_=100.0,
-                alpha=0.9, fisher_update_after=2, test_batch=128, trick=trick)
-    base.update(over)
-    return SimpleNamespace(**base)
+RUN_CASES = ('er_random', 'er_aser', 'er_mir', 'scr_review', 'agem', 'lwf', 'icarl', 'gdumb', 'ewc', 'er_adam', 'derpp',
+             'pcr', 'gem')
 
 
 def _data(r):
@@ -67,25 +46,14 @@ def _maker(params, agents):
     return make
 
 
-def _final(agent):
-    """What must match: the parameter arena, the BN statistics (and counters), the memory."""
-    eng = agent.engine
-    out = [eng.state.params, eng.state.bn_stats, eng.state.bn_tracked]
-    if hasattr(agent, 'buffer'):
-        out += [agent.buffer.buffer_img, agent.buffer.buffer_label]
-    if hasattr(agent, 'memory'):
-        out += [agent.memory.images, agent.memory.labels]
-    return [t.detach().clone() for t in out]
-
-
 def _group(case, n_concurrent, runs):
     from b200ocl import multirun
-    params, agents = _params(case), {}
+    params, agents = agent_cases.params(case), {}
     data = [_data(r) for r in runs]
     acc = multirun.run_group([d[0] for d in data], [d[1] for d in data], _maker(params, agents), n_concurrent,
                              seed=SEED, first_run=runs[0])
     torch.cuda.synchronize()
-    return {r: (a, _final(agents[r])) for r, a in zip(runs, acc)}
+    return {r: (a, agent_cases.final_state(agents[r])) for r, a in zip(runs, acc)}
 
 
 def _same(a, b, what):
@@ -94,7 +62,7 @@ def _same(a, b, what):
         assert torch.equal(x, y), (what, i)
 
 
-@pytest.mark.parametrize('case', sorted(CASES))
+@pytest.mark.parametrize('case', sorted(RUN_CASES))
 def test_concurrent_runs_match_solo_runs_bit_for_bit(case):
     if not torch.cuda.is_available():
         pytest.skip('no CUDA device')
@@ -107,7 +75,7 @@ def test_concurrent_runs_match_solo_runs_bit_for_bit(case):
     assert not np.array_equal(grouped[0][1][0].cpu().numpy(), grouped[1][1][0].cpu().numpy())   # runs differ
 
 
-@pytest.mark.parametrize('case', sorted(CASES))
+@pytest.mark.parametrize('case', sorted(RUN_CASES))
 def test_a_solo_run_matches_a_direct_train_learner_loop(case):
     """The driver at R = 1 against train_learner / evaluate from the same random state on the default stream."""
     if not torch.cuda.is_available():
@@ -117,7 +85,7 @@ def test_a_solo_run_matches_a_direct_train_learner_loop(case):
     via = _group(case, 1, [r])[r]
     memory.flush_pending()
     multirun.RunRng(multirun.run_seed(SEED, r)).swap_in()
-    params, agents = _params(case), {}
+    params, agents = agent_cases.params(case), {}
     agent = _maker(params, agents)(r)
     tasks, loaders = _data(r)
     acc = []
@@ -125,7 +93,7 @@ def test_a_solo_run_matches_a_direct_train_learner_loop(case):
         agent.train_learner(x, y)
         acc.append(agent.evaluate(loaders))
     torch.cuda.synchronize()
-    _same(via, (np.array(acc), _final(agent)), case)
+    _same(via, (np.array(acc), agent_cases.final_state(agent)), case)
 
 
 def test_the_cuda_generator_travels_with_its_run():

@@ -14,25 +14,22 @@ import numpy as np
 import pytest
 import torch
 
+import agent_cases
+
 pytestmark = pytest.mark.gpu
 
 SEED, N_RUNS, N_VAL_RUNS, NUM_VAL = 3, 2, 2, 2
 N_TASKS, PER_TASK, N_TEST, CLS_PER_TASK = 3, 30, 40, 5
 GRID = {'learning_rate': [0.05, 0.1], 'weight_decay': [0.0, 1e-3]}
-CASES = {'er_random': dict(), 'er_aser': dict(update='ASER', retrieve='ASER')}
+TUNE_CASES = ('er_random', 'er_aser')
 
 
 def _params(case):
-    trick = {k: False for k in ('labels_trick', 'kd_trick', 'separated_softmax', 'review_trick', 'ncm_trick',
-                                'kd_trick_star')}
-    base = dict(data='cifar100', cl_type='nc', cuda=True, epoch=1, batch=10, verbose=False, mem_size=20,
-                eps_mem_batch=10, mem_iters=1, update='random', retrieve='random', agent='ER', k=3, aser_type='asvm',
-                n_smp_cls=1.5, num_tasks=N_TASKS, buffer_tracker=False, optimizer='SGD', learning_rate=0.1,
-                weight_decay=0.0, temp=0.07, head='mlp', subsample=20, error_analysis=False, test_batch=128,
-                trick=trick, num_runs=N_RUNS, seed=SEED, num_val=NUM_VAL, num_runs_val=N_VAL_RUNS, online=True,
-                train_val=False, model_name='ER', data_name='cifar100')
-    base.update(CASES[case])
-    return types.SimpleNamespace(**base)
+    """agent_cases.params(case) on CIFAR-100 with the fields of main_tune.py's loop."""
+    p = agent_cases.params(case)
+    vars(p).update(data='cifar100', cl_type='nc', weight_decay=0.0, num_runs=N_RUNS, seed=SEED, num_val=NUM_VAL,
+                   num_runs_val=N_VAL_RUNS, online=True, train_val=False, model_name='ER', data_name='cifar100')
+    return p
 
 
 def _data(r):
@@ -47,13 +44,6 @@ def _data(r):
         loaders.append([(x[:25], torch.from_numpy(labels[np.arange(25) % CLS_PER_TASK])),
                         (x[25:], torch.from_numpy(labels[np.arange(15) % CLS_PER_TASK]))])
     return tasks, loaders
-
-
-def _final(agent):
-    eng = agent.engine
-    out = [eng.state.params, eng.state.bn_stats, eng.state.bn_tracked, agent.buffer.buffer_img,
-           agent.buffer.buffer_label]
-    return [t.detach().clone() for t in out]
 
 
 def _build(params):
@@ -112,7 +102,7 @@ def _stub_reference(records, live):
         def evaluate(self, loaders):
             acc = super().evaluate(loaders)
             self.rec['acc'].append(acc)
-            self.rec['final'] = _final(self)
+            self.rec['final'] = agent_cases.final_state(self)
             return acc
 
     def compute_performance(a):
@@ -159,7 +149,7 @@ def _same(a, b, what):
         assert torch.equal(x, y), (what, i)
 
 
-@pytest.mark.parametrize('case', sorted(CASES))
+@pytest.mark.parametrize('case', sorted(TUNE_CASES))
 def test_tuning_trainings_match_across_R_and_solo_loops(case, monkeypatch, tmp_path):
     if not torch.cuda.is_available():
         pytest.skip('no CUDA device')
@@ -188,7 +178,7 @@ def test_tuning_trainings_match_across_R_and_solo_loops(case, monkeypatch, tmp_p
             agent.train_learner(x, y)
             acc.append(agent.evaluate(loaders[:NUM_VAL]))
         torch.cuda.synchronize()
-        _same(rec1[i], {'acc': acc, 'final': _final(agent)}, (case, r, g, v, 'solo'))
+        _same(rec1[i], {'acc': acc, 'final': agent_cases.final_state(agent)}, (case, r, g, v, 'solo'))
         del agent
 
     # the chosen point: the best mean end accuracy over the repetitions, the earliest on a tie

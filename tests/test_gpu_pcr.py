@@ -13,11 +13,10 @@
   * Whole steps against oracle/pcr.py (fp64) on CIFAR-100, Mini-ImageNet, OpenLORIS and CORe50 with the identity
     transform, and once with the engine's own augmented images; mem_iters = 2, an empty memory, a memory smaller than
     eps_mem_batch, Adam and weight decay.
-  * Two-task runs whose accuracies are the fp64 cosine arg-max of the engine's own features; checkpoint resume
-    (synchronous and asynchronous), R = 2 against R = 1 and B200OCL_GRAPHS=0 against graphs, bit for bit."""
-import os
-import sys
-import textwrap
+  * Two-task runs whose accuracies are the fp64 cosine arg-max of the engine's own features.
+Checkpoint resume, staged snapshots, concurrent runs and graphs against eager launches are checked with the other
+agents, as agent_cases.CASES['pcr'] (test_gpu_checkpoint.py, test_gpu_checkpoint_async.py, test_gpu_multirun.py,
+test_gpu_graphs.py)."""
 from collections import OrderedDict
 from types import SimpleNamespace
 
@@ -25,6 +24,7 @@ import numpy as np
 import pytest
 import torch
 
+from agent_cases import HW, NCLS, _learner, _load
 from oracle import agem as oagem
 from oracle import pcr as opcr
 from oracle import resnet as oresnet
@@ -304,23 +304,6 @@ def make_params(**kw):
     return SimpleNamespace(**base)
 
 
-HW = {'cifar100': 32, 'mini_imagenet': 84, 'core50': 128, 'openloris': 50}
-NCLS = {'cifar100': 100, 'mini_imagenet': 100, 'core50': 50, 'openloris': 69}
-
-
-def _load(agent, p, bn, spec):
-    agent.engine.load(list(p.values()), [(bn[n + '.running_mean'], bn[n + '.running_var']) for n in oresnet.bn_names(spec)])
-
-
-def _learner(b, params, seed, opt=None):
-    spec = oresnet.Spec(HW[params.data], 20, NCLS[params.data])
-    p0, bn0 = oresnet.seeded_state(spec, seed)
-    model = b.nets.setup_architecture(params)
-    agent = b.registry.extra_agents['PCR'](model, opt(model) if opt else None, params)
-    _load(agent, p0, bn0, spec)
-    return agent, spec
-
-
 class _Transform(torch.nn.Module):
     def __init__(self, fn):
         super().__init__()
@@ -351,7 +334,7 @@ def _steps_against_oracle(b, data, n_steps, seed, own_aug=False, adam=False, **k
     params = make_params(data=data, **kw)
     opt = (lambda m: torch.optim.Adam(m.parameters(), lr=params.learning_rate,
                                       weight_decay=params.weight_decay)) if adam else None
-    agent, spec = _learner(b, params, seed, opt=opt)
+    agent, spec = _learner(params, seed, opt=opt)
     if own_aug:
         seen = _recording(agent)
     else:
@@ -440,7 +423,7 @@ def _task(rs, n, labels, hw):
 @pytest.mark.parametrize('data', ['cifar100', 'core50'])
 def test_two_task_run_accuracy_is_the_fp64_cosine_argmax(b, data):
     params = make_params(data=data, mem_size=40)
-    agent, _ = _learner(b, params, 9)
+    agent, _ = _learner(params, 9)
     hw = HW[data]
     rs = np.random.RandomState(3)
     labels = [range(0, 5), range(5, 10)]
@@ -470,106 +453,8 @@ def test_two_task_run_accuracy_is_the_fp64_cosine_argmax(b, data):
 
 
 def test_error_analysis_is_refused_before_anything_launches(b):
-    agent, _ = _learner(b, make_params(error_analysis=True), 9)
+    agent, _ = _learner(make_params(error_analysis=True), 9)
     before = b.native.launch_count()
     with pytest.raises(b.learners.ErrorAnalysisUnsupported):
         agent.evaluate([[(torch.zeros(2, 3, 32, 32), torch.zeros(2, dtype=torch.int64))]])
     assert b.native.launch_count() == before
-
-
-def _run_task_bits(b, graphs):
-    b.engine.set_graphs(graphs)
-    try:
-        params = make_params(mem_size=40)
-        agent, _ = _learner(b, params, 12)
-        rs = np.random.RandomState(6)
-        for t in range(2):
-            np.random.seed(t); torch.manual_seed(t)
-            agent.train_learner(*_task(rs, 60, range(5 * t, 5 * t + 5), 32))
-        torch.cuda.synchronize()
-        eng = agent.engine
-        return [eng.state.params.cpu(), eng.state.bn_stats.cpu(), agent.buffer.buffer_img.cpu(),
-                agent.buffer.buffer_label.cpu()]
-    finally:
-        b.engine.set_graphs(True)
-
-
-def test_graphs_off_gives_the_graphed_bits(b):
-    on, off = _run_task_bits(b, True), _run_task_bits(b, False)
-    for i, (x, y) in enumerate(zip(on, off)):
-        assert torch.equal(x, y), i
-
-
-# ----------------------------------------------------------------------------- experiments (checkpoints, multirun)
-import test_gpu_checkpoint as ck                                                   # noqa: E402
-import test_gpu_multidevice as md                                                  # noqa: E402
-
-
-@pytest.fixture
-def stub_tree(monkeypatch, tmp_path):
-    if not torch.cuda.is_available():
-        pytest.skip('no CUDA device')
-    from b200ocl import checkpoint, multirun
-    ref = tmp_path / 'reference'
-    for rel, src in ck.TREE.items():
-        (ref / rel).parent.mkdir(parents=True, exist_ok=True)
-        (ref / rel).write_text(textwrap.dedent(src))
-    saved = {k: v for k, v in sys.modules.items() if k.split('.')[0] in md.PACKAGES}
-    for k in saved:
-        del sys.modules[k]
-    monkeypatch.syspath_prepend(str(ref))
-    monkeypatch.chdir(tmp_path)
-    for k in (multirun.ENV, multirun.DEVICES_ENV, checkpoint.ENV, checkpoint.ASYNC_ENV, 'CHECKPOINT_FAIL_STEP'):
-        monkeypatch.delenv(k, raising=False)
-    from b200ocl import registry
-    import utils.name_match as nm
-    registry.install(nm, extra=('PCR',))
-    yield tmp_path
-    registry.uninstall(nm)
-    for k in [k for k in sys.modules if k.split('.')[0] in md.PACKAGES]:
-        del sys.modules[k]
-    sys.modules.update(saved)
-
-
-def _experiment(R, name, d, monkeypatch, capsys):
-    from b200ocl import multirun
-    params = ck._params('er_random')
-    vars(params).update(agent='PCR', pcr_temp=0.09)
-    out = os.path.join(os.getcwd(), 'states_' + name)
-    os.makedirs(out, exist_ok=True)
-    monkeypatch.setenv('CHECKPOINT_OUT', out)
-    multirun.multiple_run(params, store=True, save_path=name + '.pkl', n_concurrent=R, checkpoint_dir=d)
-    torch.cuda.synchronize()
-    lines = capsys.readouterr().out.splitlines()
-    import pickle
-    with open('result/cifar10/%s.pkl' % name, 'rb') as f:
-        acc = pickle.load(f)['acc_array']
-    return acc, lines[-1], [torch.load(os.path.join(out, 'run%d.pt' % r)) for r in range(ck.N_RUNS)]
-
-
-@pytest.mark.parametrize('asynchronous', [False, True], ids=['sync', 'async'])
-def test_a_resumed_experiment_matches_an_uninterrupted_one(stub_tree, monkeypatch, capsys, asynchronous):
-    from b200ocl import checkpoint, multirun
-    want = _experiment(1, 'plain', '', monkeypatch, capsys)
-    d = str(stub_tree / 'ck')
-    if asynchronous:
-        monkeypatch.setenv(checkpoint.ASYNC_ENV, '1')
-    on_task = multirun._Repetitions.on_task
-
-    def failing(self, r, t, x, y):
-        if (r, t) == (0, 1):
-            raise ck.Interrupt('run 0, task 1')
-        return on_task(self, r, t, x, y)
-    monkeypatch.setattr(multirun._Repetitions, 'on_task', failing)
-    with pytest.raises(ck.Interrupt):
-        _experiment(1, 'resumed', d, monkeypatch, capsys)
-    monkeypatch.setattr(multirun._Repetitions, 'on_task', on_task)
-    assert sorted(os.listdir(os.path.join(d, 'runs'))) == ['run0.snapshot']
-    got = _experiment(1, 'resumed', d, monkeypatch, capsys)
-    ck._same(got, want, ('PCR', asynchronous))
-
-
-def test_two_runs_at_once_give_one_at_a_times_bits(stub_tree, monkeypatch, capsys):
-    want = _experiment(1, 'one', '', monkeypatch, capsys)
-    got = _experiment(2, 'two', '', monkeypatch, capsys)
-    ck._same(got, want, 'R = 2')
